@@ -1,16 +1,21 @@
 #!/usr/bin/env python
 """bench.py — images/sec of one MobileNetV2-1.0 224x224 training step (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path
   python bench.py --impl reference --gpus N --steps K ...   # the reference's CPU path (port)
   python bench.py --impl torch_gpu --steps K ...            # context: the reference's stock-torch
-                                                            # graph (cuDNN/ATen) on the same B200
+                                                            # graph (cuDNN/ATen) on the same H100
+  python bench.py ... --dump-outputs DIR                    # + what the last timed step computed
 
 A step = forward + label-smoothed CE + backward + gradient all-reduce + RMSprop (with L2 decay,
 EMA, bf16 repack) on one synthetic batch of 256 images per GPU (BASELINE.json configs[1];
 apps/mobilenet/mobilenet_v2_mnas.yml: ReLU, BN momentum 0.01 / eps 1e-3, RMSprop alpha .9 mom .9
 eps 1e-3 inside sqrt, label smoothing .1, wd 1e-5 'mnas', EMA .9999 adjusted to the batch).
-One JSON line on stdout (rank 0).
+One JSON line on stdout (rank 0).  With --dump-outputs DIR, rank 0 also writes what the last timed
+step left to its caller as DIR/<name>.npy (float32): the loss and top-1 / top-5 fractions of the
+step, every parameter of the model after its update (concatenated in named_parameters order) and
+the BatchNorm running statistics.  Inputs and initial weights are seeded, so two builds can be
+compared output for output.
 """
 import argparse
 import json
@@ -32,7 +37,7 @@ MODEL_KW = dict(num_classes=1000, input_channel=32, last_channel=1280, width_mul
 
 # The other BASELINE.json configurations (③ proxyless_mobile, ④ atomnas_c+, ⑤ autonl_l): model
 # keywords as the reference's own yml loader resolves them (tests/golden/model_cfgs.json, written by
-# oracle/make_model_cfgs.py from apps/**/*.yml; /root/reference does not exist on the GPU box).
+# oracle/make_model_cfgs.py from the reference's apps/**/*.yml).
 CONFIGS = {"mobilenet_v2": ("MobileNetV2-1.0", 256), "proxyless_mobile": ("Proxyless-mobile", 256),
            "atomnas_c+": ("AtomNAS-C+ (SE, Swish)", 256), "autonl_l": ("AutoNL-L (non-local)", 128)}
 _PLUGIN = {"models.mobilenet_supernet": "yet_another_mobilenet_series_b200.mobilenet_supernet",
@@ -282,7 +287,7 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    # every requested step is timed (the driver checks steps x ms against its own clock); the CPU
+    # every requested step is timed (steps x ms_per_step is the timed wall time); the CPU
     # step takes ~1-2 s, so the default 20 + 5 steps stay well under a minute
     base, med = cpu_baseline(steps=max(1, args.steps), warmup=max(1, args.warmup))
     base["host_cpu"] = host_cpu()
@@ -342,7 +347,20 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured"
-    return 6650.0, 1400.0, "fallback"
+    return 3350.0, 989.0, "fallback: H100 SXM data sheet (HBM3, dense BF16), not measured"
+
+
+def dump_outputs(out_dir, ts, model):
+    """The last timed step's results as float32 .npy files (< 64 MB for every configuration)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {"loss": ts.loss.reshape(1), "top1": ts.top1.reshape(1), "top5": ts.top5.reshape(1),
+              "params": torch.cat([p.detach().float().flatten() for p in model.parameters()]),
+              "bn_running_stats": torch.cat([b.detach().float().flatten() for b in ts.stat_bufs])}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy().astype(np.float32))
 
 
 def run_ours(args):
@@ -353,7 +371,7 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the sm_100a path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device — the sm_90a path has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -425,6 +443,8 @@ def run_ours(args):
     e2e_ms = float(ms2)
     clocks = sampler.stop() if rank == 0 else None
     loss_end = float(host_loss[args.steps - 1])
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, ts, model)
     # ---- per-kernel profile + CPU baseline (rank 0, N=1) ----
     if rank != 0:
         if world > 1:
@@ -507,7 +527,7 @@ def run_ours(args):
                                % CONFIGS[args.config][0],
                    "per_gpu_batch": B, "global_batch": B * world, "parallelism": "dp%d" % world,
                    "l2_flush": "working set per step (>10 GB of activations at N=256) exceeds the "
-                               "126 MB L2, inputs larger than L2",
+                               "50 MB L2, inputs larger than L2",
                    "cuda_graph": True},
         "clocks": clocks,
         "e2e": {"value": e2e_val, "unit": "img/s", "ms_per_step": e2e_ms / args.steps,
@@ -542,6 +562,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-context", action="store_true",
                     help="skip the stock-PyTorch-on-this-GPU context measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = CONFIGS[args.config][1]

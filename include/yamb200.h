@@ -1,4 +1,4 @@
-/* yamb200 — C ABI of the B200-native inverted-residual training path.
+/* yamb200 — C ABI of the H100-native inverted-residual training path.
  *
  * This is the drop-in boundary of the hot path of meijieru/yet_another_mobilenet_series
  * (SURVEY.md §8b).  The reference's boundary is a Python nn.Module registry
@@ -85,11 +85,11 @@ typedef struct yamb_bn_bwd {
   int32_t use_batch_stats; /* 1: train-mode BN (batch statistics); 0: eval-mode BN => dh = ca*dz */
 } yamb_bn_bwd;
 
-/* ---- pointwise (1x1) convolution = GEMM on tcgen05 tensor cores ----------------------------------
+/* ---- pointwise (1x1) convolution = GEMM on Hopper tensor cores (wgmma) ----------------------------------
  * Replaces nn.Conv2d(k=1) forward, dgrad and wgrad inside the block
  * (reference: models/mobilenet_base.py:391-395 expand, :413 project, :253-257/:284-285 fused).
  *
- *   D[M,N] = A'[M,K] * B'[N,K]^T        fp32 accumulation in TMEM
+ *   D[M,N] = A'[M,K] * B'[N,K]^T        fp32 accumulation in registers
  *
  * a_mn_major = 0: A is a row-major [M][lda] array (K contiguous); 1: a row-major [K][lda] array
  * (M contiguous) — same for B with N.  With pixels on M this covers
@@ -103,7 +103,7 @@ typedef struct yamb_bn_bwd {
  * Epilogues:
  *   epi 0: D bf16 = acc (+ residual), optional per-column BN forward statistics (bn_fwd)
  *   epi 1: D bf16 = acc * act'(h_scale*H + h_shift), statistics sum(dz), sum(dz*xhat) (bn_bwd)
- *   epi 2: D fp32 += acc (atomic; split-K partial sums) */
+ *   epi 2: D fp32 += acc (split-K partial tiles added in slab order: deterministic) */
 typedef struct yamb_gemm {
   int32_t M, N, K;
   int32_t a_mn_major, b_mn_major;
@@ -355,7 +355,7 @@ int yamb_colsum_bf16(const void* X, int64_t M, int32_t C, int64_t ld, float* out
  * single branch, 3x3 depthwise, stride 1 or 2, with the 1x1 expansion or without it (:397-404,
  * hidden == input)) when every BatchNorm uses its running statistics (model.eval(): validation /
  * forward_loss under no_grad, common.py:67-80, train.py:273-309): x tile (TMA, halo zero-filled)
- * -> tcgen05 expand -> BN1+act -> 3x3 stencil -> BN2+act -> tcgen05 project (accumulated over
+ * -> wgmma expand -> BN1+act -> 3x3 stencil -> BN2+act -> wgmma project (accumulated over
  * 64-channel slices of the hidden dimension) -> BN3 (+x) -> y.  The BatchNorm folding
  * scale = gamma*rsqrt(var+eps), shift = beta - mean*scale is done inside the kernel from the
  * module's buffers (csrc/block_eval.cu).  Shapes it does not cover return YAMB_EINVAL; the caller

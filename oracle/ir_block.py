@@ -176,7 +176,7 @@ def forward(x, cfg, P, training=True, quant=False):
     the batch statistics (for the running-stat check)."""
     q = bool(quant)
     # quant="fused": rounding points of the one-launch eval kernel (csrc/block_eval.cu), which keeps
-    # the raw convolution outputs h1 / h2 / h3 in fp32 (TMEM / registers) and rounds only the
+    # the raw convolution outputs h1 / h2 / h3 in fp32 (registers) and rounds only the
     # activations it stages as tensor-core operands and the block output
     qr = quant is True
     S = {}

@@ -1,7 +1,9 @@
 """ORACLE tooling — generates tests/golden/*.pt by running the LIVE reference
 (/root/reference, imported unmodified) on seeded inputs.  Run in the build container only:
 
-    python oracle/make_golden.py
+    python oracle/make_golden.py            # blocks.pt, optim.pt
+    python oracle/make_golden.py --nl       # blocks_nl.pt
+    python oracle/make_golden.py --step     # step.pt
 
 The fixtures travel to the GPU box; /root/reference does not.
 Reference entry points exercised:
@@ -209,8 +211,65 @@ def main():
         print(f, os.path.getsize(os.path.join(OUT, f)), "bytes")
 
 
+# the small network of tests/test_oracle_step_vs_reference.py
+STEP_ROWS = [[1, 16, 1, 1, [3]], [6, 24, 1, 2, [3]], [6, 32, 1, 2, [3, 5]], [3, 40, 1, 2, [5]],
+             [3, 48, 2, 2, [3]]]
+STEP_KW = dict(inverted_residual_setting=STEP_ROWS, active_fn="nn.ReLU", batch_norm_momentum=0.01,
+               batch_norm_epsilon=1e-3, input_size=64, num_classes=10, last_channel=64)
+STEP_BATCH = 8
+
+
+def main_step():
+    """Three reference training steps of a small network (seeded init and batches): the loss of
+    every step, the state after the last step and the EMA shadows (tests/golden/step.pt)."""
+    sys.path.insert(0, REF)
+    warnings.simplefilter("ignore")
+    import models.mobilenet_base as rmb
+    import models.mobilenet_supernet as rsup
+    from utils.rmsprop import RMSprop
+    from utils import optim as roptim
+    torch.manual_seed(1995)
+    ref = rsup.Model(**STEP_KW)
+    ref.apply(rmb.init_weights_mnas)
+    for m in ref.modules():
+        if isinstance(m, torch.nn.Dropout):
+            m.p = 0.0
+    B = STEP_BATCH
+    opt = RMSprop(ref.parameters(), lr=0.016 * B / 256, alpha=0.9, momentum=0.9, eps=1e-3,
+                  eps_inside_sqrt=True, weight_decay=0)
+    crit = roptim.CrossEntropyLabelSmooth(10, 0.1)
+    ema = roptim.ExponentialMovingAverage(0.9999 ** (B / 4096.0))
+    for n, p in ref.named_parameters():
+        ema.register(n, p)
+    for n, b in ref.named_buffers():
+        if "running_var" in n or "running_mean" in n:
+            ema.register(n, b)
+    g = torch.Generator().manual_seed(0)
+    losses = []
+    for step in range(1, 4):
+        x = torch.randn(B, 3, 64, 64, generator=g)
+        t = torch.randint(0, 10, (B,), generator=g)
+        ref.train()
+        opt.zero_grad()
+        loss = crit(ref(x), t).mean() + roptim.cal_l2_loss(ref, 1e-5, "mnas")
+        loss.backward()
+        opt.step()
+        named = dict(ref.named_parameters())
+        named.update(dict(ref.named_buffers()))
+        for n in ema.average_names():
+            ema(n, named[n], step)
+        losses.append(float(loss))
+    rec = {"losses": losses,
+           "state": {k: v.detach().clone() for k, v in ref.state_dict().items()},
+           "ema": {n: ema.average(n).detach().clone() for n in ema.average_names()}}
+    torch.save(rec, os.path.join(OUT, "step.pt"))
+    print("step.pt", os.path.getsize(os.path.join(OUT, "step.pt")), "bytes")
+
+
 if __name__ == "__main__":
     if "--nl" in sys.argv:          # separate process: FLAGS of the reference is a singleton
         main_nl()
+    elif "--step" in sys.argv:
+        main_step()
     else:
         main()

@@ -52,7 +52,7 @@ def as_reference(model):
     ref = copy.deepcopy(model)
     for m in ref.modules():
         if isinstance(m, nn.Sequential) and type(m).forward is not nn.Sequential.forward:
-            # ConvBNReLU of the boundary package routes BatchNorm+activation to the sm_100a
+            # ConvBNReLU of the boundary package routes BatchNorm+activation to the sm_90a
             # kernels on CUDA; the reference's ConvBNReLU (:181-203) is a plain nn.Sequential
             m.forward = types.MethodType(nn.Sequential.forward, m)
         if hasattr(m, "pw_bn") and hasattr(m, "ops"):

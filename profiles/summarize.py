@@ -82,7 +82,7 @@ def step(rnd):
     tot = sum(a["us"] for a in agg.values())
     ours = sum(a["us"] for k, a in agg.items() if not k.startswith("torch:"))
     with open(os.path.join(OUT, rnd + "_step_summary.md"), "w") as f:
-        f.write("# %s — one eager MobileNetV2-1.0 training step under ncu (N=256, B200)\n\n" % rnd)
+        f.write("# %s — one eager MobileNetV2-1.0 training step under ncu (N=256)\n\n" % rnd)
         f.write("`ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum "
                 "--clock-control none` over `tests/gpu_step_once.py` (serialised, cold caches: "
                 "use the SHARES).  %d launches, %.2f ms of kernel time, %.1f %% in this repo's "

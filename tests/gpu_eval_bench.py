@@ -1,4 +1,4 @@
-"""Eval-mode (inference) timing of MobileNetV2-1.0 on one B200: the one-launch blocks
+"""Eval-mode (inference) timing of MobileNetV2-1.0 on one H100: the one-launch blocks
 (csrc/block_eval.cu) against this repo's four-launch sequence and against the reference graph in
 stock PyTorch (fp32 NCHW, autocast-bf16 channels_last).  Driver script (not a pytest test):
 

@@ -1,5 +1,5 @@
 """GPU: BASELINE.json configs built from the reference's real ymls (fixture
-tests/golden/model_cfgs.json) — three iterations of `TrainStep` (sm_100a kernels, CUDA graph from
+tests/golden/model_cfgs.json) — three iterations of `TrainStep` (sm_90a kernels, CUDA graph from
 the 3rd call, flat-arena RMSprop/L2/EMA) against the reference step sequence (train.py:64-114 as
 restated by oracle.torch_model.RefTrainer) running the reference's stock-torch graph on the same
 GPU in fp32 (truth) and under autocast-bf16 (yardstick, SURVEY.md §8c gate ii/iv).

@@ -3,7 +3,7 @@
 Every one of the 17 inverted-residual blocks of MobileNetV2-1.0 (SURVEY.md §8d: 224x224-derived
 spatial sizes 112^2 .. 7^2; reference models/mobilenet_base.py:446-451 built by
 models/mobilenet_supernet.py:132-149 from apps/mobilenet/mobilenet_v2_mnas.yml) runs through the
-sm_100a kernel sequence at N = 32, and blocks 1-3 also at the bench batch N = 256 (M = 3.2 M
+sm_90a kernel sequence at N = 32, and blocks 1-3 also at the bench batch N = 256 (M = 3.2 M
 pixels, split-K wgrad over K = 3.2 M), against
 
   truth      the reference's stock-torch graph of the same block in fp32 on the same GPU

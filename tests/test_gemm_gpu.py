@@ -1,4 +1,4 @@
-"""GPU parity of yamb_pointwise_gemm (tcgen05 GEMM) against plain torch fp32 math of the same op:
+"""GPU parity of yamb_pointwise_gemm (wgmma GEMM) against plain torch fp32 math of the same op:
 forward / dgrad / wgrad orientations, operand transforms, BN-statistics and dz epilogues."""
 import pytest
 

@@ -1,4 +1,4 @@
-"""GPU: the whole MobileNetV2 through the sm_100a path vs the plain-torch port of the reference
+"""GPU: the whole MobileNetV2 through the sm_90a path vs the plain-torch port of the reference
 graph (oracle/torch_model.py, fp32 on CPU), and TrainStep (CUDA graph, flat-arena optimizer)
 vs the reference step sequence."""
 import copy
@@ -161,9 +161,8 @@ def test_graph_replay_equals_eager(built_lib):
     """The SAME iteration (same state, same batch) run eagerly TWICE and once as a CUDA-graph
     replay.  Everything that crosses warps or CTAs in the BatchNorm statistics is accumulated in
     double (csrc/bn_finalize.cuh), so the forward pass and every activation gradient are the same
-    bits run after run; the only order-dependent sums left are the fp32 split-K / depthwise
-    weight-gradient reductions (1e-7 relative).  Measured on B200: identical losses, parameter
-    update 4e-7 rel-L2 between two eager runs and between eager and replay.  (With fp32 statistics
+    bits run after run; the weight-gradient reductions (split-K GEMM, depthwise, stem, classifier
+    bias) add per-CTA partials in a fixed order (csrc/det_reduce.cu).  (With fp32 statistics
     atomics, round 1, two eager runs differed by 1.6e-3 in the loss and 0.2 in the update: bf16
     rounding flips amplified the last-bit differences of the BatchNorm coefficients.)"""
     from yet_another_mobilenet_series_b200.trainer import TrainStep
@@ -199,6 +198,17 @@ def test_graph_replay_equals_eager(built_lib):
     assert abs(loss_e2 - loss_e) <= 1e-6 * abs(loss_e)
     assert abs(loss_g - loss_e) <= 1e-6 * abs(loss_e)
     assert noise < 1e-4 and diff < 1e-4
+    # the weight-gradient reductions add their partials in a fixed order: the same bits every time
+    assert torch.equal(p_e2, p_e) and torch.equal(p_g, p_e)
+    # a larger eager step in between (bigger reduction scratch) must not disturb the captured graph
+    big = _model(128).cuda()
+    ts_big = TrainStep(big, 2 * B, image_size=128, use_graph=False)
+    xb = torch.randn(2 * B, 3, 128, 128, generator=g).to(torch.bfloat16)
+    ts_big(xb, torch.randint(0, 100, (2 * B,), generator=g))
+    torch.cuda.synchronize()
+    _restore(ts, m, st)
+    assert float(ts(x, t)) == loss_g              # replay of the graph captured above
+    assert torch.equal(ts.opt.arenas()["p"], p_g)
     # replaying again advances the training (the graph is not a frozen snapshot)
     loss_next = float(ts(x, t))
     assert loss_next < loss_g

@@ -1,70 +1,40 @@
-"""CPU, build container only: pin oracle/torch_model.py (the CPU-baseline port of the whole
-training step) against the LIVE reference classes.  Skipped where /root/reference is absent."""
+"""CPU: pin oracle/torch_model.py (the CPU-baseline port of the whole training step) against three
+training steps of the reference classes, recorded in tests/golden/step.pt
+(oracle/make_golden.py --step): the loss of every step, the final state and the EMA shadows."""
 import os
-import sys
 import warnings
 
-import pytest
 import torch
 
-REF = os.environ.get("YAMB_REFERENCE", "/root/reference")
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "models")),
-                                reason="reference tree not present (GPU box)")
-
-ROWS = [[1, 16, 1, 1, [3]], [6, 24, 1, 2, [3]], [6, 32, 1, 2, [3, 5]], [3, 40, 1, 2, [5]],
-        [3, 48, 2, 2, [3]]]
-KW = dict(inverted_residual_setting=ROWS, active_fn="nn.ReLU", batch_norm_momentum=0.01,
-          batch_norm_epsilon=1e-3, input_size=64, num_classes=10, last_channel=64)
+from oracle.make_golden import STEP_BATCH, STEP_KW
 
 
-def test_port_step_equals_reference_step():
-    sys.path.insert(0, REF)
+def test_port_step_equals_reference_step(golden_dir):
     warnings.simplefilter("ignore")
-    import models.mobilenet_base as rmb
-    import models.mobilenet_supernet as rsup
-    from utils.rmsprop import RMSprop
-    from utils import optim as roptim
     from yet_another_mobilenet_series_b200 import mobilenet_base as mb, mobilenet_supernet as sup
     from oracle import torch_model as tm
 
+    rec = torch.load(os.path.join(golden_dir, "step.pt"), weights_only=False)
     torch.manual_seed(1995)
-    ref = rsup.Model(**KW)
-    ref.apply(rmb.init_weights_mnas)
-    torch.manual_seed(1995)
-    ours = sup.Model(**KW)
+    ours = sup.Model(**STEP_KW)
     ours.apply(mb.init_weights_mnas)
     port = tm.as_reference(ours)
-    for m in list(ref.modules()) + list(port.modules()):
+    for m in port.modules():
         if isinstance(m, torch.nn.Dropout):
             m.p = 0.0
-    B = 8
+    B = STEP_BATCH
     trainer = tm.RefTrainer(port, B)
-    opt = RMSprop(ref.parameters(), lr=0.016 * B / 256, alpha=0.9, momentum=0.9, eps=1e-3,
-                  eps_inside_sqrt=True, weight_decay=0)
-    crit = roptim.CrossEntropyLabelSmooth(10, 0.1)
-    ema = roptim.ExponentialMovingAverage(0.9999 ** (B / 4096.0))
-    for n, p in ref.named_parameters():
-        ema.register(n, p)
-    for n, b in ref.named_buffers():
-        if "running_var" in n or "running_mean" in n:
-            ema.register(n, b)
     g = torch.Generator().manual_seed(0)
     for step in range(1, 4):
         x = torch.randn(B, 3, 64, 64, generator=g)
         t = torch.randint(0, 10, (B,), generator=g)
-        ref.train()
-        opt.zero_grad()
-        loss = crit(ref(x), t).mean() + roptim.cal_l2_loss(ref, 1e-5, "mnas")
-        loss.backward()
-        opt.step()
-        named = dict(ref.named_parameters())
-        named.update(dict(ref.named_buffers()))
-        for n in ema.average_names():
-            ema(n, named[n], step)
         lp = trainer.step(x, t)
-        assert abs(lp - float(loss)) < 1e-5 * max(1.0, abs(float(loss)))
-    sa, sb = ref.state_dict(), port.state_dict()
+        loss = rec["losses"][step - 1]
+        assert abs(lp - loss) < 1e-5 * max(1.0, abs(loss))
+    sa, sb = rec["state"], port.state_dict()
+    assert set(sa) == set(sb)
     for k in sa:
         assert torch.allclose(sa[k].float(), sb[k].float(), rtol=1e-5, atol=1e-6), k
-    for n in ema.average_names():
-        assert torch.allclose(ema.average(n), trainer.ema.shadow[n], rtol=1e-5, atol=1e-6), n
+    assert set(rec["ema"]) == set(trainer.ema.shadow)
+    for n, v in rec["ema"].items():
+        assert torch.allclose(v, trainer.ema.shadow[n], rtol=1e-5, atol=1e-6), n

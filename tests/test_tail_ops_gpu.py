@@ -1,5 +1,5 @@
-"""GPU parity of the layers around the block stack on the sm_100a path (tail_ops.py): stem 3x3/s2
-convolution, head 1x1 ConvBNReLU and classifier through the tcgen05 GEMM, label-smoothed softmax
+"""GPU parity of the layers around the block stack on the sm_90a path (tail_ops.py): stem 3x3/s2
+convolution, head 1x1 ConvBNReLU and classifier through the wgmma GEMM, label-smoothed softmax
 cross entropy with top-k.  Truth = the reference's stock-torch modules / formulas in fp32 on the
 same bf16-rounded inputs (reference models/mobilenet_supernet.py:124-130, :152-167,
 models/mobilenet_base.py:181-203, utils/optim.py:150-158, common.py:73-79)."""

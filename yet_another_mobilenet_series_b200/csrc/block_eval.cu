@@ -1,4 +1,4 @@
-// Eval-mode inverted-residual block in ONE launch, no intermediate tensor in HBM (sm_100a).
+// Eval-mode inverted-residual block in ONE launch, no intermediate tensor in HBM (sm_90a).
 //
 // Replaces, behind yamb_block_eval_fwd (include/yamb200.h), the whole forward of
 // InvertedResidualChannels (reference models/mobilenet_base.py:446-451: 1x1 expand -> BatchNorm ->
@@ -7,29 +7,33 @@
 // under torch.no_grad()).  With the statistics known up front the block is a pure function of an
 // input tile plus a one-pixel halo: SURVEY.md §7.1 step 2 / §7.2, BASELINE.json's "fused block".
 //
-// Persistent CTAs (two per SM where shared memory and TMEM allow) walk output tiles of <= 112
-// pixels (k = 3, stride 1: 7x16, 7x14 or two 7x7 images; stride 2 and k = 5 / 7: smaller tiles whose
-// input tile with its halo still fits the 256 rows of two MMA tiles).  Per tile:
+// Persistent CTAs (one per SM) walk output tiles of <= 112 pixels (k = 3, stride 1: 7x16, 7x14 or
+// two 7x7 images; stride 2, k = 5 / 7 and wide outputs: smaller tiles) whose input tile with its
+// halo fits 256 rows.  Per tile:
 //   x tile (+halo, <= 256 pixels) --TMA 4-D box, zero fill outside the image--> smem (A operand)
 //   for every 64-channel slice of the hidden dimension:
-//     W1 slice, W3 slice --TMA--> smem
-//     tcgen05.mma  [256 px x Cin] x [Cin x 64]       -> TMEM (fp32)                   expand
-//     tcgen05.ld -> BatchNorm1 + act -> bf16, zero outside the image -> smem          epilogue 1
-//     kxk stencil on the CUDA cores (FFMA2) -> BatchNorm2 + act -> bf16 -> smem (A operand layout)
-//     tcgen05.mma  [128 px x 64] x [64 x Cout]  accumulated over the slices -> TMEM   project
-//   tcgen05.ld -> BatchNorm3 (+ x) -> bf16 -> global                                  epilogue 2
+//     W1 slice --TMA--> smem
+//     wgmma  [64 px x Cin] x [Cin x 64] per 64-pixel chunk -> registers (fp32)        expand
+//     BatchNorm1 + act -> bf16, zero outside the image -> smem                         epilogue 1
+//     kxk stencil on the CUDA cores -> BatchNorm2 + act -> bf16 -> smem (A operand layout)
+//     W3 slice --TMA--> smem
+//     wgmma  [64 px x 64] x [64 x 16 j]  accumulated over the slices -> registers      project
+//   BatchNorm3 (+ x) -> bf16 -> global                                                 epilogue 2
 // Blocks without the 1x1 expansion (hidden == input) skip the first MMA: the x panel itself is the
 // stencil input.
 // HBM traffic: x once (+ halo re-reads from L2), y once; the hidden tensors (6 x the block's
 // input) never leave the SM.  BatchNorm folding (gamma * rsqrt(var + eps), beta - mean * scale) is
 // done by the kernel from the module's own buffers: no preparation launches.
 //
-// Roles: 8 warps; all of them run the two epilogues, warps 0-6 run the stencil (runs of 7 or 8
-// consecutive outputs of a row x 16 or 32 channel groups), and while they do, ONE thread of warp 7 drives the machine: TMA
-// loads of the next operands, tcgen05.mma of the next slice's expand and of this slice's project.
-// Every staging buffer is single and refilled right after its last reader retired:
-//   wait expand(gc) | TMA W1(gc+1) [+ x of the next tile] | epilogue 1 | S2 | TMA W3(gc),
-//   expand(gc+1) || stencil -> a2 | S3 | project(gc) | (last slice of a tile: epilogue 2)
+// Roles: 8 warps = two warpgroups.  Each warpgroup runs the expand MMAs and epilogue 1 of its
+// 64-pixel chunks (chunks wg, wg + 2), and the project MMAs of its share of the output: the rows
+// 64 wg.. of all columns when the tile has more than 64 pixels (Cout <= 160), else all rows of half
+// of the 16-column groups — at most 80 fp32 accumulators per thread.  Warps 0-6 run the stencil
+// (runs of 7 or 8 consecutive outputs of a row x 16 or 32 channel groups); one thread of warp 7
+// issues the TMA loads.  Every staging buffer is single and refilled right after its last reader
+// retired:
+//   wait W1(c) | expand(c) -> epilogue 1 (the MMAs of project(c-1) retire here too) | S2 |
+//   TMA W3(c), W1(c+1) [+ x of the next tile] || stencil -> a2 | S3 | project(c) (left in flight)
 //
 // Rounding points: a1 = bf16(act(bn1(fp32 accumulator))), a2 = bf16(act(bn2(fp32 stencil))),
 // y = bf16(bn3(fp32 accumulator) + x) — one rounding fewer per stage than the four-launch path
@@ -62,19 +66,20 @@ struct BlockEvalDev {
   int tiles_h, tiles_w, num_tiles;
   int KB;            // 64-channel panels of the x tile / the W1 slice
   int nks;           // K steps (16 channels) of the expand MMA
-  int Npad;          // Cout rounded up to a multiple of 16 (UMMA N)
+  int Npad;          // Cout rounded up to a multiple of 16 (project MMAs of 16 columns)
   int NC;            // 64-channel slices of the hidden dimension
   int xpanel_bytes;  // bytes between the 64-channel panels of the x tile
   int off_w1, off_w3, off_h1, off_h2, off_tab, off_c3, off_bars;
-  int tmem_cols, proj_col;
 };
+
+constexpr int kMaxProjChunks = 10;   // 16-column project accumulators per thread (80 registers)
 
 constexpr int kH1Pitch = 144;    // bytes per pixel of the a1 tile: 64 bf16 + 16 (conflict-free, no swizzle)
 // one set of per-slice tables: s1 t1 s2 t2 [64] + taps [K*K][64]
 __host__ __device__ constexpr int tab_floats(int k) { return 256 + k * k * 64; }
 
-// Output tile TI images x TOH x TOW pixels (<= 128 = the M of the project MMA); the input tile with
-// its one-pixel halo is the M of the expand MMAs (2 tiles of 128 rows, rows >= NPI are don't-care).
+// Output tile TI images x TOH x TOW pixels (<= 128: one or two 64-row project MMAs); the input tile
+// with its halo is the M of the expand MMAs (NCH chunks of 64 rows, rows >= NPI are don't-care).
 // Stencil threads (warps 0-6 = 224 threads): a thread owns CPT channels (64 / CPT channel groups)
 // and RUN consecutive outputs of one output row.
 template <int K_, int S_, int TOH_, int TOW_, int TI_, int CPT_>
@@ -87,24 +92,25 @@ struct EvGeom {
   static constexpr int RUN = (TOW % 8 == 0) ? 8 : 7;   // consecutive outputs of one row per stencil thread
   static constexpr int NRUN = NPO / RUN;
   static constexpr int NCG = 64 / CPT;                  // channel groups
-  static_assert(NPO <= 128 && NPI > 128 && NPI <= 256 && TOW % RUN == 0 && NRUN * NCG <= 224,
+  static constexpr int NCH = (NPI + 63) / 64;           // 64-row chunks of the expand MMAs
+  static constexpr int PM = NPO > 64 ? 2 : 1;           // 64-row halves of the project MMAs
+  static_assert(NPO <= 128 && NPI <= 256 && TOW % RUN == 0 && NRUN * NCG <= 224,
                 "tile geometry (warp 7 must stay free of stencil work)");
 };
 
 template <class G, bool EXPAND, bool LEAN>
-__global__ void __launch_bounds__(256, 2)
+__global__ void __launch_bounds__(256, 1)
 block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW1,
                   const __grid_constant__ CUtensorMap tmW3, const __grid_constant__ BlockEvalDev p) {
   constexpr int K = G::K, P = G::P, kTabFloats = tab_floats(G::K);
   constexpr int S = G::S, TOH = G::TOH, TOW = G::TOW, TI = G::TI, IH = G::IH, IW = G::IW;
   constexpr int NPI = G::NPI, NPO = G::NPO, RUN = G::RUN, NRUN = G::NRUN, CPT = G::CPT, NCG = G::NCG;
+  constexpr int NCH = G::NCH, PM = G::PM;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint64_t* bar_e = reinterpret_cast<uint64_t*>(smem + p.off_bars);   // expand MMAs of a slice retired
-  uint64_t* bar_p = bar_e + 1;                                         // project MMAs of a slice retired
-  uint64_t* bar_ld = bar_e + 2;                                        // TMA: W1 slice (+ x tile) landed
-  uint64_t* bar_w3 = bar_e + 3;                                        // TMA: W3 slice landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_e + 4);
+  const int wg = warp >> 2, q = warp & 3;                              // warpgroup, warp inside it
+  uint64_t* bar_ld = reinterpret_cast<uint64_t*>(smem + p.off_bars);  // TMA: W1 slice (+ x tile) landed
+  uint64_t* bar_w3 = bar_ld + 1;                                       // TMA: W3 slice landed
   float* c3 = reinterpret_cast<float*>(smem + p.off_c3);     // [scale3 | shift3] x Npad
   float* tab = reinterpret_cast<float*>(smem + p.off_tab);   // two sets of kTabFloats
   uint8_t* sH1 = smem + p.off_h1;
@@ -113,15 +119,9 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
                  sW3_u = sX_u + (uint32_t)p.off_w3, sH2_u = smem_u32(sH2);
 
   if (tid == 0) {
-    mbar_init(bar_e, 1);
-    mbar_init(bar_p, 1);
     mbar_init(bar_ld, 1);
     mbar_init(bar_w3, 1);
     fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    tmem_relinquish();
   }
   for (int i = tid; i < p.Npad; i += 256) {
     float sc = 0.f, sh = 0.f;
@@ -142,10 +142,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     tma_prefetch_desc(&tmW3);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const ActParam ap = make_act(p.act);
   constexpr bool lean = LEAN;       // relu / relu6 / none: clamp the packed bf16 pair
   const uint32_t lo2 = pack_bf16(ap.lo, ap.lo), hi2 = pack_bf16(ap.hi, ap.hi);
@@ -187,12 +184,8 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     asm volatile("cp.async.wait_group 0;" ::: "memory");   // this thread's taps have landed
   };
 
-  // ---- the control thread: TMA + tcgen05.mma ----------------------------------------------------
-  const uint64_t ad_x = umma_smem_desc(sX_u, 16, 1024), bd_w1 = umma_smem_desc(sW1_u, 16, 1024);
-  const uint64_t ad_h2 = umma_smem_desc(sH2_u, 16, 1024), bd_w3 = umma_smem_desc(sW3_u, 16, 1024);
-  const uint32_t idesc_e = umma_idesc_bf16(128, 64, 0, 0);
+  // ---- TMA (control thread) ------------------------------------------------------------------------
   const int p_halves = p.Npad > 256 ? 2 : 1, p_nn = p.Npad / p_halves;
-  const uint32_t idesc_p = umma_idesc_bf16(128, p_nn, 0, 0);
   uint32_t ld_par = 0, w3_par = 0;
   auto tma_x = [&](int t) {            // x tile of tile t: one 4-D box per 64-channel panel
     const int tx = t % p.tiles_w, ty = (t / p.tiles_w) % p.tiles_h, g = t / (p.tiles_w * p.tiles_h);
@@ -204,137 +197,91 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     for (int kb = 0; kb < p.KB; ++kb)
       tma_load_2d(&tmW1, bar_ld, smem + p.off_w1 + kb * 8192, kb * 64, c * 64);
   };
-  auto issue_expand = [&]() {          // [2 x 128 pixels, Cin] x [Cin, 64] -> TMEM columns [0, 128)
-    tc_fence_after();
-#pragma unroll 1
-    for (int mt = 0; mt < 2; ++mt)
-#pragma unroll 1
-      for (int ks = 0; ks < p.nks; ++ks) {
-        const int kb = ks >> 2, kk = ks & 3;
-        umma_bf16(tmem + (uint32_t)(mt * 64),
-                  ad_x + (uint64_t)((kb * p.xpanel_bytes + mt * 16384 + kk * 32) >> 4),
-                  bd_w1 + (uint64_t)((kb * 8192 + kk * 32) >> 4), idesc_e, ks > 0 ? 1u : 0u);
-      }
-    umma_commit(bar_e);
-  };
 
-  uint32_t pe = 0, pp = 0;          // parities of bar_e / bar_p (every thread follows them)
-  int p_waited = 0;                 // project commits waited for (whole kernel)
-  auto wait_projects = [&](int upto) {
-    while (p_waited < upto) {
-      mbar_wait(bar_p, pp);
-      pp ^= 1;
-      ++p_waited;
-    }
-  };
+  // ---- project MMAs of this warpgroup: rows p_row0.., 16-column groups [p_j0, p_j0 + p_nj) ----
+  const int NJ = p.Npad >> 4;
+  const int p_row0 = PM == 2 ? 64 * wg : 0;
+  const int p_jh = PM == 2 ? NJ : (NJ + 1) / 2;
+  const int p_j0 = PM == 2 ? 0 : wg * p_jh;
+  const int p_nj = min(p_jh, NJ - p_j0);
+  float pacc[kMaxProjChunks][8];
 
   // ---- per-thread geometry (the same in every tile) ------------------------------------------------
-  // epilogue 1: this thread's pixel row of the input tile (warps 0-3: rows 0..127, 4-7: 128..255)
-  const int e1_r = (warp >> 2) * 128 + (warp & 3) * 32 + lane;
-  const int e1_ti = e1_r / (IH * IW);
-  const int e1_dy = (e1_r % (IH * IW)) / IW - P, e1_dx = (e1_r % (IH * IW)) % IW - P;
-  // stencil: RUN consecutive outputs of one row x 4 channels
+  // stencil: RUN consecutive outputs of one row x CPT channels
   const int cg = tid % NCG, sp = tid / NCG;
   const int r0 = sp * RUN;
   const int s_ti = r0 / (TOH * TOW), s_oy = (r0 % (TOH * TOW)) / TOW, s_ox0 = (r0 % (TOH * TOW)) % TOW;
   const uint8_t* s_hb = sH1 + (s_ti * IH * IW + s_oy * S * IW + s_ox0 * S) * kH1Pitch + cg * CPT * 2;
-  // epilogue 2: this thread's output pixel
-  const int e2_r = (warp & 3) * 32 + lane;
-  const int e2_ti = e2_r / (TOH * TOW);
-  const int e2_oy = (e2_r % (TOH * TOW)) / TOW, e2_ox = (e2_r % (TOH * TOW)) % TOW;
 
   const int NC = p.NC;
   int t = blockIdx.x;
   tab_fetch(0, tab);
   tab_store(tab);
-  if (control) {
+  if (control && t < p.num_tiles) {
     mbar_arrive_expect_tx(bar_ld, (uint32_t)(p.KB * (NPI * 128 + (EXPAND ? 8192 : 0))));
     tma_x(t);
-    if (EXPAND) {
-      tma_w1(0);
-      mbar_wait(bar_ld, ld_par);
-      ld_par ^= 1;
-      issue_expand();
-    }
+    if (EXPAND) tma_w1(0);
   }
   __syncthreads();   // tables of slice 0
   int gc = 0;
   for (; t < p.num_tiles; t += gridDim.x) {
     const int tx = t % p.tiles_w, ty = (t / p.tiles_w) % p.tiles_h, g = t / (p.tiles_w * p.tiles_h);
     const bool more_tiles = t + (int)gridDim.x < p.num_tiles;
-    bool e1_inside;
-    {
-      const int n = g * TI + e1_ti, yy = ty * TOH * S + e1_dy, xx = tx * TOW * S + e1_dx;
-      e1_inside = e1_r < NPI && n < p.N && (unsigned)yy < (unsigned)p.H && (unsigned)xx < (unsigned)p.W;
-      // zero padding of the depthwise input: this thread's row of the a1 tile, once per tile (the
-      // previous tile's stencil reads are behind its last S3, this tile's first are behind S2)
-      if (EXPAND && !e1_inside && e1_r < NPI) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<uint4*>(sH1 + e1_r * kH1Pitch + j * 16) = make_uint4(0u, 0u, 0u, 0u);
-      }
-    }
+    for (int j = 0; j < kMaxProjChunks; ++j)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) pacc[j][i] = 0.f;
     for (int c = 0; c < NC; ++c, ++gc) {
       const bool last_c = c + 1 == NC;
       const bool has_next = !last_c || more_tiles;
       const float* tb = tab + (gc & 1) * kTabFloats;
       if (EXPAND) {
-        mbar_wait(bar_e, pe);           // expand(gc) retired: accumulator ready, sW1 (and sX) free
-        pe ^= 1;
-        tc_fence_after();
-        if (has_next) {
-          if (control) {
-            mbar_arrive_expect_tx(bar_ld, (uint32_t)(p.KB * (8192 + (last_c ? NPI * 128 : 0))));
-            if (last_c) tma_x(t + gridDim.x);
-            tma_w1(last_c ? 0 : c + 1);
+        mbar_wait(bar_ld, ld_par);      // W1(c) (and the x tile) landed
+        ld_par ^= 1;
+#pragma unroll
+        for (int mi = 0; mi < (NCH + 1) / 2; ++mi) {
+          const int m = wg + 2 * mi;     // 64-pixel chunk of the input tile
+          if (m >= NCH) break;
+          float e[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) e[i] = 0.f;
+          reg_fence(e);
+          wgmma_fence();
+#pragma unroll 1
+          for (int ks = 0; ks < p.nks; ++ks) {
+            const int kb = ks >> 2, kk = ks & 3;
+            wgmma_m64n64<0, 0>(e, gmma_smem_desc(sX_u + (uint32_t)(kb * p.xpanel_bytes + m * 8192 + kk * 32), 16, 1024),
+                               gmma_smem_desc(sW1_u + (uint32_t)(kb * 8192 + kk * 32), 16, 1024), 1u);
           }
-          tab_fetch(last_c ? 0 : c + 1, tab + ((gc + 1) & 1) * kTabFloats);   // published before S3
-        }
-        __syncwarp();                   // warp 7 reconverges before the warp-wide tcgen05.ld
-        // ---- epilogue 1: a1 = bf16(act(bn1(h1))), zero outside the image, -> sH1[pixel][64] ----
-        const uint32_t taddr = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * 64);
-        uint8_t* dst = sH1 + e1_r * kH1Pitch;
+          wgmma_commit();
+          wgmma_wait<0>();               // (the previous slice's project MMAs retire here too)
+          reg_fence(e);
+          // ---- epilogue 1: a1 = bf16(act(bn1(h1))), zero outside the image, -> sH1[pixel][64] ----
 #pragma unroll
-        for (int hcol = 0; hcol < 2; ++hcol) {
-          uint32_t acc[32];
-          tmem_ld_32x32(taddr + (uint32_t)(hcol * 32), acc);
-          tmem_ld_wait();
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = m * 64 + q * 16 + (lane >> 2) + 8 * hh;
+            if (r >= NPI) continue;
+            const int ti = r / (IH * IW);
+            const int dy = (r % (IH * IW)) / IW - P, dx = (r % (IH * IW)) % IW - P;
+            const int n = g * TI + ti, yy = ty * TOH * S + dy, xx = tx * TOW * S + dx;
+            const bool inside = n < p.N && (unsigned)yy < (unsigned)p.H && (unsigned)xx < (unsigned)p.W;
+            uint8_t* dst = sH1 + r * kH1Pitch + (lane & 3) * 4;
 #pragma unroll
-          for (int ch = 0; ch < 4; ++ch) {
-            const int cb = hcol * 32 + ch * 8;
-            const float4 s0 = *reinterpret_cast<const float4*>(tb + cb);
-            const float4 s1 = *reinterpret_cast<const float4*>(tb + cb + 4);
-            const float4 t0 = *reinterpret_cast<const float4*>(tb + 64 + cb);
-            const float4 t1 = *reinterpret_cast<const float4*>(tb + 64 + cb + 4);
-            const float2 ss[4] = {make_float2(s0.x, s0.y), make_float2(s0.z, s0.w),
-                                  make_float2(s1.x, s1.y), make_float2(s1.z, s1.w)};
-            const float2 tt[4] = {make_float2(t0.x, t0.y), make_float2(t0.z, t0.w),
-                                  make_float2(t1.x, t1.y), make_float2(t1.z, t1.w)};
-            uint32_t ow[4];
-            if (lean) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 v = ffma2(ss[e], make_float2(__uint_as_float(acc[ch * 8 + 2 * e]),
-                                                          __uint_as_float(acc[ch * 8 + 2 * e + 1])),
-                                       tt[e]);
-                ow[e] = clamp_bf16x2(pack_bf16(v.x, v.y), lo2, hi2);
+            for (int j = 0; j < 8; ++j) {
+              const int col = j * 8 + 2 * (lane & 3);
+              const float2 ss = *reinterpret_cast<const float2*>(tb + col);
+              const float2 tt = *reinterpret_cast<const float2*>(tb + 64 + col);
+              const float2 v = ffma2(ss, make_float2(e[4 * j + 2 * hh], e[4 * j + 2 * hh + 1]), tt);
+              uint32_t o;
+              if (lean) {
+                o = clamp_bf16x2(pack_bf16(v.x, v.y), lo2, hi2);
+              } else {
+                float a2[2] = {v.x, v.y};
+                act_vec<2>(a2, ap);
+                o = pack_bf16(a2[0], a2[1]);
               }
-            } else {
-              float v[8];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 w = ffma2(ss[e], make_float2(__uint_as_float(acc[ch * 8 + 2 * e]),
-                                                          __uint_as_float(acc[ch * 8 + 2 * e + 1])),
-                                       tt[e]);
-                v[2 * e] = w.x;
-                v[2 * e + 1] = w.y;
-              }
-              act_vec<8>(v, ap);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) ow[e] = pack_bf16(v[2 * e], v[2 * e + 1]);
+              *reinterpret_cast<uint32_t*>(dst + j * 16) = inside ? o : 0u;
             }
-            // rows outside the image were zeroed at the start of the tile and stay zero
-            if (e1_inside) *reinterpret_cast<uint4*>(dst + cb * 2) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
           }
         }
       } else {
@@ -345,7 +292,6 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           mbar_wait(bar_ld, ld_par);    // every thread follows this barrier in the no-expand variant
           ld_par ^= 1;
         }
-        if (has_next) tab_fetch(last_c ? 0 : c + 1, tab + ((gc + 1) & 1) * kTabFloats);
         if (tid < NPI) {
           const uint8_t* src = smem + c * p.xpanel_bytes + tid * 128;
           uint8_t* dst = sH1 + tid * kH1Pitch;
@@ -354,23 +300,22 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             *reinterpret_cast<uint4*>(dst + j * 16) =
                 *reinterpret_cast<const uint4*>(src + ((j ^ (tid & 7)) << 4));
         }
+        wgmma_wait<0>();                 // project(c-1) retired: sW3 and sH2 are free after S2
       }
-      // project(gc-1) retired long ago (it was issued before this slice's accumulator wait):
-      // sW3 and sH2 are free
-      wait_projects(gc);
-      tc_fence_before();
+      reg_fence(pacc);
       __syncthreads();                                                     // S2: a1 tile complete
+      if (has_next) tab_fetch(last_c ? 0 : c + 1, tab + ((gc + 1) & 1) * kTabFloats);
       if (warp == 7) {
-        // ---- control: W3 slice in, the next slice's expand out (under the stencil) ----
+        // ---- control: W3 slice in; the next slice's W1 (and the next tile's x) in ----
         if (lane == 0) {
           mbar_arrive_expect_tx(bar_w3, (uint32_t)(p.Npad * 128));
           for (int h = 0; h < p_halves; ++h)
             tma_load_2d(&tmW3, bar_w3, smem + p.off_w3 + h * p_nn * 128, c * 64, h * p_nn);
           if (EXPAND) {
             if (has_next) {
-              mbar_wait(bar_ld, ld_par);     // landed during epilogue 1
-              ld_par ^= 1;
-              issue_expand();
+              mbar_arrive_expect_tx(bar_ld, (uint32_t)(p.KB * (8192 + (last_c ? NPI * 128 : 0))));
+              if (last_c) tma_x(t + gridDim.x);
+              tma_w1(last_c ? 0 : c + 1);
             }
           } else if (last_c && more_tiles) {
             // every panel of this tile has been copied out: the next tile's x may land
@@ -382,7 +327,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       } else if (sp < NRUN) {
         // ---- KxK stencil: RUN consecutive outputs of one row x CPT channels per thread; the taps
         //      of one kernel row at a time in registers ----
-        constexpr int NV = CPT / 2;          // packed fp32 pairs per pixel
+        constexpr int NV = CPT / 2;          // fp32 pairs per pixel
         float2 o2[RUN][NV];
 #pragma unroll
         for (int j = 0; j < RUN; ++j)
@@ -439,9 +384,9 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             if (lean) {
               wv[v] = clamp_bf16x2(pack_bf16(z.x, z.y), lo2, hi2);
             } else {
-              float q[2] = {z.x, z.y};
-              act_vec<2>(q, ap);
-              wv[v] = pack_bf16(q[0], q[1]);
+              float qq[2] = {z.x, z.y};
+              act_vec<2>(qq, ap);
+              wv[v] = pack_bf16(qq[0], qq[1]);
             }
           }
           const int r = r0 + j;
@@ -453,67 +398,49 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       if (has_next) tab_store(tab + ((gc + 1) & 1) * kTabFloats);   // its readers are behind S3
       fence_proxy_async_smem();
       __syncthreads();                                                     // S3: a2 tile complete
-      if (control) {
-        mbar_wait(bar_w3, w3_par);     // landed during the stencil
-        w3_par ^= 1;
-        tc_fence_after();
-        for (int h = 0; h < p_halves; ++h)
+      // ---- project(c): [64 px x 64] x [64 x 16 j], accumulated over the slices, left in flight ----
+      mbar_wait(bar_w3, w3_par);       // landed during the stencil
+      w3_par ^= 1;
+      wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            umma_bf16(tmem + (uint32_t)(p.proj_col + h * p_nn), ad_h2 + (uint64_t)(kk * 2),
-                      bd_w3 + (uint64_t)((h * p_nn * 128 + kk * 32) >> 4), idesc_p,
-                      (c > 0 || kk > 0) ? 1u : 0u);
-        umma_commit(bar_p);
+      for (int j = 0; j < kMaxProjChunks; ++j) {
+        if (j >= p_nj) break;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_m64n16<0, 0>(pacc[j], gmma_smem_desc(sH2_u + (uint32_t)(p_row0 * 128 + kk * 32), 16, 1024),
+                             gmma_smem_desc(sW3_u + (uint32_t)((p_j0 + j) * 2048 + kk * 32), 16, 1024), 1u);
       }
+      wgmma_commit();
     }
     // ---- epilogue 2: y = bf16(bn3(h3) (+ x)) ----
-    wait_projects(gc);
-    tc_fence_after();
-    __syncwarp();
-    {
-      const int n = g * TI + e2_ti, yy = ty * TOH + e2_oy, xx = tx * TOW + e2_ox;
-      const bool valid = e2_r < NPO && n < p.N && yy < p.Ho && xx < p.Wo;
-      const size_t pix = valid ? ((size_t)(n * p.Ho + yy) * p.Wo + xx) : 0;
-      const uint32_t taddr = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)p.proj_col;
-      const int units = p.Npad >> 4;
-#pragma unroll 1
-      for (int u = warp >> 2; u < units; u += 2) {
-        uint32_t acc[16];
-        tmem_ld_32x16(taddr + (uint32_t)(u * 16), acc);
-        tmem_ld_wait();
+    wgmma_wait<0>();
+    reg_fence(pacc);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int col = u * 16 + h * 8;
-          if (valid && col < p.Cout) {
-            float v[8];
+    for (int hh = 0; hh < 2; ++hh) {
+      const int r = p_row0 + q * 16 + (lane >> 2) + 8 * hh;
+      const int ti = r / (TOH * TOW);
+      const int oy = (r % (TOH * TOW)) / TOW, ox = (r % (TOH * TOW)) % TOW;
+      const int n = g * TI + ti, yy = ty * TOH + oy, xx = tx * TOW + ox;
+      if (!(r < NPO && n < p.N && yy < p.Ho && xx < p.Wo)) continue;
+      const size_t pix = (size_t)(n * p.Ho + yy) * p.Wo + xx;
 #pragma unroll
-            for (int e = 0; e < 8; ++e)
-              v[e] = fmaf(c3[col + e], __uint_as_float(acc[h * 8 + e]), c3[p.Npad + col + e]);
-            if (p.residual) {
-              const uint4 rx = __ldg(reinterpret_cast<const uint4*>(p.x + pix * p.Cin + col));
-              const uint32_t rw[4] = {rx.x, rx.y, rx.z, rx.w};
+      for (int j = 0; j < kMaxProjChunks; ++j) {
+        if (j >= p_nj) break;
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                v[2 * e] += bf16lo(rw[e]);
-                v[2 * e + 1] += bf16hi(rw[e]);
-              }
-            }
-            *reinterpret_cast<uint4*>(p.y + pix * p.Cout + col) =
-                make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]),
-                           pack_bf16(v[6], v[7]));
+        for (int h8 = 0; h8 < 2; ++h8) {
+          const int col = (p_j0 + j) * 16 + h8 * 8 + 2 * (lane & 3);
+          if (col >= p.Cout) continue;
+          float v0 = fmaf(c3[col], pacc[j][4 * h8 + 2 * hh], c3[p.Npad + col]);
+          float v1 = fmaf(c3[col + 1], pacc[j][4 * h8 + 2 * hh + 1], c3[p.Npad + col + 1]);
+          if (p.residual) {
+            const uint32_t rx = __ldg(reinterpret_cast<const uint32_t*>(p.x + pix * p.Cin + col));
+            v0 += bf16lo(rx);
+            v1 += bf16hi(rx);
           }
+          *reinterpret_cast<uint32_t*>(p.y + pix * p.Cout + col) = pack_bf16(v0, v1);
         }
       }
     }
-    // the next tile's first project MMA (accumulate = 0) is issued behind S2 and S3 of its first
-    // slice: every warp's accumulator reads above are complete by then
-    tc_fence_before();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -536,7 +463,7 @@ static int make_map(CUtensorMap* map, const void* ptr, int rank, const cuuint64_
 template <class G, bool EXPAND, bool LEAN>
 static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream_t st) {
   // ---- shared-memory plan (bytes from the 1024-aligned base) ----
-  // x tile: NPI rows of 128 B per 64-channel panel; the second 128-row MMA tile of a panel reads
+  // x tile: NPI rows of 128 B per 64-channel panel; the last 64-row MMA chunk of a panel reads
   // past them (rows that are never used): those reads stay inside this CTA's allocation
   p.xpanel_bytes = (G::NPI * 128 + 1023) & ~1023;
   int off = p.KB * p.xpanel_bytes;
@@ -546,16 +473,14 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
   p.off_h1 = off; off += ((G::NPI * kH1Pitch) + 15) & ~15;
   p.off_tab = off; off += 2 * tab_floats(G::K) * 4;
   p.off_c3 = off; off += 2 * p.Npad * 4;
-  p.off_bars = (off + 15) & ~15; off = p.off_bars + 48;
+  p.off_bars = (off + 15) & ~15; off = p.off_bars + 16;
   int smem = off;
-  const int x_read_end = (p.KB - 1) * p.xpanel_bytes + 32768;   // last byte the expand MMA may touch
+  const int x_read_end = (p.KB - 1) * p.xpanel_bytes + G::NCH * 8192;   // last byte the expand MMA may touch
   if (smem < x_read_end) smem = x_read_end;
   if (smem > 227 * 1024) return set_error(YAMB_EINVAL, "block_eval: tile does not fit shared memory");
-  p.proj_col = 128;
-  int need = p.proj_col + p.Npad, cols = 32;
-  while (cols < need) cols *= 2;
-  if (cols > 512) return set_error(YAMB_EINVAL, "block_eval: accumulators exceed TMEM");
-  p.tmem_cols = cols;
+  // project accumulators per thread: 64 x Npad (one 64-row half) or half of the 16-column groups
+  const int chunks = G::PM == 2 ? p.Npad / 16 : (p.Npad / 16 + 1) / 2;
+  if (chunks > kMaxProjChunks) return set_error(YAMB_EINVAL, "block_eval: accumulators exceed the registers");
   const int groups = (p.N + G::TI - 1) / G::TI;
   p.tiles_h = (p.Ho + G::TOH - 1) / G::TOH;
   p.tiles_w = (p.Wo + G::TOW - 1) / G::TOW;
@@ -596,24 +521,21 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
     if (attr < smem) {
       cudaError_t e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN>,
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      if (e == cudaSuccess)   // two CTAs of ~90 KB need the largest shared-memory carve-out
+      if (e == cudaSuccess)
         e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared);
       if (e != cudaSuccess) return set_error(YAMB_ECUDA, "block_eval attr: %s", cudaGetErrorString(e));
       attr = smem;
     }
   }
-  // Resident CTAs per SM: 228 KB of shared memory (+1 KB the driver reserves per CTA), 512 TMEM
-  // columns, 64 Ki registers (__launch_bounds__(256, 2): <= 128 per thread).
-  // (cudaOccupancyMaxActiveBlocksPerMultiprocessor answers 1 for the ~100 KB configurations that
-  // ncu's launch__occupancy_limit_* and the hardware both place twice: computed here.)
-  const int per_sm = (2 * (smem + 1024) <= 228 * 1024 && 2 * cols <= 512) ? 2 : 1;
-  const long long cap = (long long)max_ctas() * per_sm;
+  // One resident CTA per SM: the project accumulators, the stencil and the expand fragments take
+  // more than the 128 registers per thread that two CTAs of 256 threads could have.
+  const long long cap = (long long)max_ctas();
   const int grid = (int)(p.num_tiles < cap ? p.num_tiles : cap);
   static const bool dbg = getenv("YAMB_EVAL_DEBUG") != nullptr;
   if (dbg)
-    fprintf(stderr, "block_eval: tiles %d grid %d per_sm %d smem %d tmem_cols %d Npad %d NC %d KB %d\n",
-            p.num_tiles, grid, per_sm, smem, cols, p.Npad, p.NC, p.KB);
+    fprintf(stderr, "block_eval: tiles %d grid %d smem %d Npad %d NC %d KB %d\n",
+            p.num_tiles, grid, smem, p.Npad, p.NC, p.KB);
   block_eval_kernel<G, EXPAND, LEAN><<<grid, 256, smem, st>>>(tmX, tmW1, tmW3, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "block_eval launch: %s", cudaGetErrorString(e));
@@ -679,7 +601,10 @@ int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
   p.Npad = (a->Cout + 15) / 16 * 16;
   p.NC = (a->Chid + 63) / 64;
   const bool ex = a->w_expand != nullptr;
-  // fewest tiles among the geometries of (k, stride); each holds its input tile in <= 256 rows
+  // fewest tiles among the geometries of (k, stride); each holds its input tile in <= 256 rows.
+  // Tiles of more than 64 output pixels keep 64 x Npad project accumulators per thread: wide
+  // outputs (Npad > 160) take one 7x7 image per tile instead.
+  const bool wide = p.Npad > 16 * kMaxProjChunks;
   auto tiles_of = [&](int toh, int tow, int ti) {
     return (long long)((p.Ho + toh - 1) / toh) * ((p.Wo + tow - 1) / tow) * ((a->N + ti - 1) / ti);
   };
@@ -687,6 +612,9 @@ int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
     if (a->stride == 2)   // 7x7 outputs from a 15x15 input tile, 2 channels per stencil thread
       return ex ? launch_eval<EvGeom<3, 2, 7, 7, 1, 2>, true>(p, a, st)
                 : launch_eval<EvGeom<3, 2, 7, 7, 1, 2>, false>(p, a, st);
+    if (wide)
+      return ex ? launch_eval<EvGeom<3, 1, 7, 7, 1, 4>, true>(p, a, st)
+                : launch_eval<EvGeom<3, 1, 7, 7, 1, 4>, false>(p, a, st);
     const long long t0 = tiles_of(7, 16, 1), t1 = tiles_of(7, 14, 1), t2 = tiles_of(7, 7, 2);
     if (t0 <= t1 && t0 <= t2)
       return ex ? launch_eval<EvGeom<3, 1, 7, 16, 1, 4>, true>(p, a, st)
@@ -699,6 +627,7 @@ int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
   }
   if (a->kernel == 5) {
     if (a->stride == 2) return launch_eval_act<EvGeom<5, 2, 6, 7, 1, 2>, true, true>(p, a, st);
+    if (wide) return launch_eval_act<EvGeom<5, 1, 7, 7, 1, 4>, true, true>(p, a, st);
     const long long t0 = tiles_of(7, 16, 1), t1 = tiles_of(7, 14, 1), t2 = tiles_of(7, 7, 2);
     if (t0 <= t1 && t0 <= t2) return launch_eval_act<EvGeom<5, 1, 7, 16, 1, 4>, true, true>(p, a, st);
     if (t1 <= t2) return launch_eval_act<EvGeom<5, 1, 7, 14, 1, 4>, true, true>(p, a, st);

@@ -1,4 +1,4 @@
-// Depthwise k x k convolution (k in {3,5,7}, stride 1/2) on NHWC bf16 activations, sm_100a.
+// Depthwise k x k convolution (k in {3,5,7}, stride 1/2) on NHWC bf16 activations, sm_90a.
 //
 // Replaces, behind yamb_depthwise_fwd / yamb_depthwise_bwd (include/yamb200.h), the
 // nn.Conv2d(groups=C) + BatchNorm2d + activation library calls of the reference block
@@ -357,6 +357,7 @@ struct DwBwdDev {
   const float *ca, *cb, *cc;
   const float* w;           // [C][K][K]
   float* dw;                // [C][K][K] +=
+  float* part;              // [CTA][C][K][K] per-CTA weight-gradient partials (zero-filled)
   const __nv_bfloat16* x;   // [N,H,W,ldc] pre-BN input of the depthwise stage
   const float *in_scale, *in_shift;
   int in_act;
@@ -445,15 +446,22 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_
 
   // registers -> shared (per chunk) -> one global reduction per (tap, channel) / channel
   auto flush = [&](int chunk) {
+    // the thread tiles that share a channel group add in a fixed order (deterministic sums)
+    for (int g = 0; g < (256 + NCG - 1) / NCG; ++g) {
+      if (sp == g) {
 #pragma unroll
-    for (int tp = 0; tp < NT; ++tp) {
-      float* dst = &s_gw[(TAP0 + tp) * CT + cg * 4];
-      atomicAdd(dst + 0, gw[tp][0].x);
-      atomicAdd(dst + 1, gw[tp][0].y);
-      atomicAdd(dst + 2, gw[tp][1].x);
-      atomicAdd(dst + 3, gw[tp][1].y);
-      gw[tp][0] = gw[tp][1] = make_float2(0.f, 0.f);
+        for (int tp = 0; tp < NT; ++tp) {
+          float* dst = &s_gw[(TAP0 + tp) * CT + cg * 4];
+          dst[0] += gw[tp][0].x;
+          dst[1] += gw[tp][0].y;
+          dst[2] += gw[tp][1].x;
+          dst[3] += gw[tp][1].y;
+        }
+      }
+      __syncthreads();
     }
+#pragma unroll
+    for (int tp = 0; tp < NT; ++tp) gw[tp][0] = gw[tp][1] = make_float2(0.f, 0.f);
     if (DGRAD) {
 #pragma unroll
       for (int v = 0; v < 4; ++v) {
@@ -467,7 +475,7 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_
     for (int i = tid; i < KK * CT; i += 256) {
       const int tp = i / CT, c = cbase + i % CT;
       const float g = s_gw[i];
-      if (c < p.C && g != 0.f) atomicAdd(p.dw + (size_t)c * KK + tp, g);
+      if (c < p.C && g != 0.f) p.part[((size_t)blockIdx.x * p.C + c) * KK + tp] = g;   // once per CTA
       s_gw[i] = 0.f;
     }
     if (DGRAD && p.has_bn && tid < 2 * CT) {
@@ -738,8 +746,9 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_
   }
 }
 
+// Grid of kernel `kern` for `tiles` tiles at `smem` bytes of dynamic shared memory.
 template <typename Kern, typename Dev>
-static cudaError_t launch_k(Kern kern, const Dev& p, size_t smem, long long tiles, cudaStream_t st) {
+static cudaError_t grid_k(Kern kern, const Dev& p, size_t smem, long long tiles, int* grid_out) {
   // The dynamic-smem limit of a kernel is process-wide state: only ever RAISE it (forward and
   // backward run on different host threads); occupancy is cached per (kernel, smem size).
   struct Ent { const void* k; size_t smem; int per_sm; };
@@ -776,19 +785,50 @@ static cudaError_t launch_k(Kern kern, const Dev& p, size_t smem, long long tile
   // of being fetched from DRAM once per chunk (ncu r01: 2.7x the algorithmic reads at C = 144).
   if (p.chunks > 1 && grid > p.chunks) grid = grid / p.chunks * p.chunks;
   if (grid < 1) grid = 1;
+  *grid_out = grid;
+  return cudaSuccess;
+}
+
+template <typename Kern, typename Dev>
+static cudaError_t launch_k(Kern kern, const Dev& p, size_t smem, long long tiles, cudaStream_t st) {
+  int grid = 0;
+  cudaError_t e = grid_k(kern, p, smem, tiles, &grid);
+  if (e != cudaSuccess) return e;
   kern<<<grid, 256, smem, st>>>(p);
   return cudaGetLastError();
 }
 
 template <int KK, int SS, int CC, typename Dev>
-static cudaError_t launch_bwd(const Dev& p, size_t smem, long long tiles, cudaStream_t st) {
-  if constexpr (KK == 7) {
-    cudaError_t e = launch_k(dw_bwd_kernel<KK, SS, CC, 0, 25, true>, p, smem, tiles, st);
-    if (e != cudaSuccess) return e;
-    return launch_k(dw_bwd_kernel<KK, SS, CC, 25, KK * KK, false>, p, smem, tiles, st);
-  } else {
-    return launch_k(dw_bwd_kernel<KK, SS, CC, 0, KK * KK, true>, p, smem, tiles, st);
+static cudaError_t launch_bwd(const Dev& p0, size_t smem, long long tiles, cudaStream_t st) {
+  // weight gradient: per-CTA partials (zero where a CTA has no tile of a channel chunk), then
+  // added in CTA order
+  auto k0 = dw_bwd_kernel<KK, SS, CC, 0, (KK == 7 ? 25 : KK * KK), true>;
+  int g0 = 0, g1 = 0;
+  cudaError_t e = grid_k(k0, p0, smem, tiles, &g0);
+  if constexpr (KK == 7)   // the taps past 25 in a second kernel
+    if (e == cudaSuccess) e = grid_k(dw_bwd_kernel<KK, SS, CC, 25, KK * KK, false>, p0, smem, tiles, &g1);
+  if (e != cudaSuccess) return e;
+  const int slabs = g0 > g1 ? g0 : g1;
+  const long long n = (long long)p0.C * KK * KK;
+  Dev p = p0;
+  if (det_alloc((size_t)(slabs * n) * sizeof(float), st, &p.part)) return cudaErrorMemoryAllocation;
+  e = cudaMemsetAsync(p.part, 0, (size_t)(slabs * n) * sizeof(float), st);
+  if (e == cudaSuccess) {
+    k0<<<g0, 256, smem, st>>>(p);
+    e = cudaGetLastError();
   }
+  if constexpr (KK == 7) {
+    if (e == cudaSuccess) {
+      dw_bwd_kernel<KK, SS, CC, 25, KK * KK, false><<<g1, 256, smem, st>>>(p);
+      e = cudaGetLastError();
+    }
+  }
+  if (e != cudaSuccess) {
+    det_free(p.part, st);
+    return e;
+  }
+  if (det_reduce_launch(p.part, slabs, n, p.dw, st)) return cudaErrorLaunchFailure;
+  return cudaSuccess;
 }
 #define YAMB_DW_BWD(KK, SS, CC, ...) e = launch_bwd<KK, SS, CC>(__VA_ARGS__)
 

@@ -1,4 +1,4 @@
-// HBM-bound per-channel kernels on [pixels, channels] bf16 matrices, sm_100a:
+// HBM-bound per-channel kernels on [pixels, channels] bf16 matrices, sm_90a:
 //   bn_apply   y = act(scale[c]*h + shift[c]) (+ residual)        — pw_bn + skip connection of
 //              the block (reference models/mobilenet_base.py:448-450, :340-341) and the
 //              ConvBNReLU tails (:203)

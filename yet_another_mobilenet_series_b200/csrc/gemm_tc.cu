@@ -1,22 +1,22 @@
-// Pointwise-convolution GEMM for sm_100a: operand loaders -> shared memory -> tcgen05.mma -> TMEM ->
+// Pointwise-convolution GEMM for sm_90a: operand loaders -> shared memory -> wgmma -> registers ->
 // epilogue.
 //
 // One persistent CTA (512 threads) per SM, warp-specialised:
 //   warp 0      TMA producer for WIDE TRANSFORMED operands only (128-byte box rows)
-//   warp 1      MMA issuer   (one elected lane, tcgen05.mma.cta_group::1.kind::f16, M=128)
-//   warp 2      TMEM allocator / deallocator
-//   warp 3      idle
-//   warps 4-11  epilogue, two warpgroups that alternate tiles (one per TMEM accumulator stage) so
-//               the latency chain of one tile hides behind the other; every WARP is independent:
-//               tcgen05.ld (its 32 TMEM lanes) -> registers -> fused math -> warp-private swizzled
-//               smem -> its own TMA store (box 64 x 32) -> per-column BatchNorm statistics read back
-//               from the staged tile.  No CTA-wide barrier in the steady state.
+//   warps 1-3   barrier set-up, then idle
+//   warps 4-11  two consumer warpgroups that alternate tiles: each runs the wgmma main loop of its
+//               tile (128 x block_n, two m64 halves, fp32 accumulators in registers) and then its
+//               epilogue, while the other warpgroup runs the next tile's main loop.  A turn barrier
+//               hands the main loop over, so the k-blocks are consumed in ring order.  Every WARP's
+//               epilogue is independent: registers -> fused math -> warp-private swizzled smem ->
+//               its own TMA stores (two boxes of 64 x 16) -> per-column BatchNorm statistics read
+//               back from the staged tile.  No CTA-wide barrier in the steady state.
 //   warps 12-15 (and 8-11 when the epilogue is light) operand loaders: one warp per pipeline stage;
 //               plain operands by cp.async into the swizzled layout, narrow transformed operands
 //               through registers, wide transformed operands rewritten in place after the TMA
 //               landed them (BN-apply + activation, or the two-source BN-backward affine)
-// (TMA tile loads cost 7-16 cycles per box row whatever its width: with the 32-96-byte rows of the
-// narrow operands the TMA unit bounded every GEMM — measured with the YAMB_GEMM_DEBUG=512 timers.)
+// (TMA tile loads cost several cycles per box row whatever its width: with the 32-96-byte rows of
+// the narrow operands the TMA unit would bound the GEMM, so those go through cp.async.)
 //
 // Replaces, behind yamb_pointwise_gemm (include/yamb200.h), the nn.Conv2d(kernel_size=1) forward /
 // dgrad / wgrad library calls of the reference block (models/mobilenet_base.py:391-395, :413,
@@ -51,8 +51,7 @@ constexpr int kABytes = 16384;       // 128 x 64 bf16
 constexpr int kWarpOutBytes = 4096;  // 32 rows x 64 cols bf16: one warp's staging sub-tile
 constexpr int kEpiWarps = 8;
 constexpr int kMaxStages = 8;
-constexpr int kTmemCols = 512;
-constexpr int kAccStride = 256;  // two accumulator stages of 256 columns
+constexpr int kMaxBlockN = 64;    // 2 x 32 fp32 accumulators per thread of a consumer warpgroup
 
 struct GemmDev {
   int M, N, K;
@@ -78,13 +77,13 @@ struct GemmDev {
   long long gate_rps;            // pixels per sample
   int wg2x;                   // 1: warps 8-11 transform (light epilogue), 0: they are epilogue WG 1
   int dbg;                    // YAMB_GEMM_DEBUG bits: 1 skip transform math, 2 skip proxy fence
-  unsigned long long* dbg_buf;  // bit 512: per-phase cycle sums of the epilogue warps
+  unsigned long long* dbg_buf;  // bit 512: per-phase cycle sums of the loader warps
   // operand tensors in global memory ([pixels|rows][channels], bf16) for the cp.async loaders
   const __nv_bfloat16 *gA, *gA2, *gB, *gB2;
   long long lda, lda2, ldb, ldb2;
   int a_tma, b_tma;           // wide transformed operand: TMA load + in-place smem transform
   int lgroup;                 // loader warps that share one stage (1, 2 or 4)
-  int red_vec;                // epi 2: D rows are 16-byte aligned -> vector reductions
+  float* part;                // epi 2: [num_work][128][64] fp32 split-K partial tiles
   yamb_bn_fwd bnf;
   int has_bnf;
   const float *h_scale, *h_shift;
@@ -99,10 +98,7 @@ struct Bars {
   uint64_t full[kMaxStages];
   uint64_t xdone[kMaxStages];
   uint64_t empty[kMaxStages];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
-  uint32_t pad;
+  uint64_t turn[2];   // main-loop hand-over between the two consumer warpgroups
 };
 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
@@ -269,6 +265,14 @@ __device__ __forceinline__ void gxform_panel(uint32_t panel, uint32_t panel2, co
   }
 }
 
+// One k16 step of a 64-row half: d[0 .. bn/2) (+)= A * B with the wgmma of width bn.
+template <int TA, int TB>
+__device__ __forceinline__ void mma_bn(float (&d)[32], int bn, uint64_t ad, uint64_t bd) {
+  if (bn == 64) wgmma_m64n64<TA, TB>(d, ad, bd, 1u);
+  else if (bn == 32) wgmma_m64n32<TA, TB>(reinterpret_cast<float(&)[16]>(d), ad, bd, 1u);
+  else wgmma_m64n16<TA, TB>(reinterpret_cast<float(&)[8]>(d), ad, bd, 1u);
+}
+
 template <bool kXform, int kEpi>
 __global__ void __launch_bounds__(512, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -295,31 +299,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int i = 0; i < S; ++i) {
       mbar_init(&bars->full[i], p.lgroup);   // the loader warps that own the stage arrive
       mbar_init(&bars->xdone[i], 1);
-      mbar_init(&bars->empty[i], 1);
+      mbar_init(&bars->empty[i], 128);       // every thread of the consuming warpgroup arrives
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bars->tmem_full[i], 1);
-      mbar_init(&bars->tmem_empty[i], 128);
-    }
+    for (int i = 0; i < 2; ++i) mbar_init(&bars->turn[i], 1);
     fence_barrier_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(&bars->tmem_base, kTmemCols);
-    tmem_relinquish();
   }
   // zero the per-CTA statistics accumulators
   if (p.has_bnf || p.has_bnb) {
     for (int i = threadIdx.x; i < 2 * p.N; i += blockDim.x) s_stats[i] = 0.0;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
   const bool use_x = kXform && (p.a_xform != 0 || p.b_xform != 0);
 
   // 512-thread variant: every thread starts with 128 registers; the control warpgroup hands its
-  // surplus to the two epilogue warpgroups (64*4 + 160*8 + 128*4 warps x 32 lanes = 64 Ki regs).
+  // surplus to the consumer and loader warps (56*4 + 152*12 warps x 32 lanes = 64 Ki regs).
   if (warp < 4) {
    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
    if (warp == 0) {
@@ -398,59 +392,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-   } else if (warp == 1) {
-    // ====================================== MMA issuer ======================================
-    const uint32_t idesc = umma_idesc_bf16(kBlockM, p.block_n, p.a_mn, p.b_mn);
-    int stage = 0, phase = 0, it = 0;
-    long long dbg_mma_full = 0, dbg_mma_empty = 0;
-    for (int w = blockIdx.x; w < p.num_work; w += gridDim.x, ++it) {
-      const int slab = w % p.ksplit;
-      const int kb0 = slab * p.kb_per_split;
-      const int kb1 = min(kb0 + p.kb_per_split, p.num_k_blocks);
-      const int as = it & 1;
-      const long long te0 = YCLK();
-      MBAR_WAIT(&bars->tmem_empty[as], ((it >> 1) & 1) ^ 1);
-      dbg_mma_empty += YCLK() - te0;
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(as * kAccStride);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        const long long tm0 = YCLK();
-        MBAR_WAIT(&bars->full[stage], phase);
-        dbg_mma_full += YCLK() - tm0;
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sA = smem_u32(smem + (size_t)stage * p.stage_bytes);
-          const uint32_t sB = sA + p.a_bytes;
-          const int krem = p.K - kb * kBlockK;
-          const int nk = krem >= kBlockK ? 4 : (krem + 15) / 16;
-          for (int kk = 0; kk < nk; ++kk) {
-            const uint64_t ad = p.a_mn ? umma_smem_desc(sA + kk * 2048, kPanelBytes64, 1024)
-                                       : umma_smem_desc(sA + kk * 32, 16, 1024);
-            const uint64_t bd = p.b_mn ? umma_smem_desc(sB + kk * 2048, kPanelBytes64, 1024)
-                                       : umma_smem_desc(sB + kk * 32, 16, 1024);
-            umma_bf16(tmem_d, ad, bd, idesc, (kb > kb0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&bars->empty[stage]);
-          if (kb == kb1 - 1) umma_commit(&bars->tmem_full[as]);
-        }
-        __syncwarp();
-        if (++stage == S) { stage = 0; phase ^= 1; }
-      }
-    }
-    if ((p.dbg & 512) && lane == 0) {
-      atomicAdd(p.dbg_buf + 10, (unsigned long long)dbg_mma_full);
-      atomicAdd(p.dbg_buf + 11, (unsigned long long)dbg_mma_empty);
-    }
    }
   } else if (warp < 8 || (warp < 12 && !(kXform && p.wg2x))) {
-    // ======================================= epilogue =======================================
+    // ============================ consumers: wgmma main loop + epilogue ============================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
     const int ew = warp - 4;           // 0..7
-    const int wg = ew >> 2;            // epilogue warpgroup = TMEM accumulator stage it serves
-    const int q = warp & 3;            // TMEM lane quadrant of this warp
-    const int row = q * 32 + lane;     // row inside the 128-row tile
+    const int wg = ew >> 2;            // consumer warpgroup
+    const int q = warp & 3;            // warp of the warpgroup: rows 16q..16q+15 of each 64-row half
+    const int ctid = threadIdx.x & 127;
     uint8_t* s_out = smem + p.off_out + (size_t)ew * p.out_bufs * kWarpOutBytes;
-    uint8_t* s_h = smem + p.off_hside + (size_t)ew * kWarpOutBytes;  // epi 1: raw H rows
+    uint8_t* s_h = smem + p.off_hside + (size_t)ew * kWarpOutBytes;  // side rows (residual / H)
     // per-column coefficient tables for epi 1:  [h_scale | h_shift | mean | invstd] x N
     const float* cz_s = s_coef;
     const float* cz_t = s_coef + p.N;
@@ -471,27 +422,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint32_t sub_count = 0;   // running sub-tile counter of this warp -> staging buffer parity
     const bool side_in = (kEpi == 1) || p.has_residual;
     const ActParam hap = make_act(kEpi == 1 ? p.h_act : ACT_NONE);
+    // A warp stages 32 rows of a tile: staged row r <-> tile row 64 * (r >> 4) + 16 q + (r & 15)
+    // (the rows of its wgmma accumulator fragments in the two 64-row halves).
+    const int lane_trow = (lane >> 4) * 64 + q * 16 + (lane & 15);
     // Column statistics: with a single n-block every lane owns the same 2 columns of sub-tile j in
     // every tile, so the sums live in registers for the whole kernel (shared-memory float atomics
     // are CAS loops and serialise the 8 epilogue warps); flushed once at the end.
     const bool reg_stats = (p.has_bnf || p.has_bnb) && p.n_blocks == 1;
-    float racc[4][4];
+    float racc[kMaxBlockN / 64][4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
+    for (int j = 0; j < kMaxBlockN / 64; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) racc[j][e] = 0.f;
-    int it = 0;
-    long long dbg_t[6] = {0, 0, 0, 0, 0, 0};
-    const long long dbg_start = YCLK();
-    // Side operand (residual / H) rows come straight from global memory (each thread owns one row:
+    // Side operand (residual / H) rows come straight from global memory (lane r loads staged row r:
     // 8 x 16 B per 64-column sub-tile).  They are requested ONE SUB-TILE AHEAD, into the registers
-    // the previous sub-tile has just finished with: issued at the top of a sub-tile their ~2 us
-    // latency was fully exposed (the "convert" phase of the dgrad epilogue was 4000 cycles).
+    // the previous sub-tile has just finished with, so their latency hides behind the math.
     uint4 sv[8];
     auto load_side = [&](int w2, int sub2) {
       const int mn2 = w2 / p.ksplit;
       const int m2 = mn2 / p.n_blocks, n2 = mn2 % p.n_blocks;
-      const int grow2 = m2 * kBlockM + row;
+      const int grow2 = m2 * kBlockM + lane_trow;
       const int col2 = n2 * p.block_n + sub2 * 64;
       const __nv_bfloat16* srow = p.side + (size_t)grow2 * p.lds + col2;
 #pragma unroll
@@ -506,253 +456,205 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int w0 = blockIdx.x + ((n_epi_wg == 2 && wg == 1) ? (int)gridDim.x : 0);
       if (w0 < p.num_work) load_side(w0, 0);
     }
+    // wgmma of one 64-row half: block_n and the operand majors select the instruction
+    auto mma_half = [&](float (&d)[32], uint64_t ad, uint64_t bd) {
+      if (p.a_mn) {
+        if (p.b_mn) mma_bn<1, 1>(d, p.block_n, ad, bd);
+        else mma_bn<1, 0>(d, p.block_n, ad, bd);
+      } else {
+        if (p.b_mn) mma_bn<0, 1>(d, p.block_n, ad, bd);
+        else mma_bn<0, 0>(d, p.block_n, ad, bd);
+      }
+    };
+    float acc[2][32];
+    int stage = 0, phase = 0, it = 0;
+    uint32_t turn_par = 0;
     for (int w = blockIdx.x; w < p.num_work; w += gridDim.x, ++it) {
-      if (n_epi_wg == 2 && (it & 1) != wg) continue;  // the other warpgroup owns this tile
-      const int mn = w / p.ksplit;
+      const int mn = w / p.ksplit, slab = w % p.ksplit;
+      const int kb0 = slab * p.kb_per_split;
+      const int kb1 = min(kb0 + p.kb_per_split, p.num_k_blocks);
+      if (n_epi_wg == 2 && (it & 1) != wg) {   // the other warpgroup owns this tile: skip its stages
+        stage += kb1 - kb0;
+        while (stage >= S) { stage -= S; phase ^= 1; }
+        continue;
+      }
       const int m_blk = mn / p.n_blocks, n_blk = mn % p.n_blocks;
-      const int as = it & 1;
-      const int grow = m_blk * kBlockM + row;
-      const bool row_ok = grow < p.M;
+      const bool hi_half = m_blk * kBlockM + 64 < p.M;   // rows 64..127 of the tile exist
+      // ---- main loop ----
+      if (n_epi_wg == 2 && it > 0) {
+        MBAR_WAIT(&bars->turn[wg], turn_par);
+        turn_par ^= 1;
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        MBAR_WAIT(&bars->full[stage], phase);
+        const uint32_t sA = smem_u32(smem + (size_t)stage * p.stage_bytes);
+        const uint32_t sB = sA + p.a_bytes;
+        const int krem = p.K - kb * kBlockK;
+        const int nk = krem >= kBlockK ? 4 : (krem + 15) / 16;
+        reg_fence(acc[0]);
+        reg_fence(acc[1]);
+        wgmma_fence();
+#pragma unroll 1
+        for (int kk = 0; kk < nk; ++kk) {
+          const uint64_t bd = p.b_mn ? gmma_smem_desc(sB + kk * 2048, kPanelBytes64, 1024)
+                                     : gmma_smem_desc(sB + kk * 32, 16, 1024);
+          mma_half(acc[0], p.a_mn ? gmma_smem_desc(sA + kk * 2048, kPanelBytes64, 1024)
+                                  : gmma_smem_desc(sA + kk * 32, 16, 1024), bd);
+          if (hi_half)
+            mma_half(acc[1], p.a_mn ? gmma_smem_desc(sA + kPanelBytes64 + kk * 2048, kPanelBytes64, 1024)
+                                    : gmma_smem_desc(sA + 64 * 128 + kk * 32, 16, 1024), bd);
+        }
+        wgmma_commit();
+        if (prev >= 0) {            // the previous k-block's MMAs retired: its stage is free
+          wgmma_wait<1>();
+          mbar_arrive(&bars->empty[prev]);
+        }
+        prev = stage;
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      if (prev >= 0) mbar_arrive(&bars->empty[prev]);
+      if (n_epi_wg == 2 && ctid == 0) mbar_arrive(&bars->turn[wg ^ 1]);   // next tile's main loop
+      // ---- epilogue ----
       // sub-tiles of 64 columns; skip the ones that lie entirely beyond N (last n-block)
       const int n_sub = min((p.block_n + 63) / 64, (p.N - n_blk * p.block_n + 63) / 64);
-      long long tq0 = YCLK();
-      if (p.dbg & 256) mbar_wait_spin(&bars->tmem_full[as], (it >> 1) & 1);
-      else mbar_wait_relaxed(&bars->tmem_full[as], (it >> 1) & 1);
-      tc_fence_after();
-      dbg_t[0] += YCLK() - tq0;
-      // NOT unrolled: one copy of the sub-tile body keeps the epilogue inside the instruction
-      // cache (4 unrolled copies x 3 epilogue kinds were ~20k instructions; "no instruction" was
-      // the top stall reason and a sub-tile took ~4000 cycles)
-#pragma unroll 1
-      for (int sub = 0; sub < n_sub; ++sub) {
+#pragma unroll
+      for (int sub = 0; sub < kMaxBlockN / 64; ++sub) {
+        if (sub >= n_sub) break;
         const int col0 = n_blk * p.block_n + sub * 64;  // global column of this sub-tile
-        const uint32_t taddr =
-            tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * kAccStride + sub * 64);
-        uint32_t acc[2][32];
-        long long tq1 = YCLK();
-        tmem_ld_32x32(taddr, acc[0]);
-        tmem_ld_32x32(taddr + 32, acc[1]);
-        tmem_ld_wait();
-        dbg_t[1] += YCLK() - tq1;
-        tq1 = YCLK();
-        if (sub == n_sub - 1) {
-          // accumulator fully read: hand the TMEM stage back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(&bars->tmem_empty[as]);
-        }
         if (kEpi == 2) {
-          // split-K partial sums: fp32 atomic accumulate into D[M][ldd]
-          // A thread owns one output row: 4 consecutive columns go out as ONE 16-byte vector
-          // reduction (red.global.add.v4.f32, sm_90+).  Scalar reds were 32 L2 atomic transactions
-          // per warp instruction (lanes = rows, 4 KB apart) and the 7x7 / 14x14 wgrads spent ~80 %
-          // of their time draining them (r2 timers: 17 us of CTA activity in a 100 us kernel).
-          if (row_ok) {
-            float* drow = reinterpret_cast<float*>(p.D) + (size_t)grow * p.ldd;
+          // split-K partial sums: plain stores of the fp32 tile into slab w of the scratch; the
+          // reduction kernel that follows adds the slabs into D in slab order (deterministic)
+          float* part = p.part + (size_t)w * (kBlockM * kMaxBlockN);
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
+          for (int h = 0; h < 2; ++h)
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const int c = col0 + h * 32 + j;
-                if (c < p.N && (sub * 64 + h * 32 + j) < p.block_n) {   // N, block_n: multiples of 8
-                  if (p.red_vec) {
-                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(drow + c),
-                                 "f"(__uint_as_float(acc[h][j])), "f"(__uint_as_float(acc[h][j + 1])),
-                                 "f"(__uint_as_float(acc[h][j + 2])), "f"(__uint_as_float(acc[h][j + 3]))
-                                 : "memory");
-                  } else {
+            for (int e = 0; e < 2; ++e) {
+              const int r = 64 * h + 16 * q + (lane >> 2) + 8 * e;
 #pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                      asm volatile("red.global.add.f32 [%0], %1;" ::"l"(drow + c + e),
-                                   "f"(__uint_as_float(acc[h][j + e]))
-                                   : "memory");
-                  }
-                }
-              }
-          }
+              for (int jj = 0; jj < 8; ++jj)
+                __stcg(reinterpret_cast<float2*>(part + r * kMaxBlockN + sub * 64 + jj * 8 + 2 * (lane & 3)),
+                       make_float2(acc[h][4 * (sub * 8 + jj) + 2 * e], acc[h][4 * (sub * 8 + jj) + 2 * e + 1]));
+            }
           continue;
         }
         uint8_t* sO = s_out + (p.out_bufs == 2 ? (sub_count & 1) : 0) * kWarpOutBytes;
-        // the TMA store that last read this staging buffer must have drained
+        // the TMA store that last read this staging buffer must have drained; the previous
+        // sub-tile's statistics reads of s_h are behind the __syncwarp that ends it
         if (lane == 0) {
           if (p.out_bufs == 2) tma_store_wait_read<1>();
           else tma_store_wait_read<0>();
         }
-        __syncwarp();
-        dbg_t[2] += YCLK() - tq1;
-        tq1 = YCLK();
-        // Straight-line conversion of the 8 chunks (8 columns each): the mode decisions are taken
-        // ONCE per sub-tile, outside the unrolled chunk loop, so the chunk bodies interleave
-        // (with a branch per chunk this phase took ~4700 cycles per sub-tile in the dgrad epilogue).
-        auto stage_chunk = [&](int ch, const float (&v)[8]) {
-          const int pc = ch ^ (lane & 7);
-          *reinterpret_cast<uint4*>(sO + lane * 128 + (pc << 4)) =
-              make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]),
-                         pack_bf16(v[6], v[7]));
-        };
-        if (kEpi == 1) {
-          auto dz_chunks = [&](const bool clampk) {   // inlined twice, `clampk` a constant in each
+        if (side_in) {
 #pragma unroll
-            for (int ch = 0; ch < 8; ++ch) {
-              float v[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) v[e] = __uint_as_float(acc[ch >> 2][(ch & 3) * 8 + e]);
-              const uint32_t sw[4] = {sv[ch].x, sv[ch].y, sv[ch].z, sv[ch].w};
-              // columns past N: read the last valid coefficients (the values are never stored)
-              const int cb = min(col0 + ch * 8, p.N - 8);
-              const float4 s0 = *reinterpret_cast<const float4*>(cz_s + cb);
-              const float4 s1 = *reinterpret_cast<const float4*>(cz_s + cb + 4);
-              const float4 t0 = *reinterpret_cast<const float4*>(cz_t + cb);
-              const float4 t1 = *reinterpret_cast<const float4*>(cz_t + cb + 4);
-              const float zs[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-              const float zt[8] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w};
-              float zz[8];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                zz[2 * e] = fmaf(zs[2 * e], bf16lo(sw[e]), zt[2 * e]);
-                zz[2 * e + 1] = fmaf(zs[2 * e + 1], bf16hi(sw[e]), zt[2 * e + 1]);
-              }
-              if (clampk) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = (zz[e] > hap.lo && zz[e] < hap.hi) ? v[e] : 0.f;
-              } else {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] *= act_bwd(zz[e], p.h_act);
-              }
-              *reinterpret_cast<uint4*>(s_h + lane * 128 + ((ch ^ (lane & 7)) << 4)) = sv[ch];
-              stage_chunk(ch, v);
-            }
-          };
-          if (hap.kind == 0) dz_chunks(true);
-          else dz_chunks(false);
-        } else if (side_in) {
-#pragma unroll
-          for (int ch = 0; ch < 8; ++ch) {
-            float v[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[e] = __uint_as_float(acc[ch >> 2][(ch & 3) * 8 + e]);
-            const uint32_t sw[4] = {sv[ch].x, sv[ch].y, sv[ch].z, sv[ch].w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              v[2 * e] += bf16lo(sw[e]);
-              v[2 * e + 1] += bf16hi(sw[e]);
-            }
-            stage_chunk(ch, v);
-          }
-        } else {
-#pragma unroll
-          for (int ch = 0; ch < 8; ++ch) {
-            float v[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[e] = __uint_as_float(acc[ch >> 2][(ch & 3) * 8 + e]);
-            stage_chunk(ch, v);
-          }
+          for (int ch = 0; ch < 8; ++ch)
+            *reinterpret_cast<uint4*>(s_h + lane * 128 + ((ch ^ (lane & 7)) << 4)) = sv[ch];
         }
-        dbg_t[3] += YCLK() - tq1;
-        tq1 = YCLK();
-        if (p.dbg & 128) {
-          // experiment: coalesced st.global from the staged tile instead of a TMA store
-          __syncwarp();
-          __nv_bfloat16* Dg = reinterpret_cast<__nv_bfloat16*>(p.D);
+        __syncwarp();
+        // fragments -> bf16 staged tile (row r at r * 128, 16-byte chunks swizzled by r & 7).
+        // Rows past M are staged as zero: the statistics below then sum all 32 rows.
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int r = (lane >> 3) + 4 * i;
-            const int gr = m_blk * kBlockM + q * 32 + r;
-            const int gc = col0 + (lane & 7) * 8;
-            const uint4 v = *reinterpret_cast<const uint4*>(sO + r * 128 + (((lane & 7) ^ (r & 7)) << 4));
-            if (gr < p.M && gc < p.N && (sub * 64 + (lane & 7) * 8) < p.block_n)
-              *reinterpret_cast<uint4*>(Dg + (size_t)gr * p.ldd + gc) = v;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int r = 16 * h + (lane >> 2) + 8 * e;
+            const bool rok = m_blk * kBlockM + 64 * h + 16 * q + (lane >> 2) + 8 * e < p.M;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int off = r * 128 + ((jj ^ (r & 7)) << 4) + ((lane & 3) << 2);
+              float v0 = acc[h][4 * (sub * 8 + jj) + 2 * e];
+              float v1 = acc[h][4 * (sub * 8 + jj) + 2 * e + 1];
+              if (kEpi == 1) {
+                const uint32_t hh = *reinterpret_cast<const uint32_t*>(s_h + off);
+                // columns past N: read the last valid coefficients (the values are never stored)
+                const int cb = min(col0 + jj * 8 + 2 * (lane & 3), p.N - 2);
+                const float z0 = fmaf(cz_s[cb], bf16lo(hh), cz_t[cb]);
+                const float z1 = fmaf(cz_s[cb + 1], bf16hi(hh), cz_t[cb + 1]);
+                if (hap.kind == 0) {
+                  v0 = (z0 > hap.lo && z0 < hap.hi) ? v0 : 0.f;
+                  v1 = (z1 > hap.lo && z1 < hap.hi) ? v1 : 0.f;
+                } else {
+                  v0 *= act_bwd(z0, p.h_act);
+                  v1 *= act_bwd(z1, p.h_act);
+                }
+              } else if (side_in) {
+                const uint32_t rr = *reinterpret_cast<const uint32_t*>(s_h + off);
+                v0 += bf16lo(rr);
+                v1 += bf16hi(rr);
+              }
+              *reinterpret_cast<uint32_t*>(sO + off) = rok ? pack_bf16(v0, v1) : 0u;
+            }
           }
-        } else {
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0 && !(p.dbg & 64)) {
-            tma_store_2d(&tmD, sO, col0, m_blk * kBlockM + q * 32);
-            tma_store_commit();
-          }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          tma_store_2d(&tmD, sO, col0, m_blk * kBlockM + q * 16);
+          tma_store_2d(&tmD, sO + 2048, col0, m_blk * kBlockM + 64 + q * 16);
+          tma_store_commit();
         }
         if (side_in) {
-          // sv is dead and the store's proxy fence (a MEMBAR that would wait for these loads) is
-          // behind us: request the next sub-tile's side rows now; they land during the
-          // statistics pass and the next accumulator load
+          // request the next sub-tile's side rows now; they land during the statistics pass and
+          // the next tile's main loop
           if (sub + 1 < n_sub) load_side(w, sub + 1);
           else if (w + w_step < p.num_work) load_side(w + w_step, 0);
         }
-        dbg_t[4] += YCLK() - tq1;
-        tq1 = YCLK();
         // ---- per-column statistics of this warp's 32 rows of the bf16-rounded output ----
         if (p.has_bnf || p.has_bnb) {
           const int c = col0 + 2 * lane;  // column pair owned by this lane
           if (c < p.N && (sub * 64 + 2 * lane) < p.block_n) {
             float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-            const int rmax = min(32, p.M - (m_blk * kBlockM + q * 32));
+            const float2 one2 = make_float2(1.f, 1.f), zero2 = make_float2(0.f, 0.f);
+            // 4 independent accumulator sets (a 32-deep dependent chain of LDS -> FADD/FFMA would
+            // sit on the epilogue's critical path)
+            float2 sA = zero2, sB = zero2, sC = zero2, sD = zero2;
+            float2 qA = zero2, qB = zero2, qC = zero2, qD = zero2;
             if (p.has_bnf) {
-              if (rmax == 32) {
-                // full sub-tile: 4 independent accumulator sets (a 32-deep dependent chain of
-                // LDS -> FADD/FFMA was ~1500 cycles on the epilogue's critical path per sub-tile);
-                // packed fp32x2: one FFMA2 adds the column pair, one squares-and-adds it
-                float2 sA = make_float2(0.f, 0.f), sB = sA, sC = sA, sD = sA;
-                float2 qA = sA, qB = sA, qC = sA, qD = sA;
-                const float2 one2 = make_float2(1.f, 1.f);
-                auto rowf = [&](int r, float2& S, float2& Q) {
-                  const uint32_t u = *reinterpret_cast<const uint32_t*>(
-                      sO + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + ((lane & 3) << 2));
-                  const float2 v = make_float2(bf16lo(u), bf16hi(u));
-                  S = ffma2(one2, v, S);
-                  Q = ffma2(v, v, Q);
-                };
+              auto rowf = [&](int r, float2& Sx, float2& Qx) {
+                const uint32_t u = *reinterpret_cast<const uint32_t*>(
+                    sO + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + ((lane & 3) << 2));
+                const float2 v = make_float2(bf16lo(u), bf16hi(u));
+                Sx = ffma2(one2, v, Sx);
+                Qx = ffma2(v, v, Qx);
+              };
 #pragma unroll
-                for (int r = 0; r < 32; r += 4) {
-                  rowf(r, sA, qA);
-                  rowf(r + 1, sB, qB);
-                  rowf(r + 2, sC, qC);
-                  rowf(r + 3, sD, qD);
-                }
-                s0 = (sA.x + sB.x) + (sC.x + sD.x); s1 = (sA.y + sB.y) + (sC.y + sD.y);
-                q0 = (qA.x + qB.x) + (qC.x + qD.x); q1 = (qA.y + qB.y) + (qC.y + qD.y);
-              } else {
-                for (int r = 0; r < rmax; ++r) {
-                  const uint32_t u = *reinterpret_cast<const uint32_t*>(
-                      sO + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + ((lane & 3) << 2));
-                  const float a = bf16lo(u), b = bf16hi(u);
-                  s0 += a; s1 += b;
-                  q0 = fmaf(a, a, q0); q1 = fmaf(b, b, q1);
-                }
+              for (int r = 0; r < 32; r += 4) {
+                rowf(r, sA, qA);
+                rowf(r + 1, sB, qB);
+                rowf(r + 2, sC, qC);
+                rowf(r + 3, sD, qD);
               }
             } else {
-              // sum(dz), sum(dz * xhat) with xhat = h * r - m * r: three packed FFMA2 per row
+              // sum(dz), sum(dz * xhat) with xhat = h * r - m * r
               const float2 r2 = make_float2(cz_r[c], cz_r[c + 1]);
               const float2 nmr2 = make_float2(-cz_m[c] * r2.x, -cz_m[c + 1] * r2.y);
-              const float2 one2 = make_float2(1.f, 1.f), zero2 = make_float2(0.f, 0.f);
-              float2 sA = zero2, sB = zero2, sC = zero2, sD = zero2;
-              float2 qA = zero2, qB = zero2, qC = zero2, qD = zero2;
-              auto rowacc = [&](int r, float2& S, float2& Q) {
+              auto rowacc = [&](int r, float2& Sx, float2& Qx) {
                 const int off = r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + ((lane & 3) << 2);
                 const uint32_t u = *reinterpret_cast<const uint32_t*>(sO + off);
                 const uint32_t hh = *reinterpret_cast<const uint32_t*>(s_h + off);
                 const float2 a = make_float2(bf16lo(u), bf16hi(u));
                 const float2 xh = ffma2(make_float2(bf16lo(hh), bf16hi(hh)), r2, nmr2);
-                S = ffma2(one2, a, S);
-                Q = ffma2(a, xh, Q);
+                Sx = ffma2(one2, a, Sx);
+                Qx = ffma2(a, xh, Qx);
               };
-              int r = 0;
 #pragma unroll 2
-              for (; r + 3 < rmax; r += 4) {   // four independent accumulator sets
+              for (int r = 0; r < 32; r += 4) {
                 rowacc(r, sA, qA);
                 rowacc(r + 1, sB, qB);
                 rowacc(r + 2, sC, qC);
                 rowacc(r + 3, sD, qD);
               }
-              for (; r < rmax; ++r) rowacc(r, sA, qA);
-              s0 = (sA.x + sB.x) + (sC.x + sD.x); s1 = (sA.y + sB.y) + (sC.y + sD.y);
-              q0 = (qA.x + qB.x) + (qC.x + qD.x); q1 = (qA.y + qB.y) + (qC.y + qD.y);
             }
+            s0 = (sA.x + sB.x) + (sC.x + sD.x); s1 = (sA.y + sB.y) + (sC.y + sD.y);
+            q0 = (qA.x + qB.x) + (qC.x + qD.x); q1 = (qA.y + qB.y) + (qC.y + qD.y);
             if (reg_stats) {
-              switch (sub) {  // constant register indices in every case
-                case 0: racc[0][0] += s0; racc[0][1] += s1; racc[0][2] += q0; racc[0][3] += q1; break;
-                case 1: racc[1][0] += s0; racc[1][1] += s1; racc[1][2] += q0; racc[1][3] += q1; break;
-                case 2: racc[2][0] += s0; racc[2][1] += s1; racc[2][2] += q0; racc[2][3] += q1; break;
-                default: racc[3][0] += s0; racc[3][1] += s1; racc[3][2] += q0; racc[3][3] += q1; break;
-              }
+              racc[sub][0] += s0; racc[sub][1] += s1; racc[sub][2] += q0; racc[sub][3] += q1;
             } else {
               atomicAdd(&s_stats[c], (stat_t)s0);
               atomicAdd(&s_stats[c + 1], (stat_t)s1);
@@ -760,21 +662,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               atomicAdd(&s_stats[p.N + c + 1], (stat_t)q1);
             }
           }
-          __syncwarp();  // s_h / sO reads done before the next sub-tile overwrites them
         }
-        dbg_t[5] += YCLK() - tq1;
+        __syncwarp();  // s_h / sO reads done before the next sub-tile overwrites them
         ++sub_count;
       }
     }
-    if ((p.dbg & 512) && lane == 0) {
-#pragma unroll
-      for (int i = 0; i < 6; ++i) atomicAdd(p.dbg_buf + i, (unsigned long long)dbg_t[i]);
-      atomicAdd(p.dbg_buf + 6, (unsigned long long)(YCLK() - dbg_start));
-      atomicAdd(p.dbg_buf + 7, 1ull);
-    }
     if (reg_stats) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
+      for (int j = 0; j < kMaxBlockN / 64; ++j) {
         const int c = j * 64 + 2 * lane;
         if (c < p.N) {
           atomicAdd(&s_stats[c], (stat_t)racc[j][0]);
@@ -793,7 +688,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // transformed operands through registers, wide transformed operands by rewriting the tile the
     // TMA producer (warp 0) landed; then they publish the stage to the MMA warp.  (TMA tile loads cost ~7-16 cycles per box ROW whatever its width:
     // with 32-96-byte rows of the narrow operands the TMA unit, not HBM, bounded every GEMM.)
-    // registers: 4 control warps x 56 + (epilogue + loader) warps x 152 = 64 Ki / 32
     asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
     const int nxt = p.wg2x ? 256 : 128;
     const int t = warp >= 12 ? threadIdx.x - 384 : threadIdx.x - 256 + 128;
@@ -1001,12 +895,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   // ---- teardown ---------------------------------------------------------------------------------
-  tc_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
   if (p.has_bnf) {
     if (publish_partials(s_stats, p.N, p.bnf.partials, p.bnf.counter)) {
       bn_fwd_finalize(p.bnf, p.N);
@@ -1019,6 +908,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       __syncthreads();
       if (threadIdx.x == 0) *p.bnb.counter = 0;
     }
+  }
+}
+
+// D[m][n] += the split-K partial tiles of (m, n), added in slab order
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ part, float* D,
+                                                            long long ldd, int M, int N, int block_n,
+                                                            int n_blocks, int ksplit) {
+  const long long total = (long long)M * N;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int m = (int)(i / N), n = (int)(i % N);
+    const int mn = (m / kBlockM) * n_blocks + n / block_n;
+    const float* pp = part + (size_t)mn * ksplit * (kBlockM * kMaxBlockN) + (m % kBlockM) * kMaxBlockN + n % block_n;
+    float acc = 0.f;
+    for (int k = 0; k < ksplit; ++k) acc += __ldcg(pp + (size_t)k * (kBlockM * kMaxBlockN));
+    D[(size_t)m * ldd + n] += acc;
   }
 }
 
@@ -1043,16 +947,12 @@ static int make_map_2d(CUtensorMap* map, const void* ptr, uint64_t inner, uint64
   return 0;
 }
 
-static int pick_block_n(int N) {
-  if (N <= 256) return (N + 15) / 16 * 16;
-  // multi-block: block_n must be a multiple of 64 so staging sub-tiles never straddle blocks
-  int best = 256, best_waste = 1 << 30;
-  for (int bn = 256; bn >= 128; bn -= 64) {
-    int blocks = (N + bn - 1) / bn;
-    int waste = blocks * bn - N;
-    if (waste < best_waste) { best_waste = waste; best = bn; }
-  }
-  return best;
+// block_n is the wgmma width: 16, 32 or 64.  The 128 x block_n fp32 accumulator of a tile lives in
+// the registers of one consumer warpgroup, and the kernel's 512 threads get at most 128 registers
+// each, so wider tiles would spill.  An MN-major B is read in 64-column panels.
+static int pick_block_n(int N, bool b_mn) {
+  if (b_mn || N > 32) return 64;   // several n-blocks: 64 columns each, one staging sub-tile
+  return N <= 16 ? 16 : 32;
 }
 
 int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
@@ -1069,7 +969,7 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   p.M = a->M; p.N = a->N; p.K = a->K;
   p.a_mn = a->a_mn_major ? 1 : 0;
   p.b_mn = a->b_mn_major ? 1 : 0;
-  p.block_n = pick_block_n(a->N);
+  p.block_n = pick_block_n(a->N, p.b_mn != 0);
   p.m_blocks = (a->M + kBlockM - 1) / kBlockM;
   p.n_blocks = (a->N + p.block_n - 1) / p.block_n;
   p.num_k_blocks = (a->K + kBlockK - 1) / kBlockK;
@@ -1107,8 +1007,6 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
     return set_error(YAMB_EINVAL, "gate without gate_rows_per_sample");
   if (p.b_gate && !p.b_mn) return set_error(YAMB_EINVAL, "b_gate needs an MN-major B (rows = pixels)");
   p.D = a->D; p.ldd = a->ldd;
-  p.red_vec = (a->epi == 2 && !(reinterpret_cast<uintptr_t>(a->D) & 15) && (a->ldd % 4) == 0) ? 1 : 0;
-  if (p.dbg & 4) p.red_vec = 0;
   if (a->epi == 0 && a->bn_fwd) { p.bnf = *a->bn_fwd; p.has_bnf = 1; }
   if (a->epi == 1) {
     if (!a->H || !a->h_scale || !a->h_shift || !a->bn_bwd)
@@ -1155,7 +1053,8 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   const int Cb = p.b_xform ? (p.b_mn ? p.N : p.K) : 0;
   int fixed = 0;
   // every epilogue warp stages its own 32 x 64 sub-tile: 2 buffers each unless smem is short
-  const int side_bytes = (a->epi == 1) ? kEpiWarps * kWarpOutBytes : 0;  // raw H rows (epi 1)
+  // raw side rows (H of epi 1, the residual of epi 0), one 32-row tile per epilogue warp
+  const int side_bytes = (a->epi == 1 || p.has_residual) ? kEpiWarps * kWarpOutBytes : 0;
   const int coef_bytes = ((a->epi == 1 ? 4 * p.N : 0) + 3 * Ca + 3 * Cb) * 4;
   const int stats_bytes = (p.has_bnf || p.has_bnb) ? 2 * p.N * (int)sizeof(stat_t) : 0;
   const int budget = 232448 - 2048;  // 227 KB minus the kernel's static shared memory
@@ -1238,7 +1137,7 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   p.gA2 = (const __nv_bfloat16*)(p.a_xform == 2 ? a->A2 : nullptr); p.lda2 = a->lda2;
   p.gB2 = (const __nv_bfloat16*)(p.b_xform == 2 ? a->B2 : nullptr); p.ldb2 = a->ldb2;
   if (a->epi != 2) {
-    rc = make_map_2d(&tmD, a->D, a->N, a->M, a->ldd, 64, 32);  // one epilogue warp's rows
+    rc = make_map_2d(&tmD, a->D, a->N, a->M, a->ldd, 64, 16);  // one warp's rows of a 64-row half
     if (rc) return rc;
   }
   if (a->epi == 1) { p.side = (const __nv_bfloat16*)a->H; p.lds = a->ldh; }
@@ -1248,13 +1147,21 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
 
   const int grid = p.num_work < ctas ? p.num_work : ctas;
   cudaError_t e;
+  if (a->epi == 2) {   // split-K partial tiles: released by the reduction below, on this stream
+    rc = det_alloc((size_t)p.num_work * kBlockM * kMaxBlockN * sizeof(float), stream, &p.part);
+    if (rc) return rc;
+  }
+  auto fail = [&](const char* what, cudaError_t err) {
+    if (p.part) det_free(p.part, stream);
+    return set_error(YAMB_ECUDA, "%s: %s", what, cudaGetErrorString(err));
+  };
 #define YAMB_GEMM_LAUNCH(XF, EP, THREADS)                                                         \
   do {                                                                                           \
     static int attr_smem = 0; /* per instantiation, process-wide: only ever RAISE the limit */     \
     if (attr_smem < smem_total) {                                                                \
       e = cudaFuncSetAttribute(gemm_tc_kernel<XF, EP>,                                           \
                                cudaFuncAttributeMaxDynamicSharedMemorySize, smem_total);         \
-      if (e != cudaSuccess) return set_error(YAMB_ECUDA, "smem attr: %s", cudaGetErrorString(e)); \
+      if (e != cudaSuccess) return fail("smem attr", e);                                      \
       attr_smem = smem_total;                                                                    \
     }                                                                                            \
     gemm_tc_kernel<XF, EP><<<grid, THREADS, smem_total, stream>>>(tmA, tmB, tmA2, tmB2, tmD, p); \
@@ -1270,21 +1177,26 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   }
 #undef YAMB_GEMM_LAUNCH
   e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "gemm launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail("gemm launch", e);
+  if (a->epi == 2) {
+    const long long total = (long long)a->M * a->N;
+    const long long cap = 4LL * dev_ctas, blocks = (total + 255) / 256;
+    splitk_reduce_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, stream>>>(
+        p.part, reinterpret_cast<float*>(a->D), a->ldd, a->M, a->N, p.block_n, p.n_blocks, p.ksplit);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return fail("split-K reduce launch", e);
+    rc = det_free(p.part, stream);
+    if (rc) return rc;
+  }
   if (p.dbg & 512) {
     unsigned long long h[16];
     cudaStreamSynchronize(stream);
     cudaMemcpy(h, p.dbg_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    const double n = h[7] ? (double)h[7] : 1.0;
-    fprintf(stderr, "gemm dbg (cycles per epilogue warp): wait_full %.0f tmem_ld %.0f wait_store %.0f "
-            "convert %.0f store %.0f stats %.0f total %.0f warps %.0f\n", h[0] / n, h[1] / n, h[2] / n,
-            h[3] / n, h[4] / n, h[5] / n, h[6] / n, n);
     const double lw_n = h[9] ? (double)h[9] : 1.0;
-    fprintf(stderr, "   per loader warp: wait_empty %.0f wait_tma %.0f xform(incl wait_tma) %.0f publish %.0f total %.0f "
-            "(warps %.0f); per CTA: mma wait_full %.0f wait_tmem_empty %.0f; stages %d out_bufs %d block_n %d "
-            "tma %d%d wg2x %d\n", h[12] / lw_n, h[13] / lw_n, h[14] / lw_n, h[15] / lw_n, h[8] / lw_n, lw_n,
-            h[10] / (double)grid, h[11] / (double)grid, p.num_stages, p.out_bufs, p.block_n, p.a_tma, p.b_tma,
-            p.wg2x);
+    fprintf(stderr, "gemm dbg (cycles per loader warp): wait_empty %.0f wait_tma %.0f xform(incl wait_tma) %.0f "
+            "publish %.0f total %.0f (warps %.0f); stages %d out_bufs %d block_n %d tma %d%d wg2x %d\n",
+            h[12] / lw_n, h[13] / lw_n, h[14] / lw_n, h[15] / lw_n, h[8] / lw_n, lw_n, p.num_stages,
+            p.out_bufs, p.block_n, p.a_tma, p.b_tma, p.wg2x);
   }
   return 0;
 }

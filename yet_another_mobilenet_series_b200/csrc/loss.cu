@@ -1,4 +1,4 @@
-// Label-smoothed softmax cross entropy + top-k correctness on bf16 logits, sm_100a.
+// Label-smoothed softmax cross entropy + top-k correctness on bf16 logits, sm_90a.
 //
 // Replaces, behind yamb_softmax_ce_fwd / yamb_softmax_ce_bwd (include/yamb200.h), the ~20 ATen
 // launches of the reference's loss path per step:
@@ -75,7 +75,8 @@ __global__ void __launch_bounds__(256) softmax_ce_fwd_kernel(const __grid_consta
 }
 
 // dlogits = G * dloss[n]; dbias[c] += column sums.  grid-stride over rows, thread = column pair
-__global__ void __launch_bounds__(256) softmax_ce_bwd_kernel(const __grid_constant__ yamb_softmax_ce_grad a) {
+__global__ void __launch_bounds__(256) softmax_ce_bwd_kernel(const __grid_constant__ yamb_softmax_ce_grad a,
+                                                                      float* part) {
   const int CP = a.C / 2;
   for (int cp = threadIdx.x; cp < CP; cp += 256) {
     float b0 = 0.f, b1 = 0.f;
@@ -88,16 +89,16 @@ __global__ void __launch_bounds__(256) softmax_ce_bwd_kernel(const __grid_consta
       b0 += bf16lo(o);
       b1 += bf16hi(o);
     }
-    if (a.dbias) {
-      atomicAdd(a.dbias + 2 * cp, b0);
-      atomicAdd(a.dbias + 2 * cp + 1, b1);
+    if (part) {   // per-CTA column sums, added in CTA order by det_reduce_launch
+      part[(size_t)blockIdx.x * a.C + 2 * cp] = b0;
+      part[(size_t)blockIdx.x * a.C + 2 * cp + 1] = b1;
     }
   }
 }
 
 // out[c] += sum_rows X[row][c]   (classifier bias gradient: column sums of dlogits)
 __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* X, long long M, int C,
-                                                          long long ld, float* out) {
+                                                          long long ld, float* part) {
   const int CP = C / 2;
   for (int cp = blockIdx.x * 256 + threadIdx.x; cp < CP; cp += gridDim.x * 256) {
     float b0 = 0.f, b1 = 0.f;
@@ -106,8 +107,8 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* X
       b0 += bf16lo(v);
       b1 += bf16hi(v);
     }
-    atomicAdd(out + 2 * cp, b0);
-    atomicAdd(out + 2 * cp + 1, b1);
+    part[(size_t)blockIdx.y * C + 2 * cp] = b0;     // row-slab sums, added in slab order
+    part[(size_t)blockIdx.y * C + 2 * cp + 1] = b1;
   }
 }
 
@@ -116,10 +117,16 @@ int colsum_bf16_launch(const void* X, long long M, int C, long long ld, float* o
     return set_error(YAMB_EINVAL, "colsum args (C and ld must be even)");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   dim3 grid((C / 2 + 255) / 256, (unsigned)(M < 32 ? M : 32));
-  colsum_bf16_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)X, M, C, ld, out);
+  float* part = nullptr;
+  int rc = det_alloc((size_t)grid.y * C * sizeof(float), st, &part);
+  if (rc) return rc;
+  colsum_bf16_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)X, M, C, ld, part);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "colsum: %s", cudaGetErrorString(e));
-  return 0;
+  if (e != cudaSuccess) {
+    det_free(part, st);
+    return set_error(YAMB_ECUDA, "colsum: %s", cudaGetErrorString(e));
+  }
+  return det_reduce_launch(part, (int)grid.y, C, out, st);
 }
 
 int softmax_ce_fwd_launch(const yamb_softmax_ce* a, cudaStream_t st) {
@@ -139,7 +146,16 @@ int softmax_ce_bwd_launch(const yamb_softmax_ce_grad* a, cudaStream_t st) {
     return set_error(YAMB_EINVAL, "softmax_ce bwd args (C and pitches must be even)");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   int grid = a->N < 2 * max_ctas() ? a->N : 2 * max_ctas();
-  softmax_ce_bwd_kernel<<<grid, 256, 0, st>>>(*a);
+  float* part = nullptr;
+  if (a->dbias) {
+    const int rc = det_alloc((size_t)grid * a->C * sizeof(float), st, &part);
+    if (rc) return rc;
+  }
+  softmax_ce_bwd_kernel<<<grid, 256, 0, st>>>(*a, part);
+  if (a->dbias) {
+    const int rc = det_reduce_launch(part, grid, a->C, a->dbias, st);
+    if (rc) return rc;
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "softmax_ce bwd: %s", cudaGetErrorString(e));
   return 0;

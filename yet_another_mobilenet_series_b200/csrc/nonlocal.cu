@@ -1,4 +1,4 @@
-// Lightweight non-local block (AutoNL) core on NHWC bf16 activations, sm_100a.
+// Lightweight non-local block (AutoNL) core on NHWC bf16 activations, sm_90a.
 //
 // Replaces, behind yamb_nl_gram / yamb_nl_rowmat (include/yamb200.h), the two einsums of
 // Nonlocal.forward (reference models/mobilenet_base.py:158-173) and their autograd backward:

@@ -1,4 +1,4 @@
-// Fused flat-arena optimizer step, sm_100a.  One launch replaces the ~7 ATen launches per tensor
+// Fused flat-arena optimizer step, sm_90a.  One launch replaces the ~7 ATen launches per tensor
 // of the reference's Python-loop RMSprop (utils/rmsprop.py:67-129), the L2 penalty's autograd
 // graph (utils/optim.py:177-200, folded as grad += wd[i]*p), the DDP mean (utils/distributed.py:136,
 // folded as grad_scale = 1/world), the EMA update (utils/optim.py:53-64) and the fp32->bf16 weight

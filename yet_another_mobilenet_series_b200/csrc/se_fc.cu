@@ -1,4 +1,4 @@
-// Squeeze-and-Excitation fully connected layers on the pooled [N, C] vectors, sm_100a.
+// Squeeze-and-Excitation fully connected layers on the pooled [N, C] vectors, sm_90a.
 //
 // Replaces, behind yamb_se_fc_fwd / yamb_se_fc_bwd (include/yamb200.h), the two 1x1 convolutions
 // on [N, C, 1, 1] of SqueezeAndExcitation.forward and the sigmoid

@@ -1,5 +1,5 @@
 // Stem convolution: 3x3, stride 2, pad 1, 3 input channels (RGB) -> Cout (<= 64, multiple of 8)
-// on NHWC bf16, sm_100a.
+// on NHWC bf16, sm_90a.
 //
 // Replaces, behind yamb_stem_conv_fwd / yamb_stem_conv_wgrad (include/yamb200.h), the cuDNN
 // implicit-GEMM forward / weight-gradient kernels (and the nhwcAddPadding copies cuDNN needs for a
@@ -32,6 +32,7 @@ struct StemDev {
   __nv_bfloat16* y;           // [N][Ho][Wo][Cout]        (forward)
   const __nv_bfloat16* dh;    // [N][Ho][Wo][Cout]        (wgrad)
   float* dw;                  // [Cout][3][3][3] +=       (wgrad)
+  float* part;                // [CTA x pixel subset][Cout][27] wgrad partials
   int tiles_h, tiles_w, num_tiles;
 };
 
@@ -111,7 +112,7 @@ __global__ void __launch_bounds__(256) stem_fwd_kernel(const __grid_constant__ S
       }
     }
     __syncthreads();
-    // 3 x 5 x 3 input patch of this thread's two output pixels, as (a, a) pairs for FFMA2
+    // 3 x 5 x 3 input patch of this thread's two output pixels, as (a, a) pairs for the pair FMAs
     float in[3][5][3];
 #pragma unroll
     for (int a = 0; a < 3; ++a)
@@ -168,7 +169,7 @@ __global__ void __launch_bounds__(256) stem_fwd_kernel(const __grid_constant__ S
 }
 
 // wgrad: thread = (8 output channels co8, 4 positions jq, pixel subset ps): 256 threads =
-// (Cout/8) x 8 x PS.  32 FMAs (16 FFMA2) per 2 + 4 shared-memory loads.  Positions are walked in
+// (Cout/8) x 8 x PS.  32 FMAs per 2 + 4 shared-memory loads.  Positions are walked in
 // staging order jj = (ky*3 + kx)*3 + ci and mapped to the parameter's j = ci*9 + ky*3 + kx at the end.
 __global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__ StemDev p) {
   extern __shared__ __align__(16) unsigned char stem_smem[];
@@ -243,11 +244,12 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__
     if (jj < 27) {
       const int tap = jj / 3, ci = jj % 3;
       const int j = ci * 9 + tap;
-      float* d = p.dw + (size_t)(8 * co8) * 27 + j;
+      // partial of (CTA, pixel subset): every slot gets all Cout x 27 values; added in slot order
+      float* d = p.part + ((size_t)blockIdx.x * PS + ps) * (p.Cout * 27) + (size_t)(8 * co8) * 27 + j;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        atomicAdd(d + (2 * e) * 27, acc[k][e].x);
-        atomicAdd(d + (2 * e + 1) * 27, acc[k][e].y);
+        d[(2 * e) * 27] = acc[k][e].x;
+        d[(2 * e + 1) * 27] = acc[k][e].y;
       }
     }
   }
@@ -320,7 +322,13 @@ int stem_conv_wgrad_launch(const yamb_stem_conv* a, cudaStream_t st) {
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_w, stem_wgrad_kernel, 256, smem) != cudaSuccess)
     per_sm_w = 2;
   const int res_w = max_ctas() * (per_sm_w > 0 ? per_sm_w : 1);
-  stem_wgrad_kernel<<<p.num_tiles < res_w ? p.num_tiles : res_w, 256, smem, st>>>(p);
+  const int grid = p.num_tiles < res_w ? p.num_tiles : res_w;
+  const int slots = grid * (256 / p.Cout);
+  rc = det_alloc((size_t)slots * p.Cout * 27 * sizeof(float), st, &p.part);
+  if (rc) return rc;
+  stem_wgrad_kernel<<<grid, 256, smem, st>>>(p);
+  if (cudaPeekAtLastError() != cudaSuccess) det_free(p.part, st);
+  else if ((rc = det_reduce_launch(p.part, slots, (long long)p.Cout * 27, p.dw, st)) != 0) return rc;
   e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv wgrad: %s", cudaGetErrorString(e));
   return 0;

@@ -4,7 +4,7 @@ copied to the GPU on a side stream while the current step computes, and `__next_
 device tensors after making the compute stream wait for that copy.
 
 Differences from the reference, all on the device side:
-  * the batch lands directly in the layout and dtype the sm_100a kernels consume — bf16,
+  * the batch lands directly in the layout and dtype the sm_90a kernels consume — bf16,
     channels_last — in ONE copy kernel (the reference uploads fp32 NCHW and calls `.float()`;
     its cuDNN path then converts per layer);
   * host batches should be pinned (`pin_memory=True` in the DataLoader) for the copy to overlap;

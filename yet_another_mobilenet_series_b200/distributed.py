@@ -1,5 +1,5 @@
 """Data-parallel plumbing with the surface of the reference's `utils/distributed.py`, one process
-per GPU over NCCL (NVLink 5 / NVSwitch on one B200 box).
+per GPU over NCCL (NVLink / NVSwitch inside one node).
 
 The data path of the reference has exactly one exchange step per iteration: the SUM all-reduce of
 all gradients followed by a division by the world size (utils/distributed.py:131-139, called from

@@ -1,4 +1,4 @@
-"""Host-side sequencing of the sm_100a kernels for one inverted-residual block.
+"""Host-side sequencing of the sm_90a kernels for one inverted-residual block.
 
 A `BlockPlan` owns the HBM-resident intermediates of one block for one input shape
 (NHWC bf16 [pixels, channels] matrices) and the pre-built C-ABI argument structs; `block_apply`
@@ -222,7 +222,7 @@ class BlockPlan:
         self.Chid = sum(self.channels)
         if self.Cin % 8 or self.Cout % 8 or any(c % 8 for c in self.channels):
             raise nat.NativeError(
-                "channel counts must be multiples of 8 for the sm_100a path "
+                "channel counts must be multiples of 8 for the sm_90a path "
                 "(inp=%d oup=%d hidden=%s)" % (self.Cin, self.Cout, self.channels))
         if not self.expand and not self.fused and len(self.channels) > 1:
             raise nat.NativeError("expand=False with several branches is not supported")
@@ -264,7 +264,7 @@ class BlockPlan:
             nl = self.nl
             if not isinstance(nl.bn, torch.nn.BatchNorm2d):
                 raise nat.NativeError("non-local block: only the BatchNorm nl_norm is on the "
-                                      "sm_100a path (got %s)" % type(nl.bn).__name__)
+                                      "sm_90a path (got %s)" % type(nl.bn).__name__)
             self.nl_cr = int(nl.nl_c * Cout)        # theta / phi channels (:163)
             self.nl_sub = int(nl.nl_s)
             if self.nl_cr <= 0 or self.nl_cr % 2 or self.nl_sub < 1:
@@ -871,7 +871,7 @@ def block_params(block):
 
 
 class _BlockFn(torch.autograd.Function):
-    """autograd boundary of the fused block: forward/backward run the sm_100a kernel sequences.
+    """autograd boundary of the fused block: forward/backward run the sm_90a kernel sequences.
 
     Parameter gradients: when a parameter carries a pre-allocated fp32 `.grad` that the flat-arena
     optimizer marked with `_yamb_direct` the kernels accumulate straight into it and autograd gets
@@ -1421,10 +1421,10 @@ def fused_eval_forward(block, x):
 
 
 def block_apply(block, x):
-    """Forward of a reference-compatible block module through the sm_100a path."""
+    """Forward of a reference-compatible block module through the sm_90a path."""
     if not x.is_cuda:
         raise nat.NativeError(
-            "the inverted-residual block runs only on CUDA sm_100a (no CPU fallback); got a %s "
+            "the inverted-residual block runs only on CUDA sm_90a (no CPU fallback); got a %s "
             "tensor" % x.device)
     x = to_nhwc_bf16(x)
     if fused_eval_supported(block, x):

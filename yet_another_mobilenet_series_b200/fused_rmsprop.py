@@ -1,4 +1,4 @@
-"""Fused flat-arena RMSprop for sm_100a with the surface of the reference's `utils/rmsprop.py`.
+"""Fused flat-arena RMSprop for sm_90a with the surface of the reference's `utils/rmsprop.py`.
 
 Drop-in contract (SURVEY.md §8b): `torch.optim.Optimizer` subclass, constructor
 `(params, lr=1e-2, alpha=0.99, eps=1e-8, eps_inside_sqrt=False, weight_decay=0, momentum=0,

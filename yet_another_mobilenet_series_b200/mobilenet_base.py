@@ -1,5 +1,5 @@
 """Block library with the module surface of the reference's `models/mobilenet_base.py`, backed by
-the sm_100a kernels.
+the sm_90a kernels.
 
 Drop-in contract (SURVEY.md §8b): same class names, constructor signatures, attributes, child
 module names and therefore the same `state_dict()` keys/shapes, the same helper methods
@@ -171,7 +171,7 @@ class ConvBNReLU(nn.Sequential):
             active_fn())
 
     def forward(self, x):
-        # CUDA: a 1x1 convolution (the head 320 -> 1280) is the blocks' tcgen05 GEMM with the
+        # CUDA: a 1x1 convolution (the head 320 -> 1280) is the blocks' wgmma GEMM with the
         # BatchNorm statistics in its epilogue (tail_ops.pw_conv_bn_act); the 3x3 stride-2 stem
         # runs the direct kernels of tail_ops.stem_conv_bn_act; any other convolution stays a
         # library call with BatchNorm + activation on this repo's kernels.  CPU / odd widths: the

@@ -2,7 +2,7 @@
 `models/mobilenet_supernet.py` (:59-176): same constructor keywords (so
 `apps/mobilenet/models/*.yml` load unchanged through `model: <this module>`,
 reference common.py:129-130), same module tree / state_dict keys.  The inverted-residual blocks
-come from `mobilenet_base.get_block` and run on the sm_100a kernels; activations flow between
+come from `mobilenet_base.get_block` and run on the sm_90a kernels; activations flow between
 blocks as channels_last bf16."""
 import numbers
 
@@ -71,7 +71,7 @@ def run_features(model, x):
 
 
 def run_classifier(classifier, x):
-    """Dropout -> Linear (reference :163-167); the Linear runs on the tcgen05 GEMM when its
+    """Dropout -> Linear (reference :163-167); the Linear runs on the wgmma GEMM when its
     widths allow (tail_ops.linear_apply), else as the torch module."""
     from . import tail_ops
     for layer in classifier:

@@ -1,6 +1,6 @@
 """Searched-network builder with the surface of the reference's `models/searched_network.py`
 (:13-139): rows are `[c, n, s, ks, hiddens, expand]` with explicit hidden widths, optional global
-`se_ratio` (fused block only).  Same module tree / state_dict keys; blocks run on sm_100a."""
+`se_ratio` (fused block only).  Same module tree / state_dict keys; blocks run on sm_90a."""
 import warnings
 
 from torch import nn

@@ -1,11 +1,11 @@
-"""The layers around the inverted-residual stack on the sm_100a path (SURVEY.md §8f-2):
+"""The layers around the inverted-residual stack on the sm_90a path (SURVEY.md §8f-2):
 
   head   ConvBNReLU 1x1 (320 -> 1280)      reference models/mobilenet_supernet.py:152-158
   fc     nn.Linear (1280 -> classes)       reference models/mobilenet_supernet.py:163-167
   loss   CrossEntropyLabelSmooth + top-k   reference utils/optim.py:150-158, common.py:67-80
 
 A 1x1 convolution on NHWC activations and a Linear layer are the same [pixels, Cin] x [Cout, Cin]^T
-GEMM the blocks already use (`yamb_pointwise_gemm`, tcgen05): forward with the BatchNorm
+GEMM the blocks already use (`yamb_pointwise_gemm`, wgmma): forward with the BatchNorm
 statistics in the epilogue, dgrad with the weight read MN-major, wgrad as split-K with pixels on
 K.  The loss is one kernel forward / one backward (`yamb_softmax_ce_*`).  Round 1 ran all of these
 through cuDNN / cuBLAS / ~20 ATen launches.
@@ -165,7 +165,7 @@ class _PwConvBnActFn(torch.autograd.Function):
                       b_mn_major=1)
             engine.launch(lib.yamb_pointwise_gemm, g, "head_conv_dgrad", 2 * M * (Cin + Cout),
                           2 * M * Cin * Cout)
-        # wgrad: dW[Cout, Cin] += dh^T x   (pixels on K, split-K, fp32 vector reductions)
+        # wgrad: dW[Cout, Cin] += dh^T x   (pixels on K, split-K, slabs added in a fixed order)
         g2 = _gemm(Cout, Cin, M, dh.data_ptr(), Cout, xm.data_ptr(), Cin, gw.data_ptr(), Cin,
                    a_mn_major=1, b_mn_major=1, epi=2)
         engine.launch(lib.yamb_pointwise_gemm, g2, "head_conv_wgrad", 2 * M * (Cin + Cout),
@@ -266,7 +266,7 @@ class _LinearFn(torch.autograd.Function):
 
 
 def linear_apply(lin, x):
-    """nn.Linear on CUDA through the tcgen05 GEMM (in/out features multiples of 8)."""
+    """nn.Linear on CUDA through the wgmma GEMM (in/out features multiples of 8)."""
     if x.dtype != torch.bfloat16 or not x.is_contiguous():
         x = x.to(torch.bfloat16).contiguous()
     return _LinearFn.apply(x, lin, lin.weight, lin.bias)

@@ -1,4 +1,4 @@
-"""Public training-step API of the sm_100a path: `TrainStep(model, ...)(x, target)`.
+"""Public training-step API of the sm_90a path: `TrainStep(model, ...)(x, target)`.
 
 One call = one iteration of the reference's hot loop (train.py:64-114): zero_grad, forward,
 label-smoothed cross entropy (utils/optim.py:150-158) [+ top-k counts without the reference's two
