@@ -245,6 +245,7 @@ typedef struct yamb_se_fc {
   const float* w_e; const float* b_e;      /* [C][R], [C]  (se_expand) */
   float* u; float* v;                      /* out [N][R]: saved for backward */
   float* gate;                             /* out [N][C] */
+  int32_t deterministic;                   /* 1: no split-K over C (the same bits on every run) */
 } yamb_se_fc;
 
 typedef struct yamb_se_fc_grad {
@@ -285,6 +286,8 @@ typedef struct yamb_nl_gram {
   const void* Y; int64_t ldy; int32_t J;   /* J, ldy even */
   float alpha;
   float* G;                                /* [N][I][J] */
+  int32_t deterministic;                   /* 1: per-CTA partial sums added in a fixed order
+                                            * (the same bits on every run); 0: fp32 atomics */
 } yamb_nl_gram;
 
 typedef struct yamb_nl_rowmat {
@@ -359,7 +362,14 @@ int yamb_colsum_bf16(const void* X, int64_t M, int32_t C, int64_t ld, float* out
  * 64-channel slices of the hidden dimension) -> BN3 (+x) -> y.  The BatchNorm folding
  * scale = gamma*rsqrt(var+eps), shift = beta - mean*scale is done inside the kernel from the
  * module's buffers (csrc/block_eval.cu).  Shapes it does not cover return YAMB_EINVAL; the caller
- * then runs the four-launch sequence with folded coefficients. */
+ * then runs the four-launch sequence with folded coefficients.
+ *
+ * Squeeze-and-Excitation (InvertedResidualChannelsFused, reference :110-113, :336-339) takes three
+ * calls: yamb_block_eval_pool_fwd writes pooled[n][c], the spatial mean of a2 = bf16(act(bn2(h2)))
+ * (it recomputes expand -> BN1+act -> stencil -> BN2+act per tile and stops there: no project, no
+ * hidden tensor in HBM; per-tile partial sums added in a fixed order, the same bits on every run;
+ * bn3, w_project and y are not read); yamb_se_fc_fwd turns pooled into the gate; yamb_block_eval_fwd
+ * with `gate` set feeds a2s = bf16(a2 * gate[n][c]) to the project MMAs. */
 typedef struct yamb_bn_eval {
   const float* gamma;         /* [C] or NULL (=1) */
   const float* beta;          /* [C] or NULL (=0) */
@@ -371,7 +381,7 @@ typedef struct yamb_bn_eval {
 typedef struct yamb_block_eval {
   int32_t N, H, W;            /* input pixels (NHWC); output (H-1)/stride+1 x (W-1)/stride+1 */
   int32_t Cin, Chid, Cout;    /* multiples of 8; Cin <= 256, Cout <= 320 */
-  int32_t kernel, stride;     /* 3, 5 or 7 (5 / 7: with expansion, relu / relu6); 1 or 2 */
+  int32_t kernel, stride;     /* 3, 5 or 7 (5 / 7: with expansion); 1 or 2 */
   int32_t act;                /* YAMB_ACT_* of the two inner activations */
   int32_t residual;           /* y += x (needs Cin == Cout, stride 1) */
   const void* x;              /* bf16 [N,H,W,Cin] */
@@ -380,9 +390,12 @@ typedef struct yamb_block_eval {
   const void* w_project;      /* bf16 [Cout][Chid] */
   yamb_bn_eval bn1, bn2, bn3; /* over Chid, Chid, Cout channels */
   void* y;                    /* bf16 [N,Ho,Wo,Cout] */
+  const float* gate;          /* fp32 [N][Chid] SE gate applied to a2 before the project, or NULL */
+  float* pooled;              /* pool pass: out fp32 [N][Chid] spatial mean of a2 */
 } yamb_block_eval;
 
 int yamb_block_eval_fwd(const yamb_block_eval* args, yamb_stream_t stream);
+int yamb_block_eval_pool_fwd(const yamb_block_eval* args, yamb_stream_t stream);
 
 /* ---- fused flat-arena RMSprop (+L2 decay, +DDP mean, +EMA, +bf16 repack) -------------------------
  * Replaces RMSprop.step (reference utils/rmsprop.py:67-129), the gradient of cal_l2_loss

@@ -105,6 +105,7 @@ int yamb_stem_conv_wgrad(const yamb_stem_conv* a, yamb_stream_t s) { return yamb
 int yamb_nl_gram_fwd(const yamb_nl_gram* a, yamb_stream_t s) { return yamb::nl_gram_launch(a, YAMB_ST(s)); }
 int yamb_nl_rowmat_fwd(const yamb_nl_rowmat* a, yamb_stream_t s) { return yamb::nl_rowmat_launch(a, YAMB_ST(s)); }
 int yamb_block_eval_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_launch(a, YAMB_ST(s)); }
+int yamb_block_eval_pool_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_pool_launch(a, YAMB_ST(s)); }
 int yamb_rmsprop_step(const yamb_rmsprop* a, yamb_stream_t s) { return yamb::rmsprop_launch(a, YAMB_ST(s)); }
 int yamb_ema_update(float* shadow, const float* x, int64_t n, const float* hyper, float m,
                     yamb_stream_t s) {

@@ -21,6 +21,10 @@
 //   BatchNorm3 (+ x) -> bf16 -> global                                                 epilogue 2
 // Blocks without the 1x1 expansion (hidden == input) skip the first MMA: the x panel itself is the
 // stencil input.
+// Squeeze-and-Excitation (InvertedResidualChannelsFused, reference mobilenet_base.py:336-339) is the
+// MODE template flag: kGate multiplies a2 by gate[n][c] before the project; kPool (the pool pass,
+// yamb_block_eval_pool_fwd) runs the same tile walk up to a2 and writes per-tile spatial means
+// instead of the project (see the enum below).
 // HBM traffic: x once (+ halo re-reads from L2), y once; the hidden tensors (6 x the block's
 // input) never leave the SM.  BatchNorm folding (gamma * rsqrt(var + eps), beta - mean * scale) is
 // done by the kernel from the module's own buffers: no preparation launches.
@@ -37,7 +41,8 @@
 //
 // Rounding points: a1 = bf16(act(bn1(fp32 accumulator))), a2 = bf16(act(bn2(fp32 stencil))),
 // y = bf16(bn3(fp32 accumulator) + x) — one rounding fewer per stage than the four-launch path
-// (which stores the raw convolution outputs in bf16 first).
+// (which stores the raw convolution outputs in bf16 first); with the gate a2s = bf16(a2 * gate),
+// pooled = fp32 mean of the bf16 a2.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -70,7 +75,18 @@ struct BlockEvalDev {
   int NC;            // 64-channel slices of the hidden dimension
   int xpanel_bytes;  // bytes between the 64-channel panels of the x tile
   int off_w1, off_w3, off_h1, off_h2, off_tab, off_c3, off_bars;
+  const float* gate; // kGate: [N][Chid] Squeeze-and-Excitation gate
+  float* part;       // kPool: [tiles_h * tiles_w][N][Chid] per-tile partial means
+  float inv_hw;      // kPool: 1 / (Ho * Wo)
+  int mode;          // kPlain / kGate / kPool (host-side dispatch; the kernel has it as MODE)
 };
+
+// What one launch computes:
+//   kPlain  y = bn3(project(a2)) (+ x)
+//   kGate   y = bn3(project(a2s)) (+ x),  a2s = bf16(a2 * gate[n][c])   (Squeeze-and-Excitation)
+//   kPool   no project: every tile writes the spatial sums of a2 over its output pixels inside the
+//           image, times 1 / (Ho * Wo), to its own slab of `part` (det_reduce adds the slabs)
+enum { kPlain = 0, kGate = 1, kPool = 2 };
 
 constexpr int kMaxProjChunks = 10;   // 16-column project accumulators per thread (80 registers)
 
@@ -98,10 +114,11 @@ struct EvGeom {
                 "tile geometry (warp 7 must stay free of stencil work)");
 };
 
-template <class G, bool EXPAND, bool LEAN>
+template <class G, bool EXPAND, bool LEAN, int MODE>
 __global__ void __launch_bounds__(256, 1)
 block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW1,
                   const __grid_constant__ CUtensorMap tmW3, const __grid_constant__ BlockEvalDev p) {
+  constexpr bool POOL = MODE == kPool, GATE = MODE == kGate;
   constexpr int K = G::K, P = G::P, kTabFloats = tab_floats(G::K);
   constexpr int S = G::S, TOH = G::TOH, TOW = G::TOW, TI = G::TI, IH = G::IH, IW = G::IW;
   constexpr int NPI = G::NPI, NPO = G::NPO, RUN = G::RUN, NRUN = G::NRUN, CPT = G::CPT, NCG = G::NCG;
@@ -123,7 +140,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     mbar_init(bar_w3, 1);
     fence_barrier_init();
   }
-  for (int i = tid; i < p.Npad; i += 256) {
+  for (int i = tid; i < (POOL ? 0 : p.Npad); i += 256) {
     float sc = 0.f, sh = 0.f;
     if (i < p.Cout) {
       const float r = rsqrtf(p.bn3.var[i] + p.bn3.eps);
@@ -139,7 +156,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
   if (control) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW1);
-    tma_prefetch_desc(&tmW3);
+    if (!POOL) tma_prefetch_desc(&tmW3);
   }
   fence_proxy_async_smem();
   __syncthreads();
@@ -308,9 +325,11 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       if (warp == 7) {
         // ---- control: W3 slice in; the next slice's W1 (and the next tile's x) in ----
         if (lane == 0) {
-          mbar_arrive_expect_tx(bar_w3, (uint32_t)(p.Npad * 128));
-          for (int h = 0; h < p_halves; ++h)
-            tma_load_2d(&tmW3, bar_w3, smem + p.off_w3 + h * p_nn * 128, c * 64, h * p_nn);
+          if (!POOL) {
+            mbar_arrive_expect_tx(bar_w3, (uint32_t)(p.Npad * 128));
+            for (int h = 0; h < p_halves; ++h)
+              tma_load_2d(&tmW3, bar_w3, smem + p.off_w3 + h * p_nn * 128, c * 64, h * p_nn);
+          }
           if (EXPAND) {
             if (has_next) {
               mbar_arrive_expect_tx(bar_ld, (uint32_t)(p.KB * (8192 + (last_c ? NPI * 128 : 0))));
@@ -374,6 +393,21 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           s2v[v] = *reinterpret_cast<const float2*>(tb + 128 + cg * CPT + 2 * v);
           t2v[v] = *reinterpret_cast<const float2*>(tb + 192 + cg * CPT + 2 * v);
         }
+        // the image of this run's outputs (TI = 2: the second image of the last tile may be past N)
+        const int s_n = g * TI + s_ti;
+        float2 gv[NV];                       // kGate: gate of this run's image, 0 past N / Chid
+        if (GATE) {
+          const int hc = c * 64 + cg * CPT;  // CPT | 8 | Chid: all CPT channels in range, or none
+          const bool ok = s_n < p.N && hc < p.Chid;
+#pragma unroll
+          for (int v = 0; v < NV; ++v)
+            gv[v] = ok ? make_float2(__ldg(p.gate + (size_t)s_n * p.Chid + hc + 2 * v),
+                                     __ldg(p.gate + (size_t)s_n * p.Chid + hc + 2 * v + 1))
+                       : make_float2(0.f, 0.f);
+        }
+        float2 ps[NV];                       // kPool: sums of a2 over this run's outputs in the image
+#pragma unroll
+        for (int v = 0; v < NV; ++v) ps[v] = make_float2(0.f, 0.f);
         const int boff = cg * CPT * 2;       // byte offset of this thread's channels inside a row
 #pragma unroll
         for (int j = 0; j < RUN; ++j) {
@@ -388,16 +422,45 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
               act_vec<2>(qq, ap);
               wv[v] = pack_bf16(qq[0], qq[1]);
             }
+            if (GATE) wv[v] = pack_bf16(bf16lo(wv[v]) * gv[v].x, bf16hi(wv[v]) * gv[v].y);
           }
-          const int r = r0 + j;
-          uint8_t* dst = sH2 + r * 128 + (((boff >> 4) ^ (r & 7)) << 4) + (boff & 15);
-          if (CPT == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(wv[0], wv[NV - 1]);
-          else *reinterpret_cast<uint32_t*>(dst) = wv[0];
+          if (POOL) {
+            const bool in = s_n < p.N && ty * TOH + s_oy < p.Ho && tx * TOW + s_ox0 + j < p.Wo;
+#pragma unroll
+            for (int v = 0; v < NV; ++v)
+              if (in) ps[v] = make_float2(ps[v].x + bf16lo(wv[v]), ps[v].y + bf16hi(wv[v]));
+          } else {
+            const int r = r0 + j;
+            uint8_t* dst = sH2 + r * 128 + (((boff >> 4) ^ (r & 7)) << 4) + (boff & 15);
+            if (CPT == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(wv[0], wv[NV - 1]);
+            else *reinterpret_cast<uint32_t*>(dst) = wv[0];
+          }
+        }
+        if (POOL) {   // -> red[sp][channel] (the sH2 buffer, unused without the project MMAs)
+#pragma unroll
+          for (int v = 0; v < NV; ++v)
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(sH2) + sp * 64 + cg * CPT + 2 * v) = ps[v];
         }
       }
       if (has_next) tab_store(tab + ((gc + 1) & 1) * kTabFloats);   // its readers are behind S3
       fence_proxy_async_smem();
       __syncthreads();                                                     // S3: a2 tile complete
+      if (POOL) {
+        // ---- pool: per (image, channel) of the slice, the stencil threads' sums in run order ->
+        //      this tile's slab; red is rewritten only after the next S2 ----
+        constexpr int RPI = TOH * TOW / RUN;     // runs per image
+        if (tid < TI * 64) {
+          const int ti = tid >> 6, ch = tid & 63;
+          const float* red = reinterpret_cast<const float*>(sH2);
+          float s = 0.f;
+#pragma unroll 1
+          for (int r = ti * RPI; r < (ti + 1) * RPI; ++r) s += red[r * 64 + ch];
+          const int n = g * TI + ti, hc = c * 64 + ch;
+          if (n < p.N && hc < p.Chid)
+            p.part[((size_t)(ty * p.tiles_w + tx) * p.N + n) * p.Chid + hc] = s * p.inv_hw;
+        }
+        continue;
+      }
       // ---- project(c): [64 px x 64] x [64 x 16 j], accumulated over the slices, left in flight ----
       mbar_wait(bar_w3, w3_par);       // landed during the stencil
       w3_par ^= 1;
@@ -412,6 +475,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       }
       wgmma_commit();
     }
+    if (POOL) continue;
     // ---- epilogue 2: y = bf16(bn3(h3) (+ x)) ----
     wgmma_wait<0>();
     reg_fence(pacc);
@@ -460,7 +524,7 @@ static int make_map(CUtensorMap* map, const void* ptr, int rank, const cuuint64_
   return 0;
 }
 
-template <class G, bool EXPAND, bool LEAN>
+template <class G, bool EXPAND, bool LEAN, int MODE>
 static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream_t st) {
   // ---- shared-memory plan (bytes from the 1024-aligned base) ----
   // x tile: NPI rows of 128 B per 64-channel panel; the last 64-row MMA chunk of a panel reads
@@ -498,6 +562,7 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
     if (rc) return rc;
   }
   memset(&tmW1, 0, sizeof(tmW1));
+  memset(&tmW3, 0, sizeof(tmW3));
   if (EXPAND) {
     const cuuint64_t dims[2] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Chid};
     const cuuint64_t str[1] = {(cuuint64_t)p.Cin * 2};
@@ -505,7 +570,7 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
     int rc = make_map(&tmW1, a->w_expand, 2, dims, str, box);
     if (rc) return rc;
   }
-  {
+  if (MODE != kPool) {
     const int halves = p.Npad > 256 ? 2 : 1;
     const cuuint64_t dims[2] = {(cuuint64_t)p.Chid, (cuuint64_t)p.Cout};
     const cuuint64_t str[1] = {(cuuint64_t)p.Chid * 2};
@@ -519,10 +584,11 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
   {
     std::lock_guard<std::mutex> lock(mu);
     if (attr < smem) {
-      cudaError_t e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN>,
+      cudaError_t e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN, MODE>,
                                            cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN, MODE>,
+                                 cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared);
       if (e != cudaSuccess) return set_error(YAMB_ECUDA, "block_eval attr: %s", cudaGetErrorString(e));
       attr = smem;
@@ -534,22 +600,49 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
   const int grid = (int)(p.num_tiles < cap ? p.num_tiles : cap);
   static const bool dbg = getenv("YAMB_EVAL_DEBUG") != nullptr;
   if (dbg)
-    fprintf(stderr, "block_eval: tiles %d grid %d smem %d Npad %d NC %d KB %d\n",
-            p.num_tiles, grid, smem, p.Npad, p.NC, p.KB);
-  block_eval_kernel<G, EXPAND, LEAN><<<grid, 256, smem, st>>>(tmX, tmW1, tmW3, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "block_eval launch: %s", cudaGetErrorString(e));
-  return 0;
+    fprintf(stderr, "block_eval: mode %d tiles %d grid %d smem %d Npad %d NC %d KB %d\n",
+            MODE, p.num_tiles, grid, smem, p.Npad, p.NC, p.KB);
+  if (MODE != kPool) {
+    block_eval_kernel<G, EXPAND, LEAN, MODE><<<grid, 256, smem, st>>>(tmX, tmW1, tmW3, p);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "block_eval launch: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  // pool pass: one slab of N x Chid partial means per spatial tile position, every element
+  // written by exactly one tile; pooled = 0, then += the slabs in slab order (deterministic)
+  const int nslab = p.tiles_h * p.tiles_w;
+  const long long n_out = (long long)p.N * p.Chid;
+  int rc = det_alloc((size_t)nslab * n_out * sizeof(float), st, &p.part);
+  if (rc) return rc;
+  p.inv_hw = 1.f / ((float)p.Ho * (float)p.Wo);
+  cudaError_t e = cudaMemsetAsync(a->pooled, 0, (size_t)n_out * sizeof(float), st);
+  if (e == cudaSuccess) {
+    block_eval_kernel<G, EXPAND, LEAN, MODE><<<grid, 256, smem, st>>>(tmX, tmW1, tmW3, p);
+    e = cudaGetLastError();
+  }
+  if (e != cudaSuccess) {
+    det_free(p.part, st);
+    return set_error(YAMB_ECUDA, "block_eval pool launch: %s", cudaGetErrorString(e));
+  }
+  return det_reduce_launch(p.part, nslab, n_out, a->pooled, st);
+}
+
+template <class G, bool EXPAND, int MODE>
+static int launch_eval_mode(BlockEvalDev& p, const yamb_block_eval* a, cudaStream_t st) {
+  // relu / relu6 / none are clamps of the packed bf16 pair; swish / h-swish take the generic path
+  const bool lean = a->act == YAMB_ACT_NONE || a->act == YAMB_ACT_RELU || a->act == YAMB_ACT_RELU6;
+  return lean ? launch_eval_act<G, EXPAND, true, MODE>(p, a, st)
+              : launch_eval_act<G, EXPAND, false, MODE>(p, a, st);
 }
 
 template <class G, bool EXPAND>
 static int launch_eval(BlockEvalDev& p, const yamb_block_eval* a, cudaStream_t st) {
-  // relu / relu6 / none are clamps of the packed bf16 pair; swish / h-swish take the generic path
-  const bool lean = a->act == YAMB_ACT_NONE || a->act == YAMB_ACT_RELU || a->act == YAMB_ACT_RELU6;
-  return lean ? launch_eval_act<G, EXPAND, true>(p, a, st) : launch_eval_act<G, EXPAND, false>(p, a, st);
+  if (p.mode == kPool) return launch_eval_mode<G, EXPAND, kPool>(p, a, st);
+  if (p.mode == kGate) return launch_eval_mode<G, EXPAND, kGate>(p, a, st);
+  return launch_eval_mode<G, EXPAND, kPlain>(p, a, st);
 }
 
-int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
+static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, bool pool) {
   if (!a) return set_error(YAMB_EINVAL, "null args");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   if (a->N <= 0 || a->H <= 0 || a->W <= 0) return set_error(YAMB_EINVAL, "block_eval: bad shape");
@@ -560,24 +653,25 @@ int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
   if ((a->kernel != 3 && a->kernel != 5 && a->kernel != 7) || (a->stride != 1 && a->stride != 2))
     return set_error(YAMB_EINVAL, "block_eval: depthwise k in {3,5,7}, stride 1 or 2 (got k=%d s=%d)",
                      a->kernel, a->stride);
-  if (a->kernel != 3 && (!a->w_expand || (a->act != YAMB_ACT_NONE && a->act != YAMB_ACT_RELU &&
-                                          a->act != YAMB_ACT_RELU6)))
-    return set_error(YAMB_EINVAL, "block_eval: k = 5 / 7 is built with expansion and a clamp "
-                                  "activation (relu / relu6) only");
+  if (a->kernel != 3 && !a->w_expand)
+    return set_error(YAMB_EINVAL, "block_eval: k = 5 / 7 is built with expansion only");
   if (!a->w_expand && a->Chid != a->Cin)
     return set_error(YAMB_EINVAL, "block_eval: no expand weights needs Chid == Cin");
   if (a->residual && a->stride != 1)
     return set_error(YAMB_EINVAL, "block_eval: residual needs stride 1");
   if (a->residual && a->Cin != a->Cout)
     return set_error(YAMB_EINVAL, "block_eval: residual needs Cin == Cout");
-  if (!a->x || !a->y || !a->w_dw || !a->w_project)
+  // the pool pass reads x, W1, the depthwise weights and BatchNorms 1 / 2 and writes `pooled`
+  if (!a->x || !a->w_dw || (pool ? !a->pooled : (!a->y || !a->w_project)))
     return set_error(YAMB_EINVAL, "block_eval: null pointer");
   const yamb_bn_eval* bns[3] = {&a->bn1, &a->bn2, &a->bn3};
-  for (int i = a->w_expand ? 0 : 1; i < 3; ++i)
+  for (int i = a->w_expand ? 0 : 1; i < (pool ? 2 : 3); ++i)
     if (!bns[i]->running_mean || !bns[i]->running_var)
       return set_error(YAMB_EINVAL, "block_eval: BatchNorm %d has no running statistics", i + 1);
   if ((((uintptr_t)a->x) | ((uintptr_t)a->y) | ((uintptr_t)a->w_expand) | ((uintptr_t)a->w_project)) & 15)
     return set_error(YAMB_EINVAL, "block_eval: tensors must be 16-byte aligned");
+  if (!pool && a->gate && ((uintptr_t)a->gate & 7))
+    return set_error(YAMB_EINVAL, "block_eval: gate must be 8-byte aligned");
   if ((long long)a->N * a->H * a->W > 0x7fffffffLL / 2)
     return set_error(YAMB_EINVAL, "block_eval: too many pixels");
   BlockEvalDev p;
@@ -589,6 +683,8 @@ int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
   p.act = a->act; p.residual = a->residual ? 1 : 0;
   p.x = (const __nv_bfloat16*)a->x; p.y = (__nv_bfloat16*)a->y;
   p.wdw = a->w_dw;
+  p.gate = a->gate;
+  p.mode = pool ? kPool : (a->gate ? kGate : kPlain);
   auto cvt = [](const yamb_bn_eval& s) {
     BnEvalDev d;
     d.gamma = s.gamma; d.beta = s.beta; d.mean = s.running_mean; d.var = s.running_var; d.eps = s.eps;
@@ -626,15 +722,23 @@ int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
               : launch_eval<EvGeom<3, 1, 7, 7, 2, 4>, false>(p, a, st);
   }
   if (a->kernel == 5) {
-    if (a->stride == 2) return launch_eval_act<EvGeom<5, 2, 6, 7, 1, 2>, true, true>(p, a, st);
-    if (wide) return launch_eval_act<EvGeom<5, 1, 7, 7, 1, 4>, true, true>(p, a, st);
+    if (a->stride == 2) return launch_eval<EvGeom<5, 2, 6, 7, 1, 2>, true>(p, a, st);
+    if (wide) return launch_eval<EvGeom<5, 1, 7, 7, 1, 4>, true>(p, a, st);
     const long long t0 = tiles_of(7, 16, 1), t1 = tiles_of(7, 14, 1), t2 = tiles_of(7, 7, 2);
-    if (t0 <= t1 && t0 <= t2) return launch_eval_act<EvGeom<5, 1, 7, 16, 1, 4>, true, true>(p, a, st);
-    if (t1 <= t2) return launch_eval_act<EvGeom<5, 1, 7, 14, 1, 4>, true, true>(p, a, st);
-    return launch_eval_act<EvGeom<5, 1, 7, 7, 2, 4>, true, true>(p, a, st);
+    if (t0 <= t1 && t0 <= t2) return launch_eval<EvGeom<5, 1, 7, 16, 1, 4>, true>(p, a, st);
+    if (t1 <= t2) return launch_eval<EvGeom<5, 1, 7, 14, 1, 4>, true>(p, a, st);
+    return launch_eval<EvGeom<5, 1, 7, 7, 2, 4>, true>(p, a, st);
   }
-  if (a->stride == 2) return launch_eval_act<EvGeom<7, 2, 4, 7, 1, 2>, true, true>(p, a, st);
-  return launch_eval_act<EvGeom<7, 1, 7, 7, 1, 2>, true, true>(p, a, st);
+  if (a->stride == 2) return launch_eval<EvGeom<7, 2, 4, 7, 1, 2>, true>(p, a, st);
+  return launch_eval<EvGeom<7, 1, 7, 7, 1, 2>, true>(p, a, st);
+}
+
+int block_eval_launch(const yamb_block_eval* a, cudaStream_t st) {
+  return block_eval_launch_impl(a, st, false);
+}
+
+int block_eval_pool_launch(const yamb_block_eval* a, cudaStream_t st) {
+  return block_eval_launch_impl(a, st, true);
 }
 
 }  // namespace yamb

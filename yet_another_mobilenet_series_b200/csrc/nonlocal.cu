@@ -32,6 +32,7 @@ struct NlGramDev {
   float alpha;
   float* G;
   int rows_per_cta;
+  float* part;       // deterministic: [row chunks][N][I][J] slabs (plain stores), else NULL
 };
 
 // pixel index (inside one sample) of the r-th row of the row set
@@ -78,6 +79,16 @@ __global__ void __launch_bounds__(256) nl_gram_kernel(const __grid_constant__ Nl
       a10 = fmaf(x1, y0, a10); a11 = fmaf(x1, y1, a11);
     }
     const int i = 2 * ip, j = 2 * jp;
+    if (p.part) {   // this CTA's slab: every element written once, det_reduce adds the slabs in order
+      float* S = p.part + ((size_t)blockIdx.x * p.N + n) * p.I * p.J;
+      S[(size_t)i * p.J + j] = p.alpha * a00;
+      S[(size_t)i * p.J + j + 1] = p.alpha * a01;
+      if (i + 1 < p.I) {
+        S[(size_t)(i + 1) * p.J + j] = p.alpha * a10;
+        S[(size_t)(i + 1) * p.J + j + 1] = p.alpha * a11;
+      }
+      continue;
+    }
     atomicAdd(G + (size_t)i * p.J + j, p.alpha * a00);
     atomicAdd(G + (size_t)i * p.J + j + 1, p.alpha * a01);
     if (i + 1 < p.I) {
@@ -187,7 +198,7 @@ int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t st) {
   p.Hs = (a->H + a->sub - 1) / a->sub; p.Ws = (a->W + a->sub - 1) / a->sub;
   p.X = (const __nv_bfloat16*)a->X; p.ldx = a->ldx; p.I = a->I;
   p.Y = (const __nv_bfloat16*)a->Y; p.ldy = a->ldy; p.J = a->J;
-  p.alpha = a->alpha; p.G = a->G;
+  p.alpha = a->alpha; p.G = a->G; p.part = nullptr;
   const int rows = p.Hs * p.Ws;
   const int I2 = (a->I + 1) & ~1;
   int R = rows < 64 ? rows : 64;
@@ -205,9 +216,18 @@ int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t st) {
     attr = smem;
   }
   dim3 grid((rows + R - 1) / R, a->N);
+  const long long n_out = (long long)a->N * a->I * a->J;
+  if (a->deterministic) {
+    rc = det_alloc((size_t)grid.x * n_out * sizeof(float), st, &p.part);
+    if (rc) return rc;
+  }
   nl_gram_kernel<<<grid, 256, smem, st>>>(p);
   e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "nl_gram: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) {
+    if (p.part) det_free(p.part, st);
+    return set_error(YAMB_ECUDA, "nl_gram: %s", cudaGetErrorString(e));
+  }
+  if (p.part) return det_reduce_launch(p.part, (int)grid.x, n_out, a->G, st);
   return 0;
 }
 

@@ -198,7 +198,8 @@ int se_fc_fwd_launch(const yamb_se_fc* a, cudaStream_t st) {
   g.C = a->u; g.c_rs = a->R; g.alpha = 1.f; g.epi = 5;
   cudaError_t e = cudaMemsetAsync(a->u, 0, (size_t)a->N * a->R * sizeof(float), st);
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc memset: %s", cudaGetErrorString(e));
-  e = se_gemm(g, st, se_ksplit(g.M, g.N, g.K));
+  // deterministic: one K slab, so every u element is one atomicAdd onto the zeroed buffer
+  e = se_gemm(g, st, a->deterministic ? 1 : se_ksplit(g.M, g.N, g.K));
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc fwd (reduce): %s", cudaGetErrorString(e));
   {
     dim3 fg((a->R + 255) / 256, (a->N + 31) / 32);

@@ -200,6 +200,88 @@ class _Bn:
         torch.addcmul(b.detach(), rm, self.scale, value=-1.0, out=self.shift)
 
 
+class _NlTail:
+    """Non-local block (reference models/mobilenet_base.py:158-173) behind a BatchNorm output l,
+    for one shape: y = BN4(dw3x3(f)) + l (+ x), f = (W/H) theta (phi^T g).  Owns l, f, h (bf16
+    [N*H*W, C]) and F (fp32 [N][c][C]); `forward` is the four launches of the training plan and of
+    the eval path alike.  `deterministic`: the gram adds its per-CTA partial sums in a fixed order
+    (eval: the same logits on every run) instead of with fp32 atomics (training)."""
+
+    def __init__(self, nl, bn4, N, H, W, C, dev, deterministic=False):
+        self.nl, self.bn4 = nl, bn4
+        self.N, self.H, self.W, self.C, self.M = N, H, W, C, N * H * W
+        self.cr = int(nl.nl_c * C)             # theta / phi channels (:163)
+        self.sub = int(nl.nl_s)
+        if self.cr <= 0 or self.cr % 2 or self.sub < 1:
+            raise nat.NativeError("non-local block: int(nl_c * C) must be a positive even "
+                                  "number (got %d)" % self.cr)
+        self.scale = float(W) / float(H)       # sic `f / H * W` (:171)
+        self.deterministic = 1 if deterministic else 0
+        bf = torch.bfloat16
+        self.l = torch.empty(self.M, C, device=dev, dtype=bf)
+        self.f = torch.empty(self.M, C, device=dev, dtype=bf)
+        self.h = torch.empty(self.M, C, device=dev, dtype=bf)
+        self.F = _f32(N * self.cr * C, dev)
+        self.keep = []
+
+    def gram(self, X, I, Y, sub, alpha, G, tag):
+        g = nat.NlGram()
+        g.N, g.H, g.W, g.sub = self.N, self.H, self.W, sub
+        g.X, g.ldx, g.I = X.data_ptr(), self.C, I
+        g.Y, g.ldy, g.J = Y.data_ptr(), self.C, self.C
+        g.alpha, g.G = alpha, G.data_ptr()
+        g.deterministic = self.deterministic
+        self.keep.append(g)
+        launch(lib_fn("yamb_nl_gram_fwd"), g, tag, 4 * self.M * self.C // (sub * sub))
+
+    def rowmat(self, X, K, Mat, sk, so, O, sub, alpha, out, tag, base=None, accumulate=0):
+        r = nat.NlRowmat()
+        r.N, r.H, r.W, r.sub = self.N, self.H, self.W, sub
+        r.X, r.ldx, r.K = X.data_ptr(), self.C, K
+        r.Mat, r.mat_stride, r.sk, r.so, r.O = Mat.data_ptr(), self.cr * self.C, sk, so, O
+        r.alpha = alpha
+        if base is not None:
+            r.base, r.ldb, r.O_copy = base.data_ptr(), self.C, self.C
+        r.accumulate = accumulate
+        r.out, r.ldo = out.data_ptr(), self.C
+        self.keep.append(r)
+        launch(lib_fn("yamb_nl_rowmat_fwd"), r, tag, 4 * self.M * self.C // (sub * sub))
+
+    def forward(self, xm, y, residual, bn_fwd_struct=None):
+        """self.l -> y.  bn_fwd_struct(bn, count): the yamb_bn_fwd of BN4 when it normalises with
+        batch statistics (train mode); otherwise BN4 is folded from its running statistics."""
+        lib = nat.lib()
+        self.keep = []
+        Cc, c = self.C, self.cr
+        # F = phi^T g over the sub-sampled pixels; f = (W/H) theta F
+        self.gram(self.l, c, self.l, self.sub, 1.0, self.F, "nl_gram")
+        self.rowmat(self.l, c, self.F, Cc, 1, Cc, 1, self.scale, self.f, "nl_apply")
+        # depthwise 3x3 (no activation before it) + BN4 statistics
+        d = nat.DwFwd()
+        d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.H, self.W, Cc, Cc, 3, 1
+        d.x = self.f.data_ptr()
+        d.w = self.nl.depthwise_conv.weight.data_ptr()
+        d.y = self.h.data_ptr()
+        if self.bn4.batch_stats:
+            d.bn = C.pointer(bn_fwd_struct(self.bn4, self.M))
+        else:
+            self.bn4.eval_coeffs()
+        launch(lib.yamb_depthwise_fwd, d, "nl_dw_fwd", 4 * Cc * self.M, 2 * self.M * Cc * 9)
+        # y = BN4(h) + l (+ x)
+        a = nat.BnApply()
+        a.M, a.C = self.M, Cc
+        a.ldh = a.ldr = a.ldy = Cc
+        a.h, a.scale, a.shift = self.h.data_ptr(), self.bn4.scale.data_ptr(), \
+            self.bn4.shift.data_ptr()
+        a.act = 0
+        a.residual = self.l.data_ptr()
+        if residual:
+            a.residual2, a.ldr2 = xm.data_ptr(), Cc
+        a.y = y.data_ptr()
+        self.keep += [d, a]
+        launch(lib.yamb_bn_apply_fwd, a, "nl_bn_apply", 2 * self.M * Cc * (4 if residual else 3))
+
+
 class BlockPlan:
     def __init__(self, block, x):
         dev = x.device
@@ -265,20 +347,13 @@ class BlockPlan:
             if not isinstance(nl.bn, torch.nn.BatchNorm2d):
                 raise nat.NativeError("non-local block: only the BatchNorm nl_norm is on the "
                                       "sm_90a path (got %s)" % type(nl.bn).__name__)
-            self.nl_cr = int(nl.nl_c * Cout)        # theta / phi channels (:163)
-            self.nl_sub = int(nl.nl_s)
-            if self.nl_cr <= 0 or self.nl_cr % 2 or self.nl_sub < 1:
-                raise nat.NativeError("non-local block: int(nl_c * C) must be a positive even "
-                                      "number (got %d)" % self.nl_cr)
-            self.nl_scale = float(self.Wo) / float(self.Ho)   # sic `f / H * W` (:171)
-            self.nl_l = torch.empty(self.M_out, Cout, device=dev, dtype=bf)
-            self.nl_f = torch.empty(self.M_out, Cout, device=dev, dtype=bf)
-            self.nl_h = torch.empty(self.M_out, Cout, device=dev, dtype=bf)
-            self.nl_F = _f32(N * self.nl_cr * Cout, dev)
+            self.nl_tail = tail = _NlTail(nl, _Bn([nl.bn], dev), N, self.Ho, self.Wo, Cout, dev)
+            self.nl_cr, self.nl_sub, self.nl_scale = tail.cr, tail.sub, tail.scale
+            self.nl_l, self.nl_f, self.nl_h, self.nl_F = tail.l, tail.f, tail.h, tail.F
             self.nl_dF = None
             self.nl_df = None
             self.nl_dl = None
-            self.bn4 = _Bn([nl.bn], dev)
+            self.bn4 = tail.bn4
             self.g_nl = torch.zeros_like(nl.depthwise_conv.weight, dtype=torch.float32)
         if self.se is not None:
             self.se_act = act_code_of(self.se.active_fn)
@@ -527,64 +602,15 @@ class BlockPlan:
             return y
         a.y = self.nl_l.data_ptr()              # l = BN3(h3): the non-local block's input
         self._call(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * self.M_out * self.Cout)
-        self._nl_forward(xm, y)
+        self.nl_tail.forward(xm, y, self.residual, self._bn_fwd_struct)
         return y
 
     # -- non-local block (reference models/mobilenet_base.py:158-173) ------------------------------
     def _nl_gram(self, X, I, Y, sub, alpha, G, tag):
-        g = nat.NlGram()
-        g.N, g.H, g.W, g.sub = self.N, self.Ho, self.Wo, sub
-        g.X, g.ldx, g.I = X.data_ptr(), self.Cout, I
-        g.Y, g.ldy, g.J = Y.data_ptr(), self.Cout, self.Cout
-        g.alpha, g.G = alpha, G.data_ptr()
-        self._keep.append(g)
-        self._call(lib_fn("yamb_nl_gram_fwd"), g, tag, 4 * self.M_out * self.Cout // (sub * sub))
+        self.nl_tail.gram(X, I, Y, sub, alpha, G, tag)
 
     def _nl_rowmat(self, X, K, Mat, sk, so, O, sub, alpha, out, tag, base=None, accumulate=0):
-        r = nat.NlRowmat()
-        r.N, r.H, r.W, r.sub = self.N, self.Ho, self.Wo, sub
-        r.X, r.ldx, r.K = X.data_ptr(), self.Cout, K
-        r.Mat, r.mat_stride, r.sk, r.so, r.O = Mat.data_ptr(), self.nl_cr * self.Cout, sk, so, O
-        r.alpha = alpha
-        if base is not None:
-            r.base, r.ldb, r.O_copy = base.data_ptr(), self.Cout, self.Cout
-        r.accumulate = accumulate
-        r.out, r.ldo = out.data_ptr(), self.Cout
-        self._keep.append(r)
-        self._call(lib_fn("yamb_nl_rowmat_fwd"), r, tag, 4 * self.M_out * self.Cout // (sub * sub))
-
-    def _nl_forward(self, xm, y):
-        lib = self.lib
-        Cc, c = self.Cout, self.nl_cr
-        # F = phi^T g over the sub-sampled pixels; f = (W/H) theta F
-        self._nl_gram(self.nl_l, c, self.nl_l, self.nl_sub, 1.0, self.nl_F, "nl_gram")
-        self._nl_rowmat(self.nl_l, c, self.nl_F, Cc, 1, Cc, 1, self.nl_scale, self.nl_f, "nl_apply")
-        # depthwise 3x3 (no activation before it) + BN4 statistics
-        d = nat.DwFwd()
-        d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.Ho, self.Wo, Cc, Cc, 3, 1
-        d.x = self.nl_f.data_ptr()
-        d.w = self.nl.depthwise_conv.weight.data_ptr()
-        d.y = self.nl_h.data_ptr()
-        if self.bn4.batch_stats:
-            d.bn = C.pointer(self._bn_fwd_struct(self.bn4, self.M_out))
-        else:
-            self.bn4.eval_coeffs()
-        self._call(lib.yamb_depthwise_fwd, d, "nl_dw_fwd", 4 * Cc * self.M_out,
-                   2 * self.M_out * Cc * 9)
-        # y = BN4(h) + l (+ x)
-        a = nat.BnApply()
-        a.M, a.C = self.M_out, Cc
-        a.ldh = a.ldr = a.ldy = Cc
-        a.h, a.scale, a.shift = self.nl_h.data_ptr(), self.bn4.scale.data_ptr(), \
-            self.bn4.shift.data_ptr()
-        a.act = 0
-        a.residual = self.nl_l.data_ptr()
-        if self.residual:
-            a.residual2, a.ldr2 = xm.data_ptr(), Cc
-        a.y = y.data_ptr()
-        self._keep.append(a)
-        self._call(lib.yamb_bn_apply_fwd, a, "nl_bn_apply",
-                   2 * self.M_out * Cc * (4 if self.residual else 3))
+        self.nl_tail.rowmat(X, K, Mat, sk, so, O, sub, alpha, out, tag, base, accumulate)
 
     def _nl_backward(self, dym, grads):
         """dy -> dl (gradient of the BN3 output): BN4 backward, depthwise 3x3 backward, the two
@@ -1332,6 +1358,8 @@ def bn_act_apply(bn, active_fn, h):
 # YAMB_EVAL_FUSED=0 keeps the four-launch sequence (folded coefficients) for every block.
 EVAL_FUSED = os.environ.get("YAMB_EVAL_FUSED", "1") != "0"
 EVAL_FUSED_CALLS = 0     # blocks that went through yamb_block_eval_fwd (tests / bench)
+# (both eval paths: fused_eval_forward for the unfused class, fused_class_eval_forward for
+# InvertedResidualChannelsFused)
 
 
 def fused_eval_supported(block, x):
@@ -1368,6 +1396,58 @@ def fused_eval_supported(block, x):
     return True
 
 
+def _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p):
+    """bf16 tensor-core operands of the expand / project weights (the optimizer's mirrors when
+    fresh, else block-owned copies kept in the `_yamb_eval` scratch that deepcopy / pickle drop)."""
+    st = block.__dict__.get("_yamb_eval")
+    if st is None:
+        st = block.__dict__["_yamb_eval"] = _ScratchDict()
+    key = dev.index
+    own = st.get(key)
+    if own is None:
+        own = (torch.empty(Chid, Cin, device=dev, dtype=torch.bfloat16) if block.expand else None,
+               torch.empty(Cout, Chid, device=dev, dtype=torch.bfloat16))
+        st[key] = own
+    with torch.no_grad():
+        w1 = _bf16_operand(conv_e.weight, own[0], (Chid, Cin)) if block.expand else None
+        w3 = _bf16_operand(conv_p.weight, own[1], (Cout, Chid))
+    return w1, w3
+
+
+def _block_eval_args(block, x, y, w1, w3, conv_d, bns, residual):
+    """yamb_block_eval of one single-branch block; bns = (bn1 or None, bn2, bn3)."""
+    N, Cin, H, W = x.shape
+    a = nat.BlockEval()
+    a.N, a.H, a.W = N, H, W
+    a.Cin, a.Chid, a.Cout = Cin, block.channels[0], block.output_dim
+    a.kernel, a.stride = block.kernel_sizes[0], block.stride
+    a.act = act_code_of(block.active_fn)
+    a.residual = 1 if residual else 0
+    a.x, a.y = x.data_ptr(), nat.ptr(y)
+    a.w_expand, a.w_project = nat.ptr(w1), w3.data_ptr()
+    a.w_dw = conv_d.weight.data_ptr()
+    for dst, bn in zip((a.bn1, a.bn2, a.bn3), bns):
+        if bn is None:
+            continue
+        dst.gamma = nat.ptr(bn.weight)
+        dst.beta = nat.ptr(bn.bias)
+        dst.running_mean = bn.running_mean.data_ptr()
+        dst.running_var = bn.running_var.data_ptr()
+        dst.eps = bn.eps
+    return a
+
+
+def _block_eval_cost(block, x, Ho, Wo, residual, project=True):
+    """(algorithmic bytes, flops) of one block_eval launch (engine.PROFILE bookkeeping)."""
+    N, Cin, H, W = x.shape
+    Chid, Cout, k = block.channels[0], block.output_dim, block.kernel_sizes[0]
+    nbytes = 2 * N * H * W * Cin * (2 if residual else 1) + \
+        (2 * N * Ho * Wo * Cout if project else 4 * N * Chid)
+    flops = 2 * Chid * (N * H * W * (Cin if block.expand else 0) +
+                        N * Ho * Wo * ((Cout if project else 0) + k ** 2))
+    return nbytes, flops
+
+
 def fused_eval_forward(block, x):
     """y = block(x) in eval mode through ONE kernel launch; x channels_last bf16 on CUDA."""
     global EVAL_FUSED_CALLS
@@ -1381,41 +1461,131 @@ def fused_eval_forward(block, x):
     bn3 = block.pw_bn
     Chid, Cout, stride = block.channels[0], block.output_dim, block.stride
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    st = block.__dict__.get("_yamb_eval")
-    if st is None:
-        st = block.__dict__["_yamb_eval"] = _ScratchDict()
-    key = dev.index
-    own = st.get(key)
-    if own is None:
-        own = (torch.empty(Chid, Cin, device=dev, dtype=torch.bfloat16) if block.expand else None,
-               torch.empty(Cout, Chid, device=dev, dtype=torch.bfloat16))
-        st[key] = own
-    with torch.no_grad():
-        w1 = _bf16_operand(conv_e.weight, own[0], (Chid, Cin)) if block.expand else None
-        w3 = _bf16_operand(conv_p.weight, own[1], (Cout, Chid))
+    w1, w3 = _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p)
     y = torch.empty((N, Cout, Ho, Wo), device=dev, dtype=torch.bfloat16,
                     memory_format=torch.channels_last)
-    a = nat.BlockEval()
-    a.N, a.H, a.W = N, H, W
-    a.Cin, a.Chid, a.Cout = Cin, Chid, Cout
-    a.kernel, a.stride = block.kernel_sizes[0], stride
-    a.act = act_code_of(block.active_fn)
-    a.residual = 1 if block.use_res_connect else 0
-    a.x, a.y = x.data_ptr(), y.data_ptr()
-    a.w_expand, a.w_project = nat.ptr(w1), w3.data_ptr()
-    a.w_dw = conv_d.weight.data_ptr()
-    for dst, bn in ((a.bn1, bn1), (a.bn2, bn2), (a.bn3, bn3)):
-        if bn is None:
-            continue
-        dst.gamma = nat.ptr(bn.weight)
-        dst.beta = nat.ptr(bn.bias)
-        dst.running_mean = bn.running_mean.data_ptr()
-        dst.running_var = bn.running_var.data_ptr()
-        dst.eps = bn.eps
+    a = _block_eval_args(block, x, y, w1, w3, conv_d, (bn1, bn2, bn3), block.use_res_connect)
     launch(lib_fn("yamb_block_eval_fwd"), a, "block_eval",
-           2 * (N * H * W * Cin * (2 if block.use_res_connect else 1) + N * Ho * Wo * Cout),
-           2 * Chid * (N * H * W * (Cin if block.expand else 0) +
-                       N * Ho * Wo * (Cout + block.kernel_sizes[0] ** 2)))
+           *_block_eval_cost(block, x, Ho, Wo, block.use_res_connect))
+    EVAL_FUSED_CALLS += 1
+    return y
+
+
+# ---- eval mode of InvertedResidualChannelsFused (AutoNL, AtomNAS): the block kernel with the SE
+# gate and the non-local tail (reference models/mobilenet_base.py:330-342) ----------------------------
+# Shape rule of the fused-class path, measured by tests/gpu_eval_bench_fused_class.py on one H100
+# 80GB HBM3 (400 W power limit), N = 256, kernel time per block, new path vs the four-launch
+# sequence.  5x5 blocks measured slower (AutoNL-L block 3, no SE: 1.08 vs 0.97 ms; block 14, SE:
+# 0.50 vs 0.38 ms; block 21, SE + non-local: 1.06 vs 0.83 ms).  So did the blocks without the
+# expansion at 112x112, whose four-launch sequence has no expand GEMM to save (AtomNAS-C+ block 1,
+# SE: 1.64 vs 1.03 ms; AutoNL-L block 1: 0.85 vs 0.79 ms).  3x3 blocks with the expansion measured
+# as fast or within 5 % (AutoNL-L block 8, non-local: 0.39 vs 0.50 ms; block 10, SE: 0.36 vs
+# 0.42 ms; block 12, SE + non-local: 0.43 vs 0.42 ms).  k = 7 was not measured (no such block in
+# AutoNL-L / AtomNAS-C+) and stays with k = 5.  False: every block the kernel covers takes the
+# path (tests, tests/gpu_eval_bench_fused_class.py).
+FUSED_CLASS_SHAPE_RULE = True
+
+
+def _bn_eval_ready(bn):
+    return isinstance(bn, torch.nn.BatchNorm2d) and not bn.training and \
+        bn.track_running_stats and bn.running_mean is not None
+
+
+def fused_class_eval_supported(block, x):
+    """True when the eval path of InvertedResidualChannelsFused covers this block for this call: no
+    gradient wanted, every BatchNorm (the non-local block's included) normalising with running
+    statistics, one branch with a 3x3 / 5x5 / 7x7 depthwise (no expansion: 3x3 only), stride 1 or
+    2, widths that are multiples of 8 with Cin <= 256 and Cout <= 320, any activation, with or
+    without Squeeze-and-Excitation and a non-local block (every block of AutoNL-L, block 1 of
+    AtomNAS-C+), minus the shapes FUSED_CLASS_SHAPE_RULE keeps on the four-launch sequence (8
+    AutoNL-L blocks take the path with it).  The unfused class has its own rule,
+    fused_eval_supported."""
+    if not EVAL_FUSED or torch.is_grad_enabled() or not hasattr(block, "expand_conv"):
+        return False
+    if block.stride not in (1, 2) or len(block.channels) != 1:
+        return False
+    k = list(block.kernel_sizes)[0]
+    cin, chid, cout = block.input_dim, block.channels[0], block.output_dim
+    if k not in (3, 5, 7) or cin % 8 or chid % 8 or cout % 8 or cin > 256 or cout > 320:
+        return False
+    if not block.expand and (k != 3 or chid != cin):
+        return False
+    if FUSED_CLASS_SHAPE_RULE and (k != 3 or not block.expand):
+        return False        # measured slower than the four-launch sequence (see above)
+    if x.dim() != 4 or x.shape[0] * x.shape[2] * x.shape[3] >= 2 ** 30:
+        return False
+    stage = list(block.depth_ops[0].children())[-1]
+    bns = [stage[1], block.project_conv[1]] + ([block.expand_conv[1]] if block.expand else [])
+    nl = block.nl_op if type(block.nl_op).__name__ != "Identity" else None
+    if nl is not None:
+        bns.append(nl.bn)
+        c = int(nl.nl_c * cout)
+        if c <= 0 or c % 2 or int(nl.nl_s) < 1:
+            return False
+    if not all(_bn_eval_ready(bn) for bn in bns):
+        return False
+    try:
+        act_code_of(block.active_fn)
+        if hasattr(block.se_op, "se_reduce"):
+            act_code_of(block.se_op.active_fn)
+    except ValueError:
+        return False
+    return True
+
+
+def fused_class_eval_forward(block, x):
+    """y = block(x) of an InvertedResidualChannelsFused in eval mode; x channels_last bf16 on CUDA.
+    C-ABI calls: the block kernel (1); with SE the pool pass and the gate FCs first (3); with a
+    non-local block the kernel writes l = BN3(h3) and the non-local tail follows (+4)."""
+    global EVAL_FUSED_CALLS
+    dev = x.device
+    N, Cin, H, W = x.shape
+    conv_e, bn1 = (block.expand_conv[0], block.expand_conv[1]) if block.expand else (None, None)
+    stage = list(block.depth_ops[0].children())[-1]
+    conv_d, bn2 = stage[0], stage[1]
+    conv_p, bn3 = block.project_conv[0], block.project_conv[1]
+    Chid, Cout, stride = block.channels[0], block.output_dim, block.stride
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    se = block.se_op if hasattr(block.se_op, "se_reduce") else None
+    nl = block.nl_op if type(block.nl_op).__name__ != "Identity" else None
+    w1, w3 = _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p)
+    bf = torch.bfloat16
+    y = torch.empty((N, Cout, Ho, Wo), device=dev, dtype=bf, memory_format=torch.channels_last)
+    # the block kernel's output: y itself, or l = BN3(h3) (no skip connection) for the non-local tail
+    residual = block.use_res_connect and nl is None
+    tail = None
+    if nl is not None:
+        st = block.__dict__["_yamb_eval"]
+        bn4 = st.get(("bn4", dev.index))
+        if bn4 is None:
+            bn4 = st[("bn4", dev.index)] = _Bn([nl.bn], dev)
+        tail = _NlTail(nl, bn4, N, Ho, Wo, Cout, dev, deterministic=True)
+    out = y if tail is None else tail.l
+    a = _block_eval_args(block, x, out, w1, w3, conv_d, (bn1, bn2, bn3), residual)
+    if se is not None:
+        # gate = sigmoid(W_e act(W_r mean_HW(a2) + b_r) + b_e): pool pass, then the two FCs
+        R = se.se_reduce.weight.shape[0]
+        pooled = torch.empty(N, Chid, device=dev, dtype=torch.float32)
+        gate = torch.empty(N, Chid, device=dev, dtype=torch.float32)
+        uv = torch.empty(2, N, R, device=dev, dtype=torch.float32)
+        a.pooled = pooled.data_ptr()
+        launch(lib_fn("yamb_block_eval_pool_fwd"), a, "block_eval_pool",
+               *_block_eval_cost(block, x, Ho, Wo, False, project=False))
+        f = nat.SeFc()
+        f.N, f.C, f.R, f.act = N, Chid, R, act_code_of(se.active_fn)
+        f.pooled = pooled.data_ptr()
+        f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
+        f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
+        f.u, f.v, f.gate = uv[0].data_ptr(), uv[1].data_ptr(), gate.data_ptr()
+        f.deterministic = 1
+        launch(lib_fn("yamb_se_fc_fwd"), f, "se_fc", 4 * N * Chid * 2, 4 * N * Chid * R)
+        a.pooled = None
+        a.gate = gate.data_ptr()
+    launch(lib_fn("yamb_block_eval_fwd"), a, "block_eval",
+           *_block_eval_cost(block, x, Ho, Wo, residual))
+    if tail is not None:
+        xm = x.permute(0, 2, 3, 1).reshape(N * H * W, Cin)    # view, NHWC matrix
+        tail.forward(xm, y.permute(0, 2, 3, 1).reshape(N * Ho * Wo, Cout), block.use_res_connect)
     EVAL_FUSED_CALLS += 1
     return y
 
@@ -1429,6 +1599,8 @@ def block_apply(block, x):
     x = to_nhwc_bf16(x)
     if fused_eval_supported(block, x):
         return fused_eval_forward(block, x)
+    if fused_class_eval_supported(block, x):
+        return fused_class_eval_forward(block, x)
     params = list(block.parameters())
     if needs_padding(block):
         return _PadFn.apply(x, block, *params)

@@ -177,6 +177,7 @@ class SeFc(C.Structure):
         ("pooled", C.c_void_p),
         ("w_r", C.c_void_p), ("b_r", C.c_void_p), ("w_e", C.c_void_p), ("b_e", C.c_void_p),
         ("u", C.c_void_p), ("v", C.c_void_p), ("gate", C.c_void_p),
+        ("deterministic", C.c_int32),
     ]
 
 
@@ -237,6 +238,7 @@ class BlockEval(C.Structure):
         ("w_project", C.c_void_p),
         ("bn1", BnEval), ("bn2", BnEval), ("bn3", BnEval),
         ("y", C.c_void_p),
+        ("gate", C.c_void_p), ("pooled", C.c_void_p),
     ]
 
 
@@ -247,6 +249,7 @@ class NlGram(C.Structure):
         ("Y", C.c_void_p), ("ldy", C.c_int64), ("J", C.c_int32),
         ("alpha", C.c_float),
         ("G", C.c_void_p),
+        ("deterministic", C.c_int32),
     ]
 
 
@@ -270,7 +273,7 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_block_eval_fwd", "yamb_rmsprop_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_rmsprop_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -316,6 +319,7 @@ def lib():
         l.yamb_nl_gram_fwd.argtypes = [C.POINTER(NlGram), C.c_void_p]
         l.yamb_nl_rowmat_fwd.argtypes = [C.POINTER(NlRowmat), C.c_void_p]
         l.yamb_block_eval_fwd.argtypes = [C.POINTER(BlockEval), C.c_void_p]
+        l.yamb_block_eval_pool_fwd.argtypes = [C.POINTER(BlockEval), C.c_void_p]
         l.yamb_rmsprop_step.argtypes = [C.POINTER(Rmsprop), C.c_void_p]
         l.yamb_ema_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,
                                       C.c_void_p]
