@@ -41,7 +41,29 @@ namespace yamb {
 #else
 #define YCLK() 0LL
 #endif
-#define MBAR_WAIT(bar, par) do { if (p.dbg & 256) mbar_wait_spin(bar, par); else mbar_wait(bar, par); } while (0)
+
+// Why the last mbarrier wait of gemm_tc_kernel that gave up did so:
+//   bits 40..63 block, 24..39 thread, 0..23 shared-memory address of the barrier.
+// Zero while no wait has timed out; readable from a debugger or a GPU core dump after the trap.
+__device__ unsigned long long g_gemm_wait_timeout;
+
+// Bounded mbarrier wait without a call in it: the printf of mbar_wait is an out-of-line call, and a
+// call inside the window where wgmmas are in flight makes ptxas serialise the whole wgmma sequence
+// (C7520).  A pipeline bug still traps after ~4 s instead of hanging the GPU.
+__device__ __forceinline__ void gemm_wait(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const uint64_t t0 = global_timer_ns();
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if (((++spins) & 0x3fff) == 0 && global_timer_ns() - t0 > 4000000000ull) {
+      *reinterpret_cast<volatile unsigned long long*>(&g_gemm_wait_timeout) =
+          ((unsigned long long)blockIdx.x << 40) | ((unsigned long long)(threadIdx.x & 0xffff) << 24) |
+          (smem_u32(bar) & 0xffffffu);
+      __threadfence_system();
+      __trap();
+    }
+  }
+}
 
 
 constexpr int kBlockM = 128;
@@ -265,15 +287,19 @@ __device__ __forceinline__ void gxform_panel(uint32_t panel, uint32_t panel2, co
   }
 }
 
-// One k16 step of a 64-row half: d[0 .. bn/2) (+)= A * B with the wgmma of width bn.
-template <int TA, int TB>
-__device__ __forceinline__ void mma_bn(float (&d)[32], int bn, uint64_t ad, uint64_t bd) {
-  if (bn == 64) wgmma_m64n64<TA, TB>(d, ad, bd, 1u);
-  else if (bn == 32) wgmma_m64n32<TA, TB>(reinterpret_cast<float(&)[16]>(d), ad, bd, 1u);
+// One k16 step of a 64-row half: d[0 .. BN/2) (+)= A * B with the wgmma of width BN.
+template <int TA, int TB, int BN>
+__device__ __forceinline__ void mma_bn(float (&d)[32], uint64_t ad, uint64_t bd) {
+  if constexpr (BN == 64) wgmma_m64n64<TA, TB>(d, ad, bd, 1u);
+  else if constexpr (BN == 32) wgmma_m64n32<TA, TB>(reinterpret_cast<float(&)[16]>(d), ad, bd, 1u);
   else wgmma_m64n16<TA, TB>(reinterpret_cast<float(&)[8]>(d), ad, bd, 1u);
 }
 
-template <bool kXform, int kEpi>
+// kBN (block_n = wgmma width), kAmn / kBmn (operand majors) are compile-time so that the consumer's
+// wgmma sequence is straight-line code: a runtime choice of instruction, a branch around the upper
+// half or a runtime k16 count puts the wgmmas in divergent paths, and ptxas then serialises every
+// one of them (C7520).  gemm_launch instantiates only the combinations the layers produce.
+template <bool kXform, int kEpi, int kBN, int kAmn, int kBmn>
 __global__ void __launch_bounds__(512, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -308,6 +334,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (p.has_bnf || p.has_bnb) {
     for (int i = threadIdx.x; i < 2 * p.N; i += blockDim.x) s_stats[i] = 0.0;
   }
+  // The MMA reads all 64 columns (4 k16 steps) of every k-block.  A K-major operand of K <= 32
+  // is loaded into 2 or 4 of the 8 16-byte chunks of each row only (panel_of: cshift); nothing
+  // else writes the other chunks during the launch, so they are zeroed once here.
+  if (p.K <= 32 && (!kAmn || !kBmn)) {
+    for (int i = threadIdx.x; i < S * p.stage_bytes / 16; i += blockDim.x)
+      sts128(smem_u32(smem) + 16u * (uint32_t)i, make_uint4(0u, 0u, 0u, 0u));
+    fence_proxy_async_smem();   // the zeros are read by wgmma (async proxy)
+  }
   __syncthreads();
 
   const bool use_x = kXform && (p.a_xform != 0 || p.b_xform != 0);
@@ -328,35 +362,35 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int kb0 = slab * p.kb_per_split;
         const int kb1 = min(kb0 + p.kb_per_split, p.num_k_blocks);
         for (int kb = kb0; kb < kb1; ++kb) {
-          MBAR_WAIT(&bars->empty[stage], phase ^ 1);
+          gemm_wait(&bars->empty[stage], phase ^ 1);
           uint8_t* sA = smem + (size_t)stage * p.stage_bytes;
           uint8_t* sB = sA + p.a_bytes;
           uint32_t tx = 0;
-          const int a_panels = p.a_mn ? 2 : 1;
+          const int a_panels = kAmn ? 2 : 1;
           int a_issue[2] = {0, 0};
-          const int b_panels = (p.block_n + 63) / 64;
+          const int b_panels = (kBN + 63) / 64;
           if (p.a_tma) {
-            if (!p.a_mn) {
+            if (!kAmn) {
               tx += (uint32_t)kABytes;
             } else {
               for (int q = 0; q < 2; ++q)
                 if (m_blk * kBlockM + q * 64 < p.M) { a_issue[q] = 1; tx += kPanelBytes64; }
             }
-            if (p.a_xform == 2) tx += p.a_mn ? (a_issue[0] + a_issue[1]) * kPanelBytes64 : (uint32_t)kABytes;
+            if (p.a_xform == 2) tx += kAmn ? (a_issue[0] + a_issue[1]) * kPanelBytes64 : (uint32_t)kABytes;
           }
           if (p.b_tma) {
             uint32_t tb = 0;
-            if (!p.b_mn) {
-              tb = (uint32_t)p.block_n * 128u;
+            if (!kBmn) {
+              tb = (uint32_t)kBN * 128u;
             } else {
               for (int q = 0; q < b_panels; ++q)
-                if (n_blk * p.block_n + q * 64 < p.N) tb += kPanelBytes64;
+                if (n_blk * kBN + q * 64 < p.N) tb += kPanelBytes64;
             }
             tx += p.b_xform == 2 ? 2 * tb : tb;
           }
           mbar_arrive_expect_tx(&bars->xdone[stage], tx);
           if (p.a_tma) {
-            if (!p.a_mn) {
+            if (!kAmn) {
               tma_load_2d(&tmA, &bars->xdone[stage], sA, kb * kBlockK, m_blk * kBlockM);
               if (p.a_xform == 2)
                 tma_load_2d(&tmA2, &bars->xdone[stage], sA + p.a2_off, kb * kBlockK, m_blk * kBlockM);
@@ -372,19 +406,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
           }
           if (p.b_tma) {
-            if (!p.b_mn) {
-              tma_load_2d(&tmB, &bars->xdone[stage], sB, kb * kBlockK, n_blk * p.block_n);
+            if (!kBmn) {
+              tma_load_2d(&tmB, &bars->xdone[stage], sB, kb * kBlockK, n_blk * kBN);
               if (p.b_xform == 2)
                 tma_load_2d(&tmB2, &bars->xdone[stage], sA + p.b2_off, kb * kBlockK,
-                            n_blk * p.block_n);
+                            n_blk * kBN);
             } else {
               for (int q = 0; q < b_panels; ++q)
-                if (n_blk * p.block_n + q * 64 < p.N) {
+                if (n_blk * kBN + q * 64 < p.N) {
                   tma_load_2d(&tmB, &bars->xdone[stage], sB + q * kPanelBytes64,
-                              n_blk * p.block_n + q * 64, kb * kBlockK);
+                              n_blk * kBN + q * 64, kb * kBlockK);
                   if (p.b_xform == 2)
                     tma_load_2d(&tmB2, &bars->xdone[stage], sA + p.b2_off + q * kPanelBytes64,
-                                n_blk * p.block_n + q * 64, kb * kBlockK);
+                                n_blk * kBN + q * 64, kb * kBlockK);
                 }
             }
           }
@@ -442,7 +476,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int mn2 = w2 / p.ksplit;
       const int m2 = mn2 / p.n_blocks, n2 = mn2 % p.n_blocks;
       const int grow2 = m2 * kBlockM + lane_trow;
-      const int col2 = n2 * p.block_n + sub2 * 64;
+      const int col2 = n2 * kBN + sub2 * 64;
       const __nv_bfloat16* srow = p.side + (size_t)grow2 * p.lds + col2;
 #pragma unroll
       for (int ch = 0; ch < 8; ++ch) {
@@ -456,16 +490,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int w0 = blockIdx.x + ((n_epi_wg == 2 && wg == 1) ? (int)gridDim.x : 0);
       if (w0 < p.num_work) load_side(w0, 0);
     }
-    // wgmma of one 64-row half: block_n and the operand majors select the instruction
-    auto mma_half = [&](float (&d)[32], uint64_t ad, uint64_t bd) {
-      if (p.a_mn) {
-        if (p.b_mn) mma_bn<1, 1>(d, p.block_n, ad, bd);
-        else mma_bn<1, 0>(d, p.block_n, ad, bd);
-      } else {
-        if (p.b_mn) mma_bn<0, 1>(d, p.block_n, ad, bd);
-        else mma_bn<0, 0>(d, p.block_n, ad, bd);
-      }
-    };
     float acc[2][32];
     int stage = 0, phase = 0, it = 0;
     uint32_t turn_par = 0;
@@ -479,10 +503,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         continue;
       }
       const int m_blk = mn / p.n_blocks, n_blk = mn % p.n_blocks;
-      const bool hi_half = m_blk * kBlockM + 64 < p.M;   // rows 64..127 of the tile exist
       // ---- main loop ----
       if (n_epi_wg == 2 && it > 0) {
-        MBAR_WAIT(&bars->turn[wg], turn_par);
+        gemm_wait(&bars->turn[wg], turn_par);
         turn_par ^= 1;
       }
 #pragma unroll
@@ -491,23 +514,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
-        MBAR_WAIT(&bars->full[stage], phase);
+        gemm_wait(&bars->full[stage], phase);
         const uint32_t sA = smem_u32(smem + (size_t)stage * p.stage_bytes);
         const uint32_t sB = sA + p.a_bytes;
-        const int krem = p.K - kb * kBlockK;
-        const int nk = krem >= kBlockK ? 4 : (krem + 15) / 16;
         reg_fence(acc[0]);
         reg_fence(acc[1]);
         wgmma_fence();
-#pragma unroll 1
-        for (int kk = 0; kk < nk; ++kk) {
-          const uint64_t bd = p.b_mn ? gmma_smem_desc(sB + kk * 2048, kPanelBytes64, 1024)
-                                     : gmma_smem_desc(sB + kk * 32, 16, 1024);
-          mma_half(acc[0], p.a_mn ? gmma_smem_desc(sA + kk * 2048, kPanelBytes64, 1024)
-                                  : gmma_smem_desc(sA + kk * 32, 16, 1024), bd);
-          if (hi_half)
-            mma_half(acc[1], p.a_mn ? gmma_smem_desc(sA + kPanelBytes64 + kk * 2048, kPanelBytes64, 1024)
-                                    : gmma_smem_desc(sA + 64 * 128 + kk * 32, 16, 1024), bd);
+        // Both 64-row halves and all four k16 steps, unconditionally.  The loaders store zeros
+        // past K (the k16 steps past K add exact zeros); rows past M (a missing upper half, or the
+        // second panel of an MN-major A of <= 64 channels, which aliases the B region) only feed
+        // outputs that are never stored, and the epilogue stages them as zero for the statistics.
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          const uint64_t bd = kBmn ? gmma_smem_desc(sB + kk * 2048, kPanelBytes64, 1024)
+                                   : gmma_smem_desc(sB + kk * 32, 16, 1024);
+          mma_bn<kAmn, kBmn, kBN>(acc[0], kAmn ? gmma_smem_desc(sA + kk * 2048, kPanelBytes64, 1024)
+                                               : gmma_smem_desc(sA + kk * 32, 16, 1024), bd);
+          mma_bn<kAmn, kBmn, kBN>(acc[1],
+                                  kAmn ? gmma_smem_desc(sA + kPanelBytes64 + kk * 2048, kPanelBytes64, 1024)
+                                       : gmma_smem_desc(sA + 64 * 128 + kk * 32, 16, 1024), bd);
         }
         wgmma_commit();
         if (prev >= 0) {            // the previous k-block's MMAs retired: its stage is free
@@ -524,11 +549,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (n_epi_wg == 2 && ctid == 0) mbar_arrive(&bars->turn[wg ^ 1]);   // next tile's main loop
       // ---- epilogue ----
       // sub-tiles of 64 columns; skip the ones that lie entirely beyond N (last n-block)
-      const int n_sub = min((p.block_n + 63) / 64, (p.N - n_blk * p.block_n + 63) / 64);
+      const int n_sub = min((kBN + 63) / 64, (p.N - n_blk * kBN + 63) / 64);
 #pragma unroll
       for (int sub = 0; sub < kMaxBlockN / 64; ++sub) {
         if (sub >= n_sub) break;
-        const int col0 = n_blk * p.block_n + sub * 64;  // global column of this sub-tile
+        const int col0 = n_blk * kBN + sub * 64;  // global column of this sub-tile
         if (kEpi == 2) {
           // split-K partial sums: plain stores of the fp32 tile into slab w of the scratch; the
           // reduction kernel that follows adds the slabs into D in slab order (deterministic)
@@ -608,7 +633,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // ---- per-column statistics of this warp's 32 rows of the bf16-rounded output ----
         if (p.has_bnf || p.has_bnb) {
           const int c = col0 + 2 * lane;  // column pair owned by this lane
-          if (c < p.N && (sub * 64 + 2 * lane) < p.block_n) {
+          if (c < p.N && (sub * 64 + 2 * lane) < kBN) {
             float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
             const float2 one2 = make_float2(1.f, 1.f), zero2 = make_float2(0.f, 0.f);
             // 4 independent accumulator sets (a 32-deep dependent chain of LDS -> FADD/FFMA would
@@ -693,8 +718,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int t = warp >= 12 ? threadIdx.x - 384 : threadIdx.x - 256 + 128;
     const int G = p.lgroup;                       // warps sharing a stage (rows split G ways)
     const int NW = (nxt >> 5) / G, lw = (t >> 5) / G, ls = (t >> 5) % G, ln = t & 31;
-    const int Ca = (kXform && p.a_xform) ? (p.a_mn ? p.M : p.K) : 0;
-    const int Cb = (kXform && p.b_xform) ? (p.b_mn ? p.N : p.K) : 0;
+    const int Ca = (kXform && p.a_xform) ? (kAmn ? p.M : p.K) : 0;
+    const int Cb = (kXform && p.b_xform) ? (kBmn ? p.N : p.K) : 0;
     float* xa = s_coef + (kEpi == 1 ? 4 * p.N : 0);
     float* xb = xa + 3 * Ca;
     if (use_x) {
@@ -714,8 +739,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     long long dbg_l[4] = {0, 0, 0, 0};
     const ActParam apa = make_act((kXform && p.a_xform == 1) ? p.a_act : ACT_NONE);
     const ActParam apb = make_act((kXform && p.b_xform == 1) ? p.b_act : ACT_NONE);
-    const int na = p.a_mn ? 2 : 1;                                         // panels of A
-    const int nb = p.b_mn ? (p.block_n + 63) / 64 : (p.block_n + 127) / 128;  // panels of B
+    const int na = kAmn ? 2 : 1;                                         // panels of A
+    const int nb = kBmn ? (kBN + 63) / 64 : (kBN + 127) / 128;  // panels of B
 
     // (tile, k-block) cursor over this CTA's work
     struct Cur { int w, kb, kb1, m_blk, n_blk; };
@@ -741,18 +766,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       Pan g;
       g.isA = pi < na;
       const int q = g.isA ? pi : pi - na;
-      g.mn = g.isA ? (p.a_mn != 0) : (p.b_mn != 0);
+      g.mn = g.isA ? (kAmn != 0) : (kBmn != 0);
       g.off = (g.isA ? 0u : (uint32_t)p.a_bytes) + (uint32_t)q * (g.mn ? kPanelBytes64 : 128 * 128);
       g.logR = g.mn ? 6 : 7;
       if (!g.mn) {  // K-major: rows are M (A) or N (B), channels along K
-        g.row0 = g.isA ? c.m_blk * kBlockM : c.n_blk * p.block_n + q * 128;
+        g.row0 = g.isA ? c.m_blk * kBlockM : c.n_blk * kBN + q * 128;
         g.col0 = c.kb * kBlockK; g.climit = p.K;
         g.rlimit = g.isA ? min(128, p.M - g.row0)
-                         : min(128, min(p.block_n - q * 128, p.N - g.row0));
+                         : min(128, min(kBN - q * 128, p.N - g.row0));
         g.rows = g.rlimit;     // rows past the limit only feed outputs that are never stored
       } else {      // MN-major: rows are K (pixels), 64 channels of M/N per panel
         g.row0 = c.kb * kBlockK;
-        g.col0 = (g.isA ? c.m_blk * kBlockM : c.n_blk * p.block_n) + q * 64;
+        g.col0 = (g.isA ? c.m_blk * kBlockM : c.n_blk * kBN) + q * 64;
         g.climit = g.isA ? p.M : p.N;
         g.rlimit = g.col0 < g.climit ? min(64, p.K - g.row0) : 0;
         // rows past K must read as zero (they are accumulated); a panel wholly past M / N only
@@ -766,6 +791,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int ncs = (g.climit - g.col0 + 7) >> 3;
       if (!g.mn) ncs = (ncs + 1) & ~1;   // K-steps of 16 columns: the odd chunk must read as zero
       g.cshift = ncs <= 2 ? 1 : (ncs <= 4 ? 2 : 3);
+      // the last k-block of a longer K reuses a stage that full k-blocks wrote: all 8 chunks of
+      // its rows are rewritten, those past K as zero (the MMA reads all 64 columns)
+      if (!g.mn && p.num_k_blocks > 1) g.cshift = 3;
       return g;
     };
     // cp.async one panel (coalesced: 8 consecutive threads fetch the 128 bytes of one row)
@@ -787,7 +815,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     };
     auto issue = [&](const Cur& c, int stage, int rnd) {
       const long long tl0 = YCLK();
-      MBAR_WAIT(&bars->empty[stage], (rnd & 1) ^ 1);
+      gemm_wait(&bars->empty[stage], (rnd & 1) ^ 1);
       dbg_l[0] += YCLK() - tl0;
       const uint32_t sA = smem_u32(smem + (size_t)stage * p.stage_bytes);
       for (int pi = 0; pi < na + nb; ++pi) {
@@ -826,7 +854,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // wide transformed operands: the TMA producer loaded them; rewrite the tile in place
         if (p.a_tma || p.b_tma) {
           const long long tl1 = YCLK();
-          MBAR_WAIT(&bars->xdone[stage], rnd & 1);
+          gemm_wait(&bars->xdone[stage], rnd & 1);
           dbg_l[1] += YCLK() - tl1;
           if (!(p.dbg & 1)) {
 #pragma unroll 1
@@ -953,6 +981,30 @@ static int make_map_2d(CUtensorMap* map, const void* ptr, uint64_t inner, uint64
 static int pick_block_n(int N, bool b_mn) {
   if (b_mn || N > 32) return 64;   // several n-blocks: 64 columns each, one staging sub-tile
   return N <= 16 ? 16 : 32;
+}
+
+// Launch of one instantiation.  The dynamic shared-memory limit of a kernel is process-wide: one
+// counter per instantiation, the limit is only ever raised.
+using LaunchFn = cudaError_t (*)(int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&,
+                                 const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,
+                                 const GemmDev&);
+template <bool XF, int EP, int BN, int AMN, int BMN>
+static cudaError_t launch_tc(int grid, int smem, cudaStream_t stream, const CUtensorMap& tmA,
+                             const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
+                             const CUtensorMap& tmD, const GemmDev& p) {
+  static int attr_smem = 0;
+  if (attr_smem < smem) {
+    const cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<XF, EP, BN, AMN, BMN>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return e;
+    attr_smem = smem;
+  }
+  gemm_tc_kernel<XF, EP, BN, AMN, BMN><<<grid, 512, smem, stream>>>(tmA, tmB, tmA2, tmB2, tmD, p);
+  return cudaGetLastError();
+}
+template <int EP, int BN, int AMN, int BMN>
+static LaunchFn pick_tc(bool xf) {
+  return xf ? &launch_tc<true, EP, BN, AMN, BMN> : &launch_tc<false, EP, BN, AMN, BMN>;
 }
 
 int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
@@ -1145,6 +1197,20 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   if (p.side && ((reinterpret_cast<uintptr_t>(p.side) & 15) || (p.lds % 8)))
     return set_error(YAMB_EINVAL, "side operand must be 16-byte aligned with lds % 8 == 0");
 
+  // the operand layouts the layers produce (an MN-major B always has block_n 64)
+  LaunchFn fn = nullptr;
+  if (a->epi == 0 && !p.a_mn && !p.b_mn)   // forward
+    fn = p.block_n == 64 ? pick_tc<0, 64, 0, 0>(xf) : p.block_n == 32 ? pick_tc<0, 32, 0, 0>(xf)
+                                                                      : pick_tc<0, 16, 0, 0>(xf);
+  else if (a->epi == 0 && !p.a_mn)         // dgrad (+ residual)
+    fn = pick_tc<0, 64, 0, 1>(xf);
+  else if (a->epi == 1 && !p.a_mn && p.b_mn)   // dgrad + dz: the layers always transform A, so one
+    fn = &launch_tc<true, 1, 64, 0, 1>;        // variant (it runs a plain A with the transform off)
+  else if (a->epi == 2 && p.a_mn && p.b_mn)    // wgrad
+    fn = pick_tc<2, 64, 1, 1>(xf);
+  if (!fn)
+    return set_error(YAMB_EINVAL, "GEMM operand layout not supported (epi %d, A %s, B %s)", a->epi,
+                     p.a_mn ? "MN-major" : "K-major", p.b_mn ? "MN-major" : "K-major");
   const int grid = p.num_work < ctas ? p.num_work : ctas;
   cudaError_t e;
   if (a->epi == 2) {   // split-K partial tiles: released by the reduction below, on this stream
@@ -1155,28 +1221,7 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
     if (p.part) det_free(p.part, stream);
     return set_error(YAMB_ECUDA, "%s: %s", what, cudaGetErrorString(err));
   };
-#define YAMB_GEMM_LAUNCH(XF, EP, THREADS)                                                         \
-  do {                                                                                           \
-    static int attr_smem = 0; /* per instantiation, process-wide: only ever RAISE the limit */     \
-    if (attr_smem < smem_total) {                                                                \
-      e = cudaFuncSetAttribute(gemm_tc_kernel<XF, EP>,                                           \
-                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem_total);         \
-      if (e != cudaSuccess) return fail("smem attr", e);                                      \
-      attr_smem = smem_total;                                                                    \
-    }                                                                                            \
-    gemm_tc_kernel<XF, EP><<<grid, THREADS, smem_total, stream>>>(tmA, tmB, tmA2, tmB2, tmD, p); \
-  } while (0)
-  if (xf) {
-    if (a->epi == 0) YAMB_GEMM_LAUNCH(true, 0, 512);
-    else if (a->epi == 1) YAMB_GEMM_LAUNCH(true, 1, 512);
-    else YAMB_GEMM_LAUNCH(true, 2, 512);
-  } else {
-    if (a->epi == 0) YAMB_GEMM_LAUNCH(false, 0, 512);
-    else if (a->epi == 1) YAMB_GEMM_LAUNCH(false, 1, 512);
-    else YAMB_GEMM_LAUNCH(false, 2, 512);
-  }
-#undef YAMB_GEMM_LAUNCH
-  e = cudaGetLastError();
+  e = fn(grid, smem_total, stream, tmA, tmB, tmA2, tmB2, tmD, p);
   if (e != cudaSuccess) return fail("gemm launch", e);
   if (a->epi == 2) {
     const long long total = (long long)a->M * a->N;
