@@ -303,6 +303,46 @@ typedef struct yamb_nl_rowmat {
 int yamb_nl_gram_fwd(const yamb_nl_gram* args, yamb_stream_t stream);
 int yamb_nl_rowmat_fwd(const yamb_nl_rowmat* args, yamb_stream_t stream);
 
+/* ---- instance normalisation of the non-local block (nl_norm: nn.InstanceNorm) --------------------
+ * nn.InstanceNorm2d(C, affine=True, track_running_stats=True) in training mode (reference
+ * models/mobilenet_base.py:149-156, :472-481) on the raw depthwise output h of the non-local block:
+ *   forward : per (n, c) mean mu and biased variance over the HW pixels of sample n,
+ *             y = gamma*(h - mu)*invstd + beta (+ residual) (+ residual2)  (bf16);
+ *             running = (1-m)*running + m*mean_n(batch), running_var from each instance's UNBIASED
+ *             variance; momentum 0 (torch's momentum=None) or NULL running buffers: no update
+ *   backward: per (n, c) sums of dy and dy*xhat,
+ *             dh = gamma*invstd*(dy - sum(dy)/HW - xhat*sum(dy*xhat)/HW)  (bf16),
+ *             dgamma += sum_n sum(dy*xhat), dbeta += sum_n sum(dy)
+ * One CTA per (sample, 64-channel chunk) owns its statistics; the sums over n are added in sample
+ * order by the last CTA (no float atomics: the same bits on every run).  HW >= 2; C, ld* multiples
+ * of 8.  In eval mode the norm is a per-channel affine (yamb_bn_apply_fwd with folded
+ * coefficients). */
+typedef struct yamb_in_fwd {
+  int32_t N, HW, C, ldh;
+  const void* h;                              /* bf16 [N*HW][ldh] */
+  const float* gamma; const float* beta;      /* [C] or NULL (=1 / =0) */
+  float eps, momentum;
+  float* running_mean; float* running_var;    /* [C] or NULL */
+  float* mean; float* invstd;                 /* out [N][C], saved for backward */
+  const void* residual; int32_t ldr;          /* bf16 [N*HW][ldr] addend, or NULL */
+  const void* residual2; int32_t ldr2;        /* second bf16 addend, or NULL */
+  void* y; int32_t ldy;                       /* out bf16 [N*HW][ldy] */
+  uint32_t* counter;                          /* zero-initialised word, self-resetting */
+} yamb_in_fwd;
+
+typedef struct yamb_in_bwd {
+  int32_t N, HW, C, ldh, lddy, lddh;
+  const void* dy; const void* h;              /* bf16 [N*HW][lddy], [N*HW][ldh] */
+  const float* gamma;                         /* [C] or NULL */
+  const float* mean; const float* invstd;     /* [N][C] from the forward */
+  float* dgamma; float* dbeta;                /* [C] +=, or NULL */
+  void* dh;                                   /* out bf16 [N*HW][lddh] */
+  uint32_t* counter;                          /* zero-initialised word, self-resetting */
+} yamb_in_bwd;
+
+int yamb_instance_norm_fwd(const yamb_in_fwd* args, yamb_stream_t stream);
+int yamb_instance_norm_bwd(const yamb_in_bwd* args, yamb_stream_t stream);
+
 /* ---- stem convolution -----------------------------------------------------------------------------
  * 3x3, stride 2, pad 1, 3 input channels -> Cout (multiple of 8, <= 64) on NHWC bf16: the first
  * layer of the network (reference models/mobilenet_supernet.py:124-130; its BatchNorm + activation
@@ -427,7 +467,8 @@ int yamb_max_ctas(void);
 /* sizeof() of the ABI structs (0 bn_fwd, 1 bn_bwd, 2 gemm, 3 dw_fwd, 4 dw_bwd, 5 bn_apply,
  * 6 bn_reduce, 7 se_pool, 8 rmsprop, 9 se_bwd_reduce, 10 se_bwd_apply, 11 bn_stats,
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
- * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval) so bindings can self-check */
+ * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd) so bindings
+ * can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

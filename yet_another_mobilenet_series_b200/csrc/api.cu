@@ -74,6 +74,8 @@ int yamb_struct_size(int which) {
     case 19: return (int)sizeof(yamb_stem_conv);
     case 20: return (int)sizeof(yamb_bn_eval);
     case 21: return (int)sizeof(yamb_block_eval);
+    case 22: return (int)sizeof(yamb_in_fwd);
+    case 23: return (int)sizeof(yamb_in_bwd);
     default: return -1;
   }
 }
@@ -106,6 +108,8 @@ int yamb_nl_gram_fwd(const yamb_nl_gram* a, yamb_stream_t s) { return yamb::nl_g
 int yamb_nl_rowmat_fwd(const yamb_nl_rowmat* a, yamb_stream_t s) { return yamb::nl_rowmat_launch(a, YAMB_ST(s)); }
 int yamb_block_eval_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_launch(a, YAMB_ST(s)); }
 int yamb_block_eval_pool_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_pool_launch(a, YAMB_ST(s)); }
+int yamb_instance_norm_fwd(const yamb_in_fwd* a, yamb_stream_t s) { return yamb::in_fwd_launch(a, YAMB_ST(s)); }
+int yamb_instance_norm_bwd(const yamb_in_bwd* a, yamb_stream_t s) { return yamb::in_bwd_launch(a, YAMB_ST(s)); }
 int yamb_rmsprop_step(const yamb_rmsprop* a, yamb_stream_t s) { return yamb::rmsprop_launch(a, YAMB_ST(s)); }
 int yamb_ema_update(float* shadow, const float* x, int64_t n, const float* hyper, float m,
                     yamb_stream_t s) {

@@ -200,15 +200,33 @@ class _Bn:
         torch.addcmul(b.detach(), rm, self.scale, value=-1.0, out=self.shift)
 
 
+def _nl_norm_supported(norm):
+    """The non-local block's norms the sm_90a path runs (reference get_nl_norm_fn,
+    models/mobilenet_base.py:472-481): BatchNorm2d (`nl_norm: nn.BatchNorm`, the default) and the
+    tracked affine InstanceNorm2d (`nl_norm: nn.InstanceNorm`)."""
+    if isinstance(norm, torch.nn.BatchNorm2d):
+        return True
+    return isinstance(norm, torch.nn.InstanceNorm2d) and norm.affine and \
+        norm.track_running_stats and norm.running_mean is not None
+
+
 class _NlTail:
     """Non-local block (reference models/mobilenet_base.py:158-173) behind a BatchNorm output l,
-    for one shape: y = BN4(dw3x3(f)) + l (+ x), f = (W/H) theta (phi^T g).  Owns l, f, h (bf16
+    for one shape: y = norm(dw3x3(f)) + l (+ x), f = (W/H) theta (phi^T g).  Owns l, f, h (bf16
     [N*H*W, C]) and F (fp32 [N][c][C]); `forward` is the four launches of the training plan and of
     the eval path alike.  `deterministic`: the gram adds its per-CTA partial sums in a fixed order
-    (eval: the same logits on every run) instead of with fp32 atomics (training)."""
+    (eval: the same logits on every run) instead of with fp32 atomics (training).
+
+    The norm (`bn4`) runs in one of three modes, chosen per forward: BatchNorm with batch
+    statistics (the depthwise kernel takes them, yamb_bn_apply_fwd applies them), InstanceNorm with
+    per-sample statistics (yamb_instance_norm_fwd takes and applies them), or either norm folded
+    from its running statistics (yamb_bn_apply_fwd)."""
 
     def __init__(self, nl, bn4, N, H, W, C, dev, deterministic=False):
         self.nl, self.bn4 = nl, bn4
+        self.instance = isinstance(nl.bn, torch.nn.InstanceNorm2d)
+        self.used_instance_stats = False      # mode of the last forward (its backward follows it)
+        self.in_mean = self.in_invstd = None
         self.N, self.H, self.W, self.C, self.M = N, H, W, C, N * H * W
         self.cr = int(nl.nl_c * C)             # theta / phi channels (:163)
         self.sub = int(nl.nl_s)
@@ -253,6 +271,11 @@ class _NlTail:
         lib = nat.lib()
         self.keep = []
         Cc, c = self.C, self.cr
+        instance = self.instance and self.bn4.batch_stats
+        if instance and self.H * self.W == 1:
+            raise nat.NativeError("non-local block: InstanceNorm in training mode needs more than "
+                                  "one pixel per channel (the map is 1x1)")
+        self.used_instance_stats = instance
         # F = phi^T g over the sub-sampled pixels; f = (W/H) theta F
         self.gram(self.l, c, self.l, self.sub, 1.0, self.F, "nl_gram")
         self.rowmat(self.l, c, self.F, Cc, 1, Cc, 1, self.scale, self.f, "nl_apply")
@@ -262,11 +285,16 @@ class _NlTail:
         d.x = self.f.data_ptr()
         d.w = self.nl.depthwise_conv.weight.data_ptr()
         d.y = self.h.data_ptr()
-        if self.bn4.batch_stats:
+        if instance:
+            pass                               # statistics per sample: yamb_instance_norm_fwd
+        elif self.bn4.batch_stats:
             d.bn = C.pointer(bn_fwd_struct(self.bn4, self.M))
         else:
             self.bn4.eval_coeffs()
         launch(lib.yamb_depthwise_fwd, d, "nl_dw_fwd", 4 * Cc * self.M, 2 * self.M * Cc * 9)
+        if instance:
+            self._instance_forward(xm, y, residual)
+            return
         # y = BN4(h) + l (+ x)
         a = nat.BnApply()
         a.M, a.C = self.M, Cc
@@ -280,6 +308,48 @@ class _NlTail:
         a.y = y.data_ptr()
         self.keep += [d, a]
         launch(lib.yamb_bn_apply_fwd, a, "nl_bn_apply", 2 * self.M * Cc * (4 if residual else 3))
+
+    def _instance_forward(self, xm, y, residual):
+        """y = InstanceNorm(h) + l (+ x) with per-sample statistics; mean / invstd [N][C] kept for
+        the backward, running statistics updated (torch: momentum None -> no update)."""
+        Cc = self.C
+        m = self.bn4.mods[0]
+        if self.in_mean is None:
+            self.in_mean = _f32(self.N * Cc, self.l.device)
+            self.in_invstd = _f32(self.N * Cc, self.l.device)
+        s = nat.InFwd()
+        s.N, s.HW, s.C, s.ldh = self.N, self.H * self.W, Cc, Cc
+        s.h = self.h.data_ptr()
+        s.gamma, s.beta = m.weight.data_ptr(), m.bias.data_ptr()
+        s.eps = m.eps
+        s.momentum = 0.0 if m.momentum is None else float(m.momentum)
+        s.running_mean, s.running_var = m.running_mean.data_ptr(), m.running_var.data_ptr()
+        s.mean, s.invstd = self.in_mean.data_ptr(), self.in_invstd.data_ptr()
+        s.residual, s.ldr = self.l.data_ptr(), Cc
+        if residual:
+            s.residual2, s.ldr2 = xm.data_ptr(), Cc
+        s.y, s.ldy = y.data_ptr(), Cc
+        s.counter = Workspace.get(self.l.device).counter.data_ptr()
+        self.keep.append(s)
+        launch(nat.lib().yamb_instance_norm_fwd, s, "nl_in_fwd",
+               2 * self.M * Cc * (5 if residual else 4))
+
+    def instance_backward(self, dym, dh, grads):
+        """dh = InstanceNorm backward of dy (bf16), dgamma / dbeta += into grads[0]."""
+        Cc = self.C
+        m = self.bn4.mods[0]
+        s = nat.InBwd()
+        s.N, s.HW, s.C = self.N, self.H * self.W, Cc
+        s.ldh = s.lddy = s.lddh = Cc
+        s.dy, s.h = dym.data_ptr(), self.h.data_ptr()
+        s.gamma = m.weight.data_ptr()
+        s.mean, s.invstd = self.in_mean.data_ptr(), self.in_invstd.data_ptr()
+        dg, db = grads[0]
+        s.dgamma, s.dbeta = nat.ptr(dg), nat.ptr(db)
+        s.dh = dh.data_ptr()
+        s.counter = Workspace.get(self.l.device).counter.data_ptr()
+        self.keep.append(s)
+        launch(nat.lib().yamb_instance_norm_bwd, s, "nl_in_bwd", 2 * self.M * Cc * 5)
 
 
 class BlockPlan:
@@ -344,15 +414,18 @@ class BlockPlan:
         if self.nl is not None:
             # non-local block (reference models/mobilenet_base.py:131-178) between BN3 and the skip
             nl = self.nl
-            if not isinstance(nl.bn, torch.nn.BatchNorm2d):
-                raise nat.NativeError("non-local block: only the BatchNorm nl_norm is on the "
-                                      "sm_90a path (got %s)" % type(nl.bn).__name__)
+            if not _nl_norm_supported(nl.bn):
+                raise nat.NativeError(
+                    "non-local block: the sm_90a path runs nn.BatchNorm2d and "
+                    "nn.InstanceNorm2d(affine=True, track_running_stats=True) as nl_norm (got %r)"
+                    % nl.bn)
             self.nl_tail = tail = _NlTail(nl, _Bn([nl.bn], dev), N, self.Ho, self.Wo, Cout, dev)
             self.nl_cr, self.nl_sub, self.nl_scale = tail.cr, tail.sub, tail.scale
             self.nl_l, self.nl_f, self.nl_h, self.nl_F = tail.l, tail.f, tail.h, tail.F
             self.nl_dF = None
             self.nl_df = None
             self.nl_dl = None
+            self.nl_in_dh = None
             self.bn4 = tail.bn4
             self.g_nl = torch.zeros_like(nl.depthwise_conv.weight, dtype=torch.float32)
         if self.se is not None:
@@ -621,15 +694,29 @@ class BlockPlan:
             self.nl_df = torch.empty(self.M_out, Cc, device=self.dev, dtype=bf)
             self.nl_dl = torch.empty(self.M_out, Cc, device=self.dev, dtype=bf)
             self.nl_dF = _f32(self.N * c * Cc, self.dev)
-        r = nat.BnReduce()
-        r.M, r.C, r.lddy, r.ldh = self.M_out, Cc, Cc, Cc
-        r.dy, r.h = dym.data_ptr(), self.nl_h.data_ptr()
-        r.bn = C.pointer(self._bn_bwd_struct(self.bn4, self.M_out, grads["bn4"]))
-        self._call(lib.yamb_bn_reduce_bwd, r, "nl_bn_reduce", 4 * self.M_out * Cc)
+        tail = self.nl_tail
         d = nat.DwBwd()
         d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.Ho, self.Wo, Cc, Cc, 3, 1
-        d.dz, d.h = dym.data_ptr(), self.nl_h.data_ptr()
-        d.ca, d.cb, d.cc = self.bn4.ca.data_ptr(), self.bn4.cb.data_ptr(), self.bn4.cc.data_ptr()
+        if tail.used_instance_stats:
+            # InstanceNorm with per-sample statistics: its backward writes dh (bf16), which the
+            # depthwise backward takes with the identity coefficients ca = 1, cb = cc = 0
+            if self.nl_in_dh is None:
+                self.nl_in_dh = torch.empty(self.M_out, Cc, device=self.dev, dtype=bf)
+                self.nl_ones = torch.ones(Cc, device=self.dev, dtype=torch.float32)
+                self.nl_zeros = _f32(Cc, self.dev)
+            tail.instance_backward(dym, self.nl_in_dh, grads["bn4"])
+            d.dz, d.h = self.nl_in_dh.data_ptr(), self.nl_h.data_ptr()
+            d.ca, d.cb, d.cc = self.nl_ones.data_ptr(), self.nl_zeros.data_ptr(), \
+                self.nl_zeros.data_ptr()
+        else:
+            r = nat.BnReduce()
+            r.M, r.C, r.lddy, r.ldh = self.M_out, Cc, Cc, Cc
+            r.dy, r.h = dym.data_ptr(), self.nl_h.data_ptr()
+            r.bn = C.pointer(self._bn_bwd_struct(self.bn4, self.M_out, grads["bn4"]))
+            self._call(lib.yamb_bn_reduce_bwd, r, "nl_bn_reduce", 4 * self.M_out * Cc)
+            d.dz, d.h = dym.data_ptr(), self.nl_h.data_ptr()
+            d.ca, d.cb, d.cc = self.bn4.ca.data_ptr(), self.bn4.cb.data_ptr(), \
+                self.bn4.cc.data_ptr()
         d.w = self.nl.depthwise_conv.weight.data_ptr()
         d.dw = grads["nl_dw"].data_ptr()
         d.x = self.nl_f.data_ptr()
@@ -1071,6 +1158,11 @@ class _PadShadow(Scratch):
         self.shadow = base(block.input_dim, block.output_dim, block.stride, self.pad_ch,
                            list(block.kernel_sizes), block.expand, **kw).to(device)
         logging.root.setLevel(lvl)
+        if fused and hasattr(block.nl_op, "bn"):
+            # the non-local norm (output width: never padded) is of the real block's class, which
+            # the reference picks from FLAGS.nl_norm at construction time
+            import copy
+            self.shadow.nl_op.bn = copy.deepcopy(block.nl_op.bn).to(device)
         for p in self.shadow.parameters():
             p.requires_grad_(False)
         real = dict(block.named_parameters())
@@ -1172,7 +1264,7 @@ class _PadShadow(Scratch):
                     shad_b[n].copy_(real[n])
         for (_, rm), (_, sm) in zip(block.named_modules(), self.shadow.named_modules()):
             sm.training = rm.training
-            if isinstance(rm, torch.nn.BatchNorm2d):
+            if isinstance(rm, (torch.nn.BatchNorm2d, torch.nn.InstanceNorm2d)):
                 sm.momentum, sm.eps = rm.momentum, rm.eps
 
     def pull_stats(self, block):
@@ -1491,10 +1583,17 @@ def _bn_eval_ready(bn):
         bn.track_running_stats and bn.running_mean is not None
 
 
+def _nl_norm_eval_ready(norm):
+    """The non-local block's norm is a per-channel affine from running statistics."""
+    if isinstance(norm, torch.nn.InstanceNorm2d):
+        return _nl_norm_supported(norm) and not norm.training
+    return _bn_eval_ready(norm)
+
+
 def fused_class_eval_supported(block, x):
     """True when the eval path of InvertedResidualChannelsFused covers this block for this call: no
-    gradient wanted, every BatchNorm (the non-local block's included) normalising with running
-    statistics, one branch with a 3x3 / 5x5 / 7x7 depthwise (no expansion: 3x3 only), stride 1 or
+    gradient wanted, every BatchNorm (the non-local block's included, or its tracked InstanceNorm)
+    normalising with running statistics, one branch with a 3x3 / 5x5 / 7x7 depthwise (no expansion: 3x3 only), stride 1 or
     2, widths that are multiples of 8 with Cin <= 256 and Cout <= 320, any activation, with or
     without Squeeze-and-Excitation and a non-local block (every block of AutoNL-L, block 1 of
     AtomNAS-C+), minus the shapes FUSED_CLASS_SHAPE_RULE keeps on the four-launch sequence (8
@@ -1518,7 +1617,8 @@ def fused_class_eval_supported(block, x):
     bns = [stage[1], block.project_conv[1]] + ([block.expand_conv[1]] if block.expand else [])
     nl = block.nl_op if type(block.nl_op).__name__ != "Identity" else None
     if nl is not None:
-        bns.append(nl.bn)
+        if not _nl_norm_eval_ready(nl.bn):
+            return False
         c = int(nl.nl_c * cout)
         if c <= 0 or c % 2 or int(nl.nl_s) < 1:
             return False

@@ -266,14 +266,41 @@ class NlRowmat(C.Structure):
     ]
 
 
+class InFwd(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32), ("ldh", C.c_int32),
+        ("h", C.c_void_p),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p),
+        ("eps", C.c_float), ("momentum", C.c_float),
+        ("running_mean", C.c_void_p), ("running_var", C.c_void_p),
+        ("mean", C.c_void_p), ("invstd", C.c_void_p),
+        ("residual", C.c_void_p), ("ldr", C.c_int32),
+        ("residual2", C.c_void_p), ("ldr2", C.c_int32),
+        ("y", C.c_void_p), ("ldy", C.c_int32),
+        ("counter", C.c_void_p),
+    ]
+
+
+class InBwd(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32), ("ldh", C.c_int32),
+        ("lddy", C.c_int32), ("lddh", C.c_int32),
+        ("dy", C.c_void_p), ("h", C.c_void_p),
+        ("gamma", C.c_void_p), ("mean", C.c_void_p), ("invstd", C.c_void_p),
+        ("dgamma", C.c_void_p), ("dbeta", C.c_void_p),
+        ("dh", C.c_void_p),
+        ("counter", C.c_void_p),
+    ]
+
+
 _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnReduce, 7: SePool,
             8: Rmsprop, 9: SeBwdReduce, 10: SeBwdApply, 11: BnStats, 12: BnBwdApply, 13: NlGram,
             14: NlRowmat, 15: SeFc, 16: SeFcBwd, 17: SoftmaxCe, 18: SoftmaxCeGrad,
-            19: StemConv, 20: BnEval, 21: BlockEval}
+            19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_rmsprop_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -320,6 +347,8 @@ def lib():
         l.yamb_nl_rowmat_fwd.argtypes = [C.POINTER(NlRowmat), C.c_void_p]
         l.yamb_block_eval_fwd.argtypes = [C.POINTER(BlockEval), C.c_void_p]
         l.yamb_block_eval_pool_fwd.argtypes = [C.POINTER(BlockEval), C.c_void_p]
+        l.yamb_instance_norm_fwd.argtypes = [C.POINTER(InFwd), C.c_void_p]
+        l.yamb_instance_norm_bwd.argtypes = [C.POINTER(InBwd), C.c_void_p]
         l.yamb_rmsprop_step.argtypes = [C.POINTER(Rmsprop), C.c_void_p]
         l.yamb_ema_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,
                                       C.c_void_p]
