@@ -454,6 +454,27 @@ typedef struct yamb_rmsprop {
 } yamb_rmsprop;
 
 int yamb_rmsprop_step(const yamb_rmsprop* args, yamb_stream_t stream);
+
+/* ---- fused flat-arena SGD (+L2 decay, +DDP mean, +EMA, +bf16 repack) -----------------------------
+ * Replaces torch.optim.SGD.step with momentum / dampening / nesterov / weight_decay (the reference's
+ * `optimizer: sgd`, utils/optim.py:262-267) over the same flat arenas and with the same services as
+ * yamb_rmsprop: per element
+ *   g = grad_scale*g (+ l2*p where bit 0 of wd_mask is set) (+ weight_decay*p)
+ *   momentum > 0: buf = g on the parameter's first momentum step (bit 2 of wd_mask), else
+ *                 buf = momentum*buf + (1-dampening)*g;  g = g + momentum*buf (nesterov) or buf
+ *   p -= lr*g;  ema = ema_m*ema + (1-ema_m)*p;  p_bf16 = bf16(p)
+ * Bit 1 of wd_mask: the parameter received no gradient this step; only its EMA moves.  `mom` is
+ * required when momentum > 0; nesterov requires momentum > 0 and dampening == 0. */
+typedef struct yamb_sgd {
+  int64_t n;
+  float* p; const float* g; float* mom;
+  float* ema; void* p_bf16; const uint8_t* wd_mask;
+  const float* hyper;         /* optional device [lr, ema_m] */
+  float lr, momentum, dampening, weight_decay, l2, grad_scale, ema_m;
+  int32_t nesterov;
+} yamb_sgd;
+
+int yamb_sgd_step(const yamb_sgd* args, yamb_stream_t stream);
 /* shadow = m*shadow + (1-m)*x over n floats (BN running statistics; common.py:58-63) */
 int yamb_ema_update(float* shadow, const float* x, int64_t n, const float* hyper, float m,
                     yamb_stream_t stream);
@@ -467,7 +488,7 @@ int yamb_max_ctas(void);
 /* sizeof() of the ABI structs (0 bn_fwd, 1 bn_bwd, 2 gemm, 3 dw_fwd, 4 dw_bwd, 5 bn_apply,
  * 6 bn_reduce, 7 se_pool, 8 rmsprop, 9 se_bwd_reduce, 10 se_bwd_apply, 11 bn_stats,
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
- * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd) so bindings
+ * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd) so bindings
  * can self-check */
 int yamb_struct_size(int which);
 

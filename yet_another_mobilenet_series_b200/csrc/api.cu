@@ -48,7 +48,7 @@ PFN_encodeTiled get_encode_tiled() {
 extern "C" {
 
 const char* yamb_last_error(void) { return yamb::g_err; }
-int yamb_version(void) { return 100; }
+int yamb_version(void) { return 101; }
 int yamb_max_ctas(void) { int n = yamb::max_ctas(); return n > 0 ? 4 * n : n; }
 int yamb_struct_size(int which) {
   switch (which) {
@@ -76,6 +76,7 @@ int yamb_struct_size(int which) {
     case 21: return (int)sizeof(yamb_block_eval);
     case 22: return (int)sizeof(yamb_in_fwd);
     case 23: return (int)sizeof(yamb_in_bwd);
+    case 24: return (int)sizeof(yamb_sgd);
     default: return -1;
   }
 }
@@ -111,6 +112,7 @@ int yamb_block_eval_pool_fwd(const yamb_block_eval* a, yamb_stream_t s) { return
 int yamb_instance_norm_fwd(const yamb_in_fwd* a, yamb_stream_t s) { return yamb::in_fwd_launch(a, YAMB_ST(s)); }
 int yamb_instance_norm_bwd(const yamb_in_bwd* a, yamb_stream_t s) { return yamb::in_bwd_launch(a, YAMB_ST(s)); }
 int yamb_rmsprop_step(const yamb_rmsprop* a, yamb_stream_t s) { return yamb::rmsprop_launch(a, YAMB_ST(s)); }
+int yamb_sgd_step(const yamb_sgd* a, yamb_stream_t s) { return yamb::sgd_launch(a, YAMB_ST(s)); }
 int yamb_ema_update(float* shadow, const float* x, int64_t n, const float* hyper, float m,
                     yamb_stream_t s) {
   return yamb::ema_launch(shadow, x, n, hyper, m, YAMB_ST(s));

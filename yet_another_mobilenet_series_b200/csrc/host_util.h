@@ -41,6 +41,7 @@ int block_eval_pool_launch(const yamb_block_eval* a, cudaStream_t stream);
 int in_fwd_launch(const yamb_in_fwd* a, cudaStream_t stream);
 int in_bwd_launch(const yamb_in_bwd* a, cudaStream_t stream);
 int rmsprop_launch(const yamb_rmsprop* a, cudaStream_t stream);
+int sgd_launch(const yamb_sgd* a, cudaStream_t stream);
 int ema_launch(float* shadow, const float* x, long long n, const float* hyper, float m,
                cudaStream_t stream);
 int cast_bf16_launch(const float* src, void* dst, long long n, cudaStream_t stream);

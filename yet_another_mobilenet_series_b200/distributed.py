@@ -3,7 +3,7 @@ per GPU over NCCL (NVLink / NVSwitch inside one node).
 
 The data path of the reference has exactly one exchange step per iteration: the SUM all-reduce of
 all gradients followed by a division by the world size (utils/distributed.py:131-139, called from
-train.py:72-73).  Here the gradients already live in ONE flat fp32 arena (fused_rmsprop.RMSprop),
+train.py:72-73).  Here the gradients already live in ONE flat fp32 arena (fused_rmsprop.RMSprop, fused_sgd.SGD),
 so `allreduce_grads` is a single in-place NCCL all-reduce with no flatten / unflatten copies, and
 the division is folded into the optimizer kernel (`grad_scale`).  BatchNorm statistics stay local
 during training, like the reference (`allreduce_bn: False` in every training yml).

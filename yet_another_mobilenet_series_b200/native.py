@@ -171,6 +171,19 @@ class Rmsprop(C.Structure):
     ]
 
 
+class Sgd(C.Structure):
+    _fields_ = [
+        ("n", C.c_int64),
+        ("p", C.c_void_p), ("g", C.c_void_p), ("mom", C.c_void_p),
+        ("ema", C.c_void_p), ("p_bf16", C.c_void_p), ("wd_mask", C.c_void_p),
+        ("hyper", C.c_void_p),
+        ("lr", C.c_float), ("momentum", C.c_float), ("dampening", C.c_float),
+        ("weight_decay", C.c_float), ("l2", C.c_float), ("grad_scale", C.c_float),
+        ("ema_m", C.c_float),
+        ("nesterov", C.c_int32),
+    ]
+
+
 class SeFc(C.Structure):
     _fields_ = [
         ("N", C.c_int32), ("C", C.c_int32), ("R", C.c_int32), ("act", C.c_int32),
@@ -296,11 +309,11 @@ class InBwd(C.Structure):
 _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnReduce, 7: SePool,
             8: Rmsprop, 9: SeBwdReduce, 10: SeBwdApply, 11: BnStats, 12: BnBwdApply, 13: NlGram,
             14: NlRowmat, 15: SeFc, 16: SeFcBwd, 17: SoftmaxCe, 18: SoftmaxCeGrad,
-            19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd}
+            19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd, 24: Sgd}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -350,6 +363,7 @@ def lib():
         l.yamb_instance_norm_fwd.argtypes = [C.POINTER(InFwd), C.c_void_p]
         l.yamb_instance_norm_bwd.argtypes = [C.POINTER(InBwd), C.c_void_p]
         l.yamb_rmsprop_step.argtypes = [C.POINTER(Rmsprop), C.c_void_p]
+        l.yamb_sgd_step.argtypes = [C.POINTER(Sgd), C.c_void_p]
         l.yamb_ema_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,
                                       C.c_void_p]
         l.yamb_cast_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]

@@ -3,9 +3,11 @@
 One call = one iteration of the reference's hot loop (train.py:64-114): zero_grad, forward,
 label-smoothed cross entropy (utils/optim.py:150-158) [+ top-k counts without the reference's two
 host syncs, common.py:67-80], backward, gradient all-reduce (utils/distributed.py:155-161),
-RMSprop step with the 'mnas' L2 decay, the 1/world mean, the bf16 weight repack and the EMA of the
-weights folded in (utils/rmsprop.py, utils/optim.py:177-200, :53-64) and the EMA of the BatchNorm
-running statistics (common.py:58-63).
+optimizer step with the L2 decay, the 1/world mean, the bf16 weight repack and the EMA of the
+weights folded in, and the EMA of the BatchNorm running statistics (common.py:58-63).  The
+optimizer is the reference's RMSprop (utils/rmsprop.py, the default) or torch.optim.SGD
+(`optimizer="sgd"`, utils/optim.py:262-267), and the L2 rule `cal_l2_loss`'s 'mnas' (the default)
+or 'slimmable' (utils/optim.py:161-200); EMA: utils/optim.py:53-64.
 
 Forward+backward are captured once into a CUDA graph (static input buffers) and replayed; inputs
 arrive through `load(x, target)` which accepts HOST (ideally pinned) or device tensors and copies
@@ -19,6 +21,7 @@ from . import distributed as udist
 from . import engine
 from . import tail_ops
 from .fused_rmsprop import RMSprop
+from .fused_sgd import SGD
 
 
 def label_smooth_ce(logits, target, smoothing):
@@ -31,7 +34,10 @@ def label_smooth_ce(logits, target, smoothing):
 class TrainStep:
     def __init__(self, model, per_gpu_batch, image_size=224, base_lr=0.016, base_total_batch=256,
                  alpha=0.9, momentum=0.9, eps=1e-3, weight_decay=1e-5, label_smoothing=0.1,
-                 ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16):
+                 ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
+                 optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas"):
+        """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
+        `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both."""
         self.model = model
         dev = next(model.parameters()).device
         if dev.type != "cuda":
@@ -41,9 +47,15 @@ class TrainStep:
         self.batch = per_gpu_batch
         gbatch = per_gpu_batch * self.world
         self.lr = base_lr * gbatch / base_total_batch            # reference common.py:204-205
-        self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum, eps=eps,
-                           eps_inside_sqrt=True, weight_decay=0)
-        self.opt.fold_l2(weight_decay, list(model.named_parameters()), "mnas")
+        if optimizer == "rmsprop":
+            self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
+                               eps=eps, eps_inside_sqrt=True, weight_decay=0)
+        elif optimizer == "sgd":                                  # utils/optim.py:262-267
+            self.opt = SGD(model.parameters(), lr=self.lr, momentum=momentum,
+                           dampening=dampening, nesterov=nesterov, weight_decay=0)
+        else:
+            raise ValueError("Unknown optimizer: {}".format(optimizer))
+        self.opt.fold_l2(weight_decay, list(model.named_parameters()), weight_decay_method)
         self.ema_decay = None
         if ema_decay and ema_decay > 0:
             self.ema_decay = ema_decay ** (gbatch / ema_base_batch)  # adjust_momentum, :118-128
