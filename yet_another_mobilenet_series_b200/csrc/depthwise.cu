@@ -37,8 +37,10 @@ int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
   if (!a) return set_error(YAMB_EINVAL, "null args");
   int rc = check_common(a->N, a->H, a->W, a->C, a->ldc, a->k, a->stride);
   if (rc) return rc;
-  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   if (!a->x || !a->y || !a->w) return set_error(YAMB_EINVAL, "depthwise fwd: null pointer");
+  if ((((uintptr_t)a->x) | ((uintptr_t)a->y)) & 15)
+    return set_error(YAMB_EINVAL, "depthwise: activations must be 16-byte aligned");
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   const int k = a->k, s = a->stride, pad = (k - 1) / 2;
   const int ct = pick_ct(a->C, (a->H + 2 * pad - k) / s + 1);
   DwFwdDev p;
@@ -50,8 +52,6 @@ int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
   p.w = a->w;
   p.has_bn = a->bn ? 1 : 0;
   if (a->bn) p.bn = *a->bn;
-  if ((((uintptr_t)a->x) | ((uintptr_t)a->y)) & 15)
-    return set_error(YAMB_EINVAL, "depthwise: activations must be 16-byte aligned");
   const int tw = (k == 7 || p.Wo <= 8) ? 1 : 2;
   const int toh = 512 / ct, tow = 8 * tw;   // (256 / (ct / 4) strips / 8 columns) x 4 rows
   p.tiles_h = (p.Ho + toh - 1) / toh;
@@ -88,9 +88,15 @@ int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
   if (!a) return set_error(YAMB_EINVAL, "null args");
   int rc = check_common(a->N, a->H, a->W, a->C, a->ldc, a->k, a->stride);
   if (rc) return rc;
-  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   if (!a->ca || !a->cb || !a->cc || !a->dz || !a->h || !a->x || !a->dx || !a->dw || !a->w)
     return set_error(YAMB_EINVAL, "depthwise bwd: null pointer");
+  // dz, h and x stream into shared memory in 16-byte cp.async pieces; dx is stored and residual
+  // read 4 channels (8 bytes) at a time
+  if ((((uintptr_t)a->dz) | ((uintptr_t)a->h) | ((uintptr_t)a->x)) & 15)
+    return set_error(YAMB_EINVAL, "depthwise bwd: dz, h and x must be 16-byte aligned");
+  if ((((uintptr_t)a->dx) | ((uintptr_t)a->residual)) & 7)
+    return set_error(YAMB_EINVAL, "depthwise bwd: dx and residual must be 8-byte aligned");
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   const int k = a->k, s = a->stride, pad = (k - 1) / 2;
   const int ct = pick_ct(a->C, a->H);
   DwBwdDev p;
