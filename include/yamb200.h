@@ -237,7 +237,9 @@ typedef struct yamb_se_bwd_apply {
  * models/mobilenet_base.py:110-113 se_reduce / active_fn / se_expand / sigmoid) and their backward,
  * fp32:  u = W_r s + b_r, v = act(u), gate = sigmoid(W_e v + b_e);
  * backward: dt = dgate*gate*(1-gate), du = (W_e^T dt)*act'(u), dpool = (W_r^T du)*inv_hw, and the
- * parameter gradients ACCUMULATED (+=) into g_* (sums over the N samples, no atomics). */
+ * parameter gradients ACCUMULATED (+=) into g_* (sums over the N samples).  No float atomics: the
+ * split-K products u, du and the bias-gradient column sums add per-CTA slabs in a fixed order, so
+ * every call computes the same bits. */
 typedef struct yamb_se_fc {
   int32_t N, C, R; int32_t act;
   const float* pooled;                     /* [N][C] */
@@ -245,7 +247,6 @@ typedef struct yamb_se_fc {
   const float* w_e; const float* b_e;      /* [C][R], [C]  (se_expand) */
   float* u; float* v;                      /* out [N][R]: saved for backward */
   float* gate;                             /* out [N][C] */
-  int32_t deterministic;                   /* 1: no split-K over C (the same bits on every run) */
 } yamb_se_fc;
 
 typedef struct yamb_se_fc_grad {
@@ -285,9 +286,9 @@ typedef struct yamb_nl_gram {
   const void* X; int64_t ldx; int32_t I;
   const void* Y; int64_t ldy; int32_t J;   /* J, ldy even */
   float alpha;
-  float* G;                                /* [N][I][J] */
-  int32_t deterministic;                   /* 1: per-CTA partial sums added in a fixed order
-                                            * (the same bits on every run); 0: fp32 atomics */
+  float* G;                                /* [N][I][J]; the per-CTA row-chunk partial sums
+                                            * are added in a fixed order (the same bits on
+                                            * every run) */
 } yamb_nl_gram;
 
 typedef struct yamb_nl_rowmat {

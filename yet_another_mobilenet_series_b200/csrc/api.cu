@@ -48,7 +48,7 @@ PFN_encodeTiled get_encode_tiled() {
 extern "C" {
 
 const char* yamb_last_error(void) { return yamb::g_err; }
-int yamb_version(void) { return 101; }
+int yamb_version(void) { return 102; }
 int yamb_max_ctas(void) { int n = yamb::max_ctas(); return n > 0 ? 4 * n : n; }
 int yamb_struct_size(int which) {
   switch (which) {

@@ -44,21 +44,22 @@ int det_free(float* part, cudaStream_t st) {
   return 0;
 }
 
-// out[i] += sum over s = 0 .. nslab-1 of part[s * n + i], in that order
+// out[i] (+)= sum over s = 0 .. nslab-1 of part[s * n + i], in that order
 __global__ void __launch_bounds__(256) det_reduce_kernel(const float* __restrict__ part, int nslab,
-                                                         long long n, float* __restrict__ out) {
+                                                         long long n, float* __restrict__ out,
+                                                         bool add) {
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
     float s = 0.f;
     for (int k = 0; k < nslab; ++k) s += part[(size_t)k * n + i];
-    out[i] += s;
+    out[i] = add ? out[i] + s : s;
   }
 }
 
-int det_reduce_launch(float* part, int nslab, long long n, float* out, cudaStream_t st) {
+int det_reduce_launch(float* part, int nslab, long long n, float* out, cudaStream_t st, bool add) {
   if (n > 0 && nslab > 0) {
     const long long blocks = (n + 255) / 256;
     const long long cap = 4LL * (max_ctas() > 0 ? max_ctas() : 1);
-    det_reduce_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(part, nslab, n, out);
+    det_reduce_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(part, nslab, n, out, add);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
       det_free(part, st);

@@ -301,17 +301,19 @@ struct SePoolDev {
   const __nv_bfloat16* h;
   const float *scale, *shift;
   int act;
-  float* pooled;  // [N][out_ld]
+  float* pooled;  // [pixel chunks][N][out_ld] slabs (slab = pixel-chunk stride)
   int out_ld;
+  long long slab;
 };
 // grid (pixel chunks, N); thread = (8-channel group cg, pixel lane px): whole 16-byte-per-lane rows
 // are read (every lane busy whatever C is), 4 rows in flight per thread, lanes reduced through
-// shared memory, one fp32 reduction per (n, c) per CTA into the pre-zeroed output.
+// shared memory, then one plain store per (n, c) into the slab of this CTA's pixel chunk
+// (out + blockIdx.x * slab); the launcher adds the slabs in slab order.
 template <bool kBwd>
 __device__ __forceinline__ void se_rows_reduce(int N, int HW, int C, const __nv_bfloat16* h, int ldh,
                                                const __nv_bfloat16* dy, int ldd, const float* scale,
                                                const float* shift, int act, float out_scale,
-                                               float* out, int out_ld) {
+                                               float* out, int out_ld, long long slab) {
   __shared__ float red[256][9];
   const int CG = C / 8;
   const int PX = 256 / CG;                       // pixel lanes (host guarantees CG <= 256)
@@ -370,14 +372,14 @@ __device__ __forceinline__ void se_rows_reduce(int N, int HW, int C, const __nv_
     for (int e = 0; e < 8; ++e) {
       float t = 0.f;
       for (int j = 0; j < PX; ++j) t += red[j * CG + cg][e];
-      atomicAdd(out + (size_t)n * out_ld + cg * 8 + e, t * out_scale);
+      out[(size_t)blockIdx.x * slab + (size_t)n * out_ld + cg * 8 + e] = t * out_scale;
     }
   }
 }
 
 __global__ void __launch_bounds__(256) se_pool_kernel(const __grid_constant__ SePoolDev p) {
   se_rows_reduce<false>(p.N, p.HW, p.C, p.h, p.ldh, nullptr, 0, p.scale, p.shift, p.act,
-                        1.f / (float)p.HW, p.pooled, p.out_ld);
+                        1.f / (float)p.HW, p.pooled, p.out_ld, p.slab);
 }
 
 // dgate[n][c] = sum over HW of dY[n,hw,c] * round_bf16(act(scale*h + shift))  (SE backward, the
@@ -388,12 +390,13 @@ struct SeBwdReduceDev {
   const __nv_bfloat16* h;
   const float *scale, *shift;
   int act;
-  float* dgate;  // [N][out_ld]
+  float* dgate;  // [pixel chunks][N][out_ld] slabs, as SePoolDev::pooled
   int out_ld;
+  long long slab;
 };
 __global__ void __launch_bounds__(256) se_bwd_reduce_kernel(const __grid_constant__ SeBwdReduceDev p) {
   se_rows_reduce<true>(p.N, p.HW, p.C, p.h, p.ldh, p.dy, p.ldd, p.scale, p.shift, p.act, 1.f,
-                       p.dgate, p.out_ld);
+                       p.dgate, p.out_ld, p.slab);
 }
 
 // dz = (dY * gate[n][c] + dpool[n][c]) * act'(scale*h + shift)   (in place allowed: dz == dY)
@@ -556,6 +559,27 @@ static int se_chunks(int N, int HW, int C) {
   return want < 1 ? 1 : want;
 }
 
+// Slabs of the [N][C] sums of se_rows_reduce, one per pixel chunk: a stream-ordered scratch when
+// there are several (det_reduce stores their sum in chunk order afterwards), the output itself
+// when there is one.  A thread owns one 8-channel group, so channels go in launches of 2048; the
+// chunk count comes from the widest one and is the same for all.
+static int se_slabs(int N, int HW, int C, float* out, cudaStream_t st, int* chunks, float** part) {
+  *chunks = se_chunks(N, HW, C < 2048 ? C : 2048);
+  *part = out;
+  if (*chunks == 1) return 0;
+  return det_alloc((size_t)*chunks * N * C * sizeof(float), st, part);
+}
+
+static int se_slabs_done(float* part, int chunks, int N, int C, float* out, cudaStream_t st,
+                         const char* what) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    if (part != out) det_free(part, st);
+    return set_error(YAMB_ECUDA, "%s: %s", what, cudaGetErrorString(e));
+  }
+  return part != out ? det_reduce_launch(part, chunks, (long long)N * C, out, st, false) : 0;
+}
+
 int se_pool_launch(const yamb_se_pool* a, cudaStream_t st) {
   if (!a || a->N <= 0 || a->HW <= 0 || a->C <= 0 || (a->C % 8))
     return set_error(YAMB_EINVAL, "se_pool shape");
@@ -563,21 +587,20 @@ int se_pool_launch(const yamb_se_pool* a, cudaStream_t st) {
   SePoolDev p;
   p.N = a->N; p.HW = a->HW; p.C = a->C; p.ldh = a->ldh;
   p.h = (const __nv_bfloat16*)a->h; p.scale = a->scale; p.shift = a->shift; p.act = a->act;
-  p.pooled = a->pooled;
   if (a->N > 65535) return set_error(YAMB_EINVAL, "se_pool: N <= 65535");
-  cudaError_t e = cudaMemsetAsync(a->pooled, 0, (size_t)a->N * a->C * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_pool memset: %s", cudaGetErrorString(e));
+  int chunks;
+  int rc = se_slabs(a->N, a->HW, a->C, a->pooled, st, &chunks, &p.pooled);
+  if (rc) return rc;
   p.out_ld = a->C;
-  for (int c0 = 0; c0 < a->C; c0 += 2048) {       // a thread owns one 8-channel group: <= 256 per CTA
+  p.slab = (long long)a->N * a->C;
+  for (int c0 = 0; c0 < a->C; c0 += 2048) {
     SePoolDev q = p;
     q.C = a->C - c0 < 2048 ? a->C - c0 : 2048;
     q.h = p.h + c0; q.scale = p.scale + c0; q.shift = p.shift + c0; q.pooled = p.pooled + c0;
-    dim3 grid(se_chunks(a->N, a->HW, q.C), a->N);
+    dim3 grid(chunks, a->N);
     se_pool_kernel<<<grid, 256, 0, st>>>(q);
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_pool: %s", cudaGetErrorString(e));
-  return 0;
+  return se_slabs_done(p.pooled, chunks, a->N, a->C, a->pooled, st, "se_pool");
 }
 
 int se_bwd_reduce_launch(const yamb_se_bwd_reduce* a, cudaStream_t st) {
@@ -587,22 +610,22 @@ int se_bwd_reduce_launch(const yamb_se_bwd_reduce* a, cudaStream_t st) {
   SeBwdReduceDev p;
   p.N = a->N; p.HW = a->HW; p.C = a->C; p.ldd = a->ldd; p.ldh = a->ldh;
   p.dy = (const __nv_bfloat16*)a->dy; p.h = (const __nv_bfloat16*)a->h;
-  p.scale = a->scale; p.shift = a->shift; p.act = a->act; p.dgate = a->dgate;
+  p.scale = a->scale; p.shift = a->shift; p.act = a->act;
   if (a->N > 65535) return set_error(YAMB_EINVAL, "se_bwd_reduce: N <= 65535");
-  cudaError_t e = cudaMemsetAsync(a->dgate, 0, (size_t)a->N * a->C * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_bwd_reduce memset: %s", cudaGetErrorString(e));
+  int chunks;
+  int rc = se_slabs(a->N, a->HW, a->C, a->dgate, st, &chunks, &p.dgate);
+  if (rc) return rc;
   p.out_ld = a->C;
+  p.slab = (long long)a->N * a->C;
   for (int c0 = 0; c0 < a->C; c0 += 2048) {
     SeBwdReduceDev q = p;
     q.C = a->C - c0 < 2048 ? a->C - c0 : 2048;
     q.h = p.h + c0; q.dy = p.dy + c0; q.scale = p.scale + c0; q.shift = p.shift + c0;
     q.dgate = p.dgate + c0;
-    dim3 grid(se_chunks(a->N, a->HW, q.C), a->N);
+    dim3 grid(chunks, a->N);
     se_bwd_reduce_kernel<<<grid, 256, 0, st>>>(q);
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_bwd_reduce: %s", cudaGetErrorString(e));
-  return 0;
+  return se_slabs_done(p.dgate, chunks, a->N, a->C, a->dgate, st, "se_bwd_reduce");
 }
 
 int se_bwd_apply_launch(const yamb_se_bwd_apply* a, cudaStream_t st) {

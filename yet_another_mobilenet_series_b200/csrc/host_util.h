@@ -47,9 +47,11 @@ int ema_launch(float* shadow, const float* x, long long n, const float* hyper, f
 int cast_bf16_launch(const float* src, void* dst, long long n, cudaStream_t stream);
 
 // deterministic reductions (det_reduce.cu): a stream-ordered scratch per launch; det_reduce_launch
-// adds its nslab slabs of n floats into out in slab order and releases it on the same stream
+// adds its nslab slabs of n floats in slab order into out (add) or stores their sum (!add), and
+// releases the scratch on the same stream
 int det_alloc(size_t bytes, cudaStream_t stream, float** out);
 int det_free(float* part, cudaStream_t stream);
-int det_reduce_launch(float* part, int nslab, long long n, float* out, cudaStream_t stream);
+int det_reduce_launch(float* part, int nslab, long long n, float* out, cudaStream_t stream,
+                      bool add = true);
 
 }  // namespace yamb

@@ -30,9 +30,8 @@ struct NlGramDev {
   const __nv_bfloat16* X; long long ldx; int I;
   const __nv_bfloat16* Y; long long ldy; int J;
   float alpha;
-  float* G;
   int rows_per_cta;
-  float* part;       // deterministic: [row chunks][N][I][J] slabs (plain stores), else NULL
+  float* part;       // [row chunks][N][I][J] slabs (plain stores), G itself for one chunk
 };
 
 // pixel index (inside one sample) of the r-th row of the row set
@@ -40,7 +39,8 @@ __device__ __forceinline__ int nl_row_pixel(int r, int W, int sub, int Ws) {
   return sub == 1 ? r : (r / Ws) * sub * W + (r % Ws) * sub;
 }
 
-// G[n][i][j] += alpha * sum_r X[n, pix(r), i] * Y[n, pix(r), j]     grid = (row chunks, N)
+// part[chunk][n][i][j] = alpha * sum over the chunk's rows r of X[n, pix(r), i] * Y[n, pix(r), j]
+// grid = (row chunks, N); the launcher adds the chunk slabs into G in chunk order
 __global__ void __launch_bounds__(256) nl_gram_kernel(const __grid_constant__ NlGramDev p) {
   extern __shared__ __align__(16) unsigned char nl_smem[];
   const int R = p.rows_per_cta;
@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(256) nl_gram_kernel(const __grid_constant__ Nl
   }
   __syncthreads();
   const int IP = I2 / 2, JP = p.J / 2;
-  float* G = p.G + (size_t)n * p.I * p.J;
+  float* S = p.part + ((size_t)blockIdx.x * p.N + n) * p.I * p.J;   // this CTA's slab
   for (int w = threadIdx.x; w < IP * JP; w += 256) {
     const int ip = w / JP, jp = w % JP;            // consecutive threads: consecutive column pairs
     float a00 = 0.f, a01 = 0.f, a10 = 0.f, a11 = 0.f;
@@ -79,21 +79,11 @@ __global__ void __launch_bounds__(256) nl_gram_kernel(const __grid_constant__ Nl
       a10 = fmaf(x1, y0, a10); a11 = fmaf(x1, y1, a11);
     }
     const int i = 2 * ip, j = 2 * jp;
-    if (p.part) {   // this CTA's slab: every element written once, det_reduce adds the slabs in order
-      float* S = p.part + ((size_t)blockIdx.x * p.N + n) * p.I * p.J;
-      S[(size_t)i * p.J + j] = p.alpha * a00;
-      S[(size_t)i * p.J + j + 1] = p.alpha * a01;
-      if (i + 1 < p.I) {
-        S[(size_t)(i + 1) * p.J + j] = p.alpha * a10;
-        S[(size_t)(i + 1) * p.J + j + 1] = p.alpha * a11;
-      }
-      continue;
-    }
-    atomicAdd(G + (size_t)i * p.J + j, p.alpha * a00);
-    atomicAdd(G + (size_t)i * p.J + j + 1, p.alpha * a01);
+    S[(size_t)i * p.J + j] = p.alpha * a00;
+    S[(size_t)i * p.J + j + 1] = p.alpha * a01;
     if (i + 1 < p.I) {
-      atomicAdd(G + (size_t)(i + 1) * p.J + j, p.alpha * a10);
-      atomicAdd(G + (size_t)(i + 1) * p.J + j + 1, p.alpha * a11);
+      S[(size_t)(i + 1) * p.J + j] = p.alpha * a10;
+      S[(size_t)(i + 1) * p.J + j + 1] = p.alpha * a11;
     }
   }
 }
@@ -198,17 +188,20 @@ int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t st) {
   p.Hs = (a->H + a->sub - 1) / a->sub; p.Ws = (a->W + a->sub - 1) / a->sub;
   p.X = (const __nv_bfloat16*)a->X; p.ldx = a->ldx; p.I = a->I;
   p.Y = (const __nv_bfloat16*)a->Y; p.ldy = a->ldy; p.J = a->J;
-  p.alpha = a->alpha; p.G = a->G; p.part = nullptr;
+  p.alpha = a->alpha;
   const int rows = p.Hs * p.Ws;
   const int I2 = (a->I + 1) & ~1;
+  const long long n_out = (long long)a->N * a->I * a->J;
   int R = rows < 64 ? rows : 64;
-  // more row chunks when the batch alone cannot fill the SMs
-  while (R > 16 && (long long)((rows + R - 1) / R) * a->N < 2LL * max_ctas()) R /= 2;
+  // more row chunks when the batch alone cannot fill the SMs, as long as their slabs stay small
+  // next to the L2 (every chunk writes and the reduction reads back a full [N][I][J] slab)
+  while (R > 16 && (long long)((rows + R - 1) / R) * a->N < 2LL * max_ctas() &&
+         (long long)((rows + R / 2 - 1) / (R / 2)) * n_out * 4 <= (16LL << 20))
+    R /= 2;
   p.rows_per_cta = R;
   const size_t smem = (size_t)R * (I2 + a->J) * 2;
   if (smem > 200 * 1024) return set_error(YAMB_EINVAL, "nl_gram: rows too wide for shared memory");
-  cudaError_t e = cudaMemsetAsync(a->G, 0, (size_t)a->N * a->I * a->J * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "nl_gram memset: %s", cudaGetErrorString(e));
+  cudaError_t e;
   static size_t attr = 0;   // process-wide: only ever raise the limit
   if (smem > attr) {
     e = cudaFuncSetAttribute(nl_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -216,19 +209,15 @@ int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t st) {
     attr = smem;
   }
   dim3 grid((rows + R - 1) / R, a->N);
-  const long long n_out = (long long)a->N * a->I * a->J;
-  if (a->deterministic) {
-    rc = det_alloc((size_t)grid.x * n_out * sizeof(float), st, &p.part);
-    if (rc) return rc;
-  }
+  p.part = a->G;
+  if (grid.x > 1 && (rc = det_alloc((size_t)grid.x * n_out * sizeof(float), st, &p.part))) return rc;
   nl_gram_kernel<<<grid, 256, smem, st>>>(p);
   e = cudaGetLastError();
   if (e != cudaSuccess) {
-    if (p.part) det_free(p.part, st);
+    if (p.part != a->G) det_free(p.part, st);
     return set_error(YAMB_ECUDA, "nl_gram: %s", cudaGetErrorString(e));
   }
-  if (p.part) return det_reduce_launch(p.part, (int)grid.x, n_out, a->G, st);
-  return 0;
+  return p.part != a->G ? det_reduce_launch(p.part, (int)grid.x, n_out, a->G, st, false) : 0;
 }
 
 int nl_rowmat_launch(const yamb_nl_rowmat* a, cudaStream_t st) {

@@ -9,6 +9,9 @@
 //             dW_e += dt^T v, db_e += sum dt, dW_r += du^T s, db_r += sum du   (sums over samples)
 // fp32 throughout (the reference keeps these tiny layers in fp32 too).  Every product is one launch
 // of a small tiled SGEMM with the bias / activation / sigmoid / act' step as its epilogue.
+// No float atomics: the split-K products u and du store one slab per K slab and the finish kernel
+// adds the slabs in slab order; the bias gradients are column sums per sample slab, added into
+// g_b* in slab order by det_reduce.  Every call computes the same bits.
 // C <= 4096, R <= 1024.
 #include <cuda_runtime.h>
 #include <string.h>
@@ -30,15 +33,11 @@ struct SeGemm {
   const float* B; long long b_rs, b_cs;
   float* C; long long c_rs;          // C[m*c_rs + n]
   float alpha;
-  int epi;                           // 0 store alpha*acc | 1 u=acc+bias: C=u, C2=act(u) | 2 C=sigmoid(acc+bias)
-                                     // 3 C=acc*act'(E[m][n]) (+ column sums into colsum) | 4 C += acc
-                                     // 5 atomicAdd(C, acc): split-K partial sums (grid.z slabs)
-  int k_per_slab;                    // K range of one grid.z slab (epi 5), else K
+  int epi;                           // 0 store alpha*acc | 1 C=sigmoid(acc+bias) | 2 C += acc
+                                     // 3 split-K: slab z = blockIdx.z of C, C[z*M*c_rs + m*c_rs + n] = acc
+                                     //   (plain stores; the caller adds the slabs in slab order)
+  int k_per_slab;                    // K range of one grid.z slab (se_split), 0 = all of K
   const float* bias;                 // [N]
-  const float* E; long long e_rs;    // epi 3
-  float* C2;                         // epi 1 second output, same layout as C
-  float* colsum;                     // epi 3: colsum[n] += sum_m C[m][n]
-  int act;
 };
 
 constexpr int kSgT = 64, kSgK = 16;
@@ -46,7 +45,6 @@ constexpr int kSgT = 64, kSgK = 16;
 __global__ void __launch_bounds__(256) se_gemm_kernel(const __grid_constant__ SeGemm p) {
   __shared__ float sA[kSgK][kSgT + 4];
   __shared__ float sB[kSgK][kSgT + 4];
-  __shared__ float s_col[kSgT];
   const int tid = threadIdx.x;
   const int m0 = blockIdx.y * kSgT, n0 = blockIdx.x * kSgT;
   const int tm = (tid / 16) * 4, tn = (tid % 16) * 4;      // this thread's 4 x 4 outputs
@@ -87,11 +85,7 @@ __global__ void __launch_bounds__(256) se_gemm_kernel(const __grid_constant__ Se
     }
     __syncthreads();
   }
-  if (p.epi == 3 && p.colsum) {
-    if (tid < kSgT) s_col[tid] = 0.f;
-    __syncthreads();
-  }
-  float csum[4] = {0.f, 0.f, 0.f, 0.f};
+  float* C = p.epi == 3 ? p.C + (size_t)blockIdx.z * p.M * p.c_rs : p.C;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int m = m0 + tm + i;
@@ -101,27 +95,25 @@ __global__ void __launch_bounds__(256) se_gemm_kernel(const __grid_constant__ Se
       const int n = n0 + tn + j;
       if (n >= p.N) continue;
       float v = acc[i][j] * p.alpha;
-      float* c = p.C + (size_t)m * p.c_rs + n;
+      float* c = C + (size_t)m * p.c_rs + n;
       switch (p.epi) {
-        case 1: { v += p.bias[n]; *c = v; p.C2[(size_t)m * p.c_rs + n] = act_fwd(v, p.act); break; }
-        case 2: { v += p.bias[n]; *c = 1.f / (1.f + __expf(-v)); break; }
-        case 3: { v *= act_bwd(p.E[(size_t)m * p.e_rs + n], p.act); *c = v; csum[j] += v; break; }
-        case 4: *c += v; break;
-        case 5: atomicAdd(c, v); break;
+        case 1: { v += p.bias[n]; *c = 1.f / (1.f + __expf(-v)); break; }
+        case 2: *c += v; break;
         default: *c = v;
       }
     }
   }
-  if (p.epi == 3 && p.colsum) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) atomicAdd(&s_col[tn + j], csum[j]);
-    __syncthreads();
-    if (tid < kSgT && n0 + tid < p.N) atomicAdd(p.colsum + n0 + tid, s_col[tid]);
-  }
 }
 
-static cudaError_t se_gemm(SeGemm g, cudaStream_t st, int ksplit = 1) {
+// Sets the K range of one slab for `ksplit` slabs (a multiple of the K chunk) and returns the
+// number of slabs the launch writes, which can be less than ksplit.
+static int se_split(SeGemm& g, int ksplit) {
   g.k_per_slab = ((g.K + ksplit - 1) / ksplit + kSgK - 1) / kSgK * kSgK;
+  return (g.K + g.k_per_slab - 1) / g.k_per_slab;
+}
+
+static cudaError_t se_gemm(SeGemm g, cudaStream_t st) {
+  if (g.k_per_slab <= 0) g.k_per_slab = g.K;
   dim3 grid((g.N + kSgT - 1) / kSgT, (g.M + kSgT - 1) / kSgT, (g.K + g.k_per_slab - 1) / g.k_per_slab);
   se_gemm_kernel<<<grid, 256, 0, st>>>(g);
   return cudaGetLastError();
@@ -137,32 +129,48 @@ static int se_ksplit(int M, int N, int K) {
   return want < 1 ? 1 : want;
 }
 
-// finish of the split-K products:  u += b_r, v = act(u)   |   du = acc * act'(u), db_r += col sums
-__global__ void __launch_bounds__(256) se_finish_kernel(int N, int R, float* u, float* v,
-                                                        const float* b_r, const float* u_saved,
-                                                        float* g_br, int act, int mode) {
-  const int j = blockIdx.x * 256 + threadIdx.x;
-  if (j >= R) return;
-  const int n0 = blockIdx.y * 32, n1 = min(N, n0 + 32);
-  float s = 0.f;
-  for (int n = n0; n < n1; ++n) {
-    const size_t i = (size_t)n * R + j;
+// finish of the split-K products u, du [N][R]; CTA = 32 columns x 8 samples, thread = one
+// element: acc = the nslab slabs part[z][N][R] added in slab order, then
+//   mode 0: u = acc + b_r, v = act(u)
+//   mode 1: du = acc * act'(u_saved), and colpart[blockIdx.y][j] = sum of du over the CTA's 8
+//           samples in sample order (one slab of the db_r column sums)
+// part may be u (mode 0) or du (mode 1) itself when nslab == 1.
+__global__ void __launch_bounds__(256) se_finish_kernel(int N, int R, const float* part, int nslab,
+                                                        float* u, float* v, const float* b_r,
+                                                        const float* u_saved, float* colpart,
+                                                        int act, int mode) {
+  __shared__ float s_col[8][33];
+  const int j = blockIdx.x * 32 + threadIdx.x, n = blockIdx.y * 8 + threadIdx.y;
+  float d = 0.f;
+  if (j < R && n < N) {
+    const size_t i = (size_t)n * R + j, slab = (size_t)N * R;
+    float a = 0.f;
+#pragma unroll 4
+    for (int z = 0; z < nslab; ++z) a += part[z * slab + i];
     if (mode == 0) {
-      const float x = u[i] + b_r[j];
+      const float x = a + b_r[j];
       u[i] = x;
       v[i] = act_fwd(x, act);
     } else {
-      const float d = u[i] * act_bwd(u_saved[i], act);   // here `u` is the du accumulator
+      d = a * act_bwd(u_saved[i], act);   // here `u` is du
       u[i] = d;
-      s += d;
     }
   }
-  if (mode == 1) atomicAdd(g_br + j, s);
+  if (mode == 1) {
+    s_col[threadIdx.y][threadIdx.x] = d;
+    __syncthreads();
+    if (threadIdx.y == 0 && j < R) {
+      float s = 0.f;
+      for (int r = 0; r < 8; ++r) s += s_col[r][threadIdx.x];
+      colpart[(size_t)blockIdx.y * R + j] = s;
+    }
+  }
 }
 
-// dt = dgate * gate * (1 - gate); g_be[c] += sum_n dt[n][c]     thread = channel, CTA = sample slab
+// dt = dgate * gate * (1 - gate); colpart[blockIdx.y][c] = sum of dt over this CTA's samples (one
+// slab of the db_e column sums)          thread = channel, CTA = sample slab
 __global__ void __launch_bounds__(256) se_dt_kernel(int N, int C, const float* dgate, const float* gate,
-                                                    float* dt, float* g_be, int rows_per_cta) {
+                                                    float* dt, float* colpart, int rows_per_cta) {
   const int c = blockIdx.x * 256 + threadIdx.x;
   if (c >= C) return;
   const int n0 = blockIdx.y * rows_per_cta, n1 = min(N, n0 + rows_per_cta);
@@ -173,14 +181,44 @@ __global__ void __launch_bounds__(256) se_dt_kernel(int N, int C, const float* d
     dt[(size_t)n * C + c] = v;
     s += v;
   }
-  atomicAdd(g_be + c, s);
+  colpart[(size_t)blockIdx.y * C + c] = s;
 }
 
 static int se_fc_check(int N, int C, int R) {
-  if (N <= 0 || C <= 0 || R <= 0 || C > 4096 || R > 1024)
+  if (N <= 0 || C <= 0 || R <= 0 || C > 4096 || R > 1024 || N > 8 * 65535)
     return set_error(YAMB_EINVAL, "se_fc: N=%d C=%d R=%d", N, C, R);
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   return 0;
+}
+
+// The split-K product [N][R] (u or du) of g, K = C: each K slab stored into its own slab of a
+// stream-ordered scratch *part, or straight into `out` when there is only one slab (*part = out).
+// The slab count depends on the shape and the device only, so the order of the sum does too.
+static int se_split_product(SeGemm g, float* out, cudaStream_t st, float** part, int* nslab,
+                            const char* what) {
+  *nslab = se_split(g, se_ksplit(g.M, g.N, g.K));
+  *part = out;
+  if (*nslab > 1) {
+    int rc = det_alloc((size_t)*nslab * g.M * g.N * sizeof(float), st, part);
+    if (rc) return rc;
+  }
+  g.C = *part; g.c_rs = g.N; g.epi = 3;
+  cudaError_t e = se_gemm(g, st);
+  if (e != cudaSuccess) {
+    if (*part != out) det_free(*part, st);
+    return set_error(YAMB_ECUDA, "se_fc %s: %s", what, cudaGetErrorString(e));
+  }
+  return 0;
+}
+
+// se_finish_kernel launch check; releases the split-K scratch
+static int se_finish_done(float* part, float* out, cudaStream_t st, const char* what) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    if (part != out) det_free(part, st);
+    return set_error(YAMB_ECUDA, "se_fc %s: %s", what, cudaGetErrorString(e));
+  }
+  return part != out ? det_free(part, st) : 0;
 }
 
 int se_fc_fwd_launch(const yamb_se_fc* a, cudaStream_t st) {
@@ -195,23 +233,23 @@ int se_fc_fwd_launch(const yamb_se_fc* a, cudaStream_t st) {
   g.M = a->N; g.N = a->R; g.K = a->C;
   g.A = a->pooled; g.a_rs = a->C; g.a_cs = 1;
   g.B = a->w_r; g.b_rs = 1; g.b_cs = a->C;
-  g.C = a->u; g.c_rs = a->R; g.alpha = 1.f; g.epi = 5;
-  cudaError_t e = cudaMemsetAsync(a->u, 0, (size_t)a->N * a->R * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc memset: %s", cudaGetErrorString(e));
-  // deterministic: one K slab, so every u element is one atomicAdd onto the zeroed buffer
-  e = se_gemm(g, st, a->deterministic ? 1 : se_ksplit(g.M, g.N, g.K));
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc fwd (reduce): %s", cudaGetErrorString(e));
+  g.alpha = 1.f;
+  float* part;
+  int nslab;
+  if ((rc = se_split_product(g, a->u, st, &part, &nslab, "fwd (reduce)"))) return rc;
   {
-    dim3 fg((a->R + 255) / 256, (a->N + 31) / 32);
-    se_finish_kernel<<<fg, 256, 0, st>>>(a->N, a->R, a->u, a->v, a->b_r, nullptr, nullptr, a->act, 0);
+    dim3 fg((a->R + 31) / 32, (a->N + 7) / 8);
+    se_finish_kernel<<<fg, dim3(32, 8), 0, st>>>(a->N, a->R, part, nslab, a->u, a->v, a->b_r,
+                                                 nullptr, nullptr, a->act, 0);
+    if ((rc = se_finish_done(part, a->u, st, "fwd (finish)"))) return rc;
   }
   // gate[N][C] = sigmoid(v[N][R] * W_e[C][R]^T + b_e)
   memset(&g, 0, sizeof(g));
   g.M = a->N; g.N = a->C; g.K = a->R;
   g.A = a->v; g.a_rs = a->R; g.a_cs = 1;
   g.B = a->w_e; g.b_rs = 1; g.b_cs = a->R;
-  g.C = a->gate; g.c_rs = a->C; g.alpha = 1.f; g.epi = 2; g.bias = a->b_e;
-  e = se_gemm(g, st);
+  g.C = a->gate; g.c_rs = a->C; g.alpha = 1.f; g.epi = 1; g.bias = a->b_e;
+  cudaError_t e = se_gemm(g, st);
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc fwd (expand): %s", cudaGetErrorString(e));
   return 0;
 }
@@ -223,28 +261,45 @@ int se_fc_bwd_launch(const yamb_se_fc_grad* a, cudaStream_t st) {
   if (!a->dgate || !a->gate || !a->u || !a->v || !a->pooled || !a->w_r || !a->w_e || !a->dpool ||
       !a->dt || !a->du || !a->g_wr || !a->g_br || !a->g_we || !a->g_be)
     return set_error(YAMB_EINVAL, "se_fc bwd: null pointer");
-  // dt = dgate * gate * (1 - gate), db_e += column sums
-  {
-    const int rows = 32;
-    dim3 grid((a->C + 255) / 256, (a->N + rows - 1) / rows);
-    se_dt_kernel<<<grid, 256, 0, st>>>(a->N, a->C, a->dgate, a->gate, a->dt, a->g_be, rows);
-  }
-  SeGemm g;
   cudaError_t e;
-  // du[N][R] = (dt[N][C] * W_e[C][R]) * act'(u), db_r += column sums
+  float* colpart;
+  // dt = dgate * gate * (1 - gate), db_e += column sums (slabs of 32 samples)
+  int nrow = (a->N + 31) / 32;
+  if ((rc = det_alloc((size_t)nrow * a->C * sizeof(float), st, &colpart))) return rc;
+  {
+    dim3 grid((a->C + 255) / 256, nrow);
+    se_dt_kernel<<<grid, 256, 0, st>>>(a->N, a->C, a->dgate, a->gate, a->dt, colpart, 32);
+    if ((e = cudaGetLastError()) != cudaSuccess) {
+      det_free(colpart, st);
+      return set_error(YAMB_ECUDA, "se_fc bwd (dt): %s", cudaGetErrorString(e));
+    }
+  }
+  if ((rc = det_reduce_launch(colpart, nrow, a->C, a->g_be, st))) return rc;
+  SeGemm g;
+  // du[N][R] = (dt[N][C] * W_e[C][R]) * act'(u), db_r += column sums (slabs of 8 samples)
   memset(&g, 0, sizeof(g));
   g.M = a->N; g.N = a->R; g.K = a->C;
   g.A = a->dt; g.a_rs = a->C; g.a_cs = 1;
   g.B = a->w_e; g.b_rs = a->R; g.b_cs = 1;
-  g.C = a->du; g.c_rs = a->R; g.alpha = 1.f; g.epi = 5;
-  e = cudaMemsetAsync(a->du, 0, (size_t)a->N * a->R * sizeof(float), st);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc memset: %s", cudaGetErrorString(e));
-  if ((e = se_gemm(g, st, se_ksplit(g.M, g.N, g.K))) != cudaSuccess)
-    return set_error(YAMB_ECUDA, "se_fc bwd (du): %s", cudaGetErrorString(e));
-  {
-    dim3 fg((a->R + 255) / 256, (a->N + 31) / 32);
-    se_finish_kernel<<<fg, 256, 0, st>>>(a->N, a->R, a->du, nullptr, nullptr, a->u, a->g_br, a->act, 1);
+  g.alpha = 1.f;
+  float* part;
+  int nslab;
+  nrow = (a->N + 7) / 8;
+  if ((rc = det_alloc((size_t)nrow * a->R * sizeof(float), st, &colpart))) return rc;
+  if ((rc = se_split_product(g, a->du, st, &part, &nslab, "bwd (du)"))) {
+    det_free(colpart, st);
+    return rc;
   }
+  {
+    dim3 fg((a->R + 31) / 32, nrow);
+    se_finish_kernel<<<fg, dim3(32, 8), 0, st>>>(a->N, a->R, part, nslab, a->du, nullptr, nullptr,
+                                                 a->u, colpart, a->act, 1);
+    if ((rc = se_finish_done(part, a->du, st, "bwd (du finish)"))) {
+      det_free(colpart, st);
+      return rc;
+    }
+  }
+  if ((rc = det_reduce_launch(colpart, nrow, a->R, a->g_br, st))) return rc;
   // dpool[N][C] = inv_hw * du[N][R] * W_r[R][C]
   memset(&g, 0, sizeof(g));
   g.M = a->N; g.N = a->C; g.K = a->R;
@@ -257,14 +312,14 @@ int se_fc_bwd_launch(const yamb_se_fc_grad* a, cudaStream_t st) {
   g.M = a->C; g.N = a->R; g.K = a->N;
   g.A = a->dt; g.a_rs = 1; g.a_cs = a->C;
   g.B = a->v; g.b_rs = a->R; g.b_cs = 1;
-  g.C = a->g_we; g.c_rs = a->R; g.alpha = 1.f; g.epi = 4;
+  g.C = a->g_we; g.c_rs = a->R; g.alpha = 1.f; g.epi = 2;
   if ((e = se_gemm(g, st)) != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc bwd (dW_e): %s", cudaGetErrorString(e));
   // dW_r[R][C] += du^T[R][N] * s[N][C]
   memset(&g, 0, sizeof(g));
   g.M = a->R; g.N = a->C; g.K = a->N;
   g.A = a->du; g.a_rs = 1; g.a_cs = a->R;
   g.B = a->pooled; g.b_rs = a->C; g.b_cs = 1;
-  g.C = a->g_wr; g.c_rs = a->C; g.alpha = 1.f; g.epi = 4;
+  g.C = a->g_wr; g.c_rs = a->C; g.alpha = 1.f; g.epi = 2;
   if ((e = se_gemm(g, st)) != cudaSuccess) return set_error(YAMB_ECUDA, "se_fc bwd (dW_r): %s", cudaGetErrorString(e));
   return 0;
 }

@@ -214,15 +214,14 @@ class _NlTail:
     """Non-local block (reference models/mobilenet_base.py:158-173) behind a BatchNorm output l,
     for one shape: y = norm(dw3x3(f)) + l (+ x), f = (W/H) theta (phi^T g).  Owns l, f, h (bf16
     [N*H*W, C]) and F (fp32 [N][c][C]); `forward` is the four launches of the training plan and of
-    the eval path alike.  `deterministic`: the gram adds its per-CTA partial sums in a fixed order
-    (eval: the same logits on every run) instead of with fp32 atomics (training).
+    the eval path alike.
 
     The norm (`bn4`) runs in one of three modes, chosen per forward: BatchNorm with batch
     statistics (the depthwise kernel takes them, yamb_bn_apply_fwd applies them), InstanceNorm with
     per-sample statistics (yamb_instance_norm_fwd takes and applies them), or either norm folded
     from its running statistics (yamb_bn_apply_fwd)."""
 
-    def __init__(self, nl, bn4, N, H, W, C, dev, deterministic=False):
+    def __init__(self, nl, bn4, N, H, W, C, dev):
         self.nl, self.bn4 = nl, bn4
         self.instance = isinstance(nl.bn, torch.nn.InstanceNorm2d)
         self.used_instance_stats = False      # mode of the last forward (its backward follows it)
@@ -234,7 +233,6 @@ class _NlTail:
             raise nat.NativeError("non-local block: int(nl_c * C) must be a positive even "
                                   "number (got %d)" % self.cr)
         self.scale = float(W) / float(H)       # sic `f / H * W` (:171)
-        self.deterministic = 1 if deterministic else 0
         bf = torch.bfloat16
         self.l = torch.empty(self.M, C, device=dev, dtype=bf)
         self.f = torch.empty(self.M, C, device=dev, dtype=bf)
@@ -248,7 +246,6 @@ class _NlTail:
         g.X, g.ldx, g.I = X.data_ptr(), self.C, I
         g.Y, g.ldy, g.J = Y.data_ptr(), self.C, self.C
         g.alpha, g.G = alpha, G.data_ptr()
-        g.deterministic = self.deterministic
         self.keep.append(g)
         launch(lib_fn("yamb_nl_gram_fwd"), g, tag, 4 * self.M * self.C // (sub * sub))
 
@@ -1659,7 +1656,7 @@ def fused_class_eval_forward(block, x):
         bn4 = st.get(("bn4", dev.index))
         if bn4 is None:
             bn4 = st[("bn4", dev.index)] = _Bn([nl.bn], dev)
-        tail = _NlTail(nl, bn4, N, Ho, Wo, Cout, dev, deterministic=True)
+        tail = _NlTail(nl, bn4, N, Ho, Wo, Cout, dev)
     out = y if tail is None else tail.l
     a = _block_eval_args(block, x, out, w1, w3, conv_d, (bn1, bn2, bn3), residual)
     if se is not None:
@@ -1677,7 +1674,6 @@ def fused_class_eval_forward(block, x):
         f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
         f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
         f.u, f.v, f.gate = uv[0].data_ptr(), uv[1].data_ptr(), gate.data_ptr()
-        f.deterministic = 1
         launch(lib_fn("yamb_se_fc_fwd"), f, "se_fc", 4 * N * Chid * 2, 4 * N * Chid * R)
         a.pooled = None
         a.gate = gate.data_ptr()

@@ -190,7 +190,6 @@ class SeFc(C.Structure):
         ("pooled", C.c_void_p),
         ("w_r", C.c_void_p), ("b_r", C.c_void_p), ("w_e", C.c_void_p), ("b_e", C.c_void_p),
         ("u", C.c_void_p), ("v", C.c_void_p), ("gate", C.c_void_p),
-        ("deterministic", C.c_int32),
     ]
 
 
@@ -262,7 +261,6 @@ class NlGram(C.Structure):
         ("Y", C.c_void_p), ("ldy", C.c_int64), ("J", C.c_int32),
         ("alpha", C.c_float),
         ("G", C.c_void_p),
-        ("deterministic", C.c_int32),
     ]
 
 
