@@ -91,7 +91,9 @@ def main():
                        "shape": "%dx%dx%d -> %d (hidden %d, k %s, stride %d)" % (
                            inp.shape[1], inp.shape[2], inp.shape[3], m.output_dim,
                            sum(m.channels), list(m.kernel_sizes), m.stride),
-                       "one_launch": bool(engine.fused_eval_supported(m, inp))}
+                       # InvertedResidualChannelsFused: tests/gpu_eval_bench_fused_class.py
+                       "one_launch": bool(engine.eval_supported(m, inp) and
+                                          not engine.block_parts(m).fused)}
                 M_in = inp.shape[0] * inp.shape[2] * inp.shape[3]
                 ho = (inp.shape[2] - 1) // m.stride + 1
                 M_out = inp.shape[0] * ho * ho

@@ -1,6 +1,6 @@
 """Eval-mode (inference) timing of the InvertedResidualChannelsFused blocks (AutoNL, AtomNAS) on
 one H100: the one-launch block kernel with the Squeeze-and-Excitation gate and the non-local tail
-(engine.fused_class_eval_forward) against this repo's four-launch sequence.  Driver script (not a
+(engine.eval_forward) against this repo's four-launch sequence.  Driver script (not a
 pytest test):
 
     python tests/gpu_eval_bench_fused_class.py [--config autonl_l] [--batch 256] [--iters 20]
@@ -72,10 +72,10 @@ def main():
         for i, m in enumerate(feats):
             if hasattr(m, "expand_conv"):
                 inp = h
-                covered = with_rule(False, lambda: engine.fused_class_eval_supported(m, inp))
+                covered = with_rule(False, lambda: engine.eval_supported(m, inp))
                 if covered:
-                    se = hasattr(m.se_op, "se_reduce")
-                    nl = type(m.nl_op).__name__ != "Identity"
+                    parts = engine.block_parts(m)
+                    se, nl = parts.se is not None, parts.nl is not None
                     want = 1 + (2 if se else 0) + (4 if nl else 0)
                     rec = {"block": sum(hasattr(q, "use_res_connect") for q in feats[:i + 1]),
                            "shape": "%dx%dx%d -> %d (hidden %d, k %s, stride %d%s%s)" % (
@@ -83,7 +83,7 @@ def main():
                                sum(m.channels), list(m.kernel_sizes), m.stride,
                                ", SE" if se else "", ", non-local" if nl else ""),
                            "shape_rule_keeps_four_launches":
-                               not engine.fused_class_eval_supported(m, inp)}
+                               not engine.eval_supported(m, inp)}
                     t1, n1 = with_rule(False, lambda: kernel_time(lambda: m(inp), args.iters, flush))
                     assert n1 == want, (n1, want)
                     engine.EVAL_FUSED = False

@@ -234,8 +234,8 @@ def test_kernel_scratch_does_not_travel_with_a_deepcopy():
 
 
 def test_one_launch_eval_dispatch_rules():
-    """engine.fused_eval_supported decides from module structure only (no GPU needed): eval +
-    no_grad + unfused single-branch k in {3,5,7}; everything else keeps the four-launch path."""
+    """engine.eval_supported decides from module structure only (no GPU needed): eval + no_grad +
+    single-branch k in {3,5,7}; everything else keeps the four-launch path."""
     from yet_another_mobilenet_series_b200 import engine
     bn = {"momentum": 0.01, "eps": 1e-3}
     relu, swish = mb.get_active_fn("nn.ReLU6"), mb.get_active_fn("nn.Swish")
@@ -245,29 +245,72 @@ def test_one_launch_eval_dispatch_rules():
         return mb.InvertedResidualChannels(*a, **k).eval()
 
     plain = blk(32, 32, 1, [192], [3], True, active_fn=relu, batch_norm_kwargs=bn)
-    assert not engine.fused_eval_supported(plain, x)              # gradient mode is on
+    assert not engine.eval_supported(plain, x)              # gradient mode is on
     with torch.no_grad():
-        assert engine.fused_eval_supported(plain, x)
-        assert engine.fused_eval_supported(blk(32, 64, 2, [192], [7], True, active_fn=relu,
-                                               batch_norm_kwargs=bn), x)
-        assert engine.fused_eval_supported(blk(32, 16, 1, [32], [3], False, active_fn=relu,
-                                               batch_norm_kwargs=bn), x)
-        assert engine.fused_eval_supported(blk(32, 32, 1, [96], [3], True, active_fn=swish,
-                                               batch_norm_kwargs=bn), x)
-        # not covered: Swish with k = 5, several branches, odd widths, the fused class, train mode
-        assert not engine.fused_eval_supported(blk(32, 32, 1, [96], [5], True, active_fn=swish,
-                                                   batch_norm_kwargs=bn), x)
-        assert not engine.fused_eval_supported(blk(32, 32, 1, [48, 48], [3, 5], True, active_fn=relu,
-                                                   batch_norm_kwargs=bn), x)
-        assert not engine.fused_eval_supported(blk(32, 32, 1, [90], [3], True, active_fn=relu,
-                                                   batch_norm_kwargs=bn), x)
+        assert engine.eval_supported(plain, x)
+        assert engine.eval_supported(blk(32, 64, 2, [192], [7], True, active_fn=relu,
+                                         batch_norm_kwargs=bn), x)
+        assert engine.eval_supported(blk(32, 16, 1, [32], [3], False, active_fn=relu,
+                                         batch_norm_kwargs=bn), x)
+        assert engine.eval_supported(blk(32, 32, 1, [96], [3], True, active_fn=swish,
+                                         batch_norm_kwargs=bn), x)
+        # not covered: Swish with k = 5, several branches, odd widths, train mode
+        assert not engine.eval_supported(blk(32, 32, 1, [96], [5], True, active_fn=swish,
+                                             batch_norm_kwargs=bn), x)
+        assert not engine.eval_supported(blk(32, 32, 1, [48, 48], [3, 5], True, active_fn=relu,
+                                             batch_norm_kwargs=bn), x)
+        assert not engine.eval_supported(blk(32, 32, 1, [90], [3], True, active_fn=relu,
+                                             batch_norm_kwargs=bn), x)
         fused = mb.InvertedResidualChannelsFused(32, 32, 1, [96], [3], True, active_fn=relu,
                                                  batch_norm_kwargs=bn).eval()
-        assert not engine.fused_eval_supported(fused, x)
-        assert not engine.fused_eval_supported(plain.train(), x)
+        assert engine.eval_supported(fused, x)              # the fused class's rule
+        assert not engine.eval_supported(plain.train(), x)
         plain.eval()
         prev, engine.EVAL_FUSED = engine.EVAL_FUSED, False
         try:
-            assert not engine.fused_eval_supported(plain, x)      # YAMB_EVAL_FUSED=0
+            assert not engine.eval_supported(plain, x)      # YAMB_EVAL_FUSED=0
         finally:
             engine.EVAL_FUSED = prev
+
+
+@pytest.mark.parametrize("make,paths", [
+    (lambda: _unfused(True),
+     (["ops.0.0.0", "ops.1.0.0"], ["ops.0.0.1", "ops.1.0.1"],
+      [("ops.0.1.0", "ops.0.1.1"), ("ops.1.1.0", "ops.1.1.1")], ["ops.0.2", "ops.1.2"], "pw_bn",
+      None, None)),
+    (lambda: _unfused(False),
+     ([], [], [("ops.0.0.0", "ops.0.0.1")], ["ops.0.1"], "pw_bn", None, None)),
+    (lambda: mb.InvertedResidualChannelsFused(16, 16, 1, [48, 32], [3, 5], True,
+                                              mb.get_active_fn("nn.Swish"), BN, se_ratio=0.5,
+                                              nl_c=0.25, nl_s=1),
+     (["expand_conv.0"], ["expand_conv.1"],
+      [("depth_ops.0.1.0", "depth_ops.0.1.1"), ("depth_ops.1.1.0", "depth_ops.1.1.1")],
+      ["project_conv.0"], "project_conv.1", "se_op", "nl_op")),
+    (lambda: mb.InvertedResidualChannelsFused(16, 24, 1, [16], [3], False,
+                                              mb.get_active_fn("nn.ReLU"), BN, nl_c=0.25, nl_s=1),
+     ([], [], [("depth_ops.0.0.0", "depth_ops.0.0.1")], ["project_conv.0"], "project_conv.1",
+      None, "nl_op")),
+], ids=["unfused_expand_2branch", "unfused_no_expand", "fused_expand_2branch_se_nl",
+        "fused_no_expand_nl"])
+def test_block_parts_follow_the_reference_module_tree(make, paths):
+    """engine.block_parts returns, for either block class, the modules at the reference's
+    state_dict paths."""
+    from yet_another_mobilenet_series_b200 import engine
+    blk = make()
+    keys = set(blk.state_dict())
+    exp, bn1, dws, proj, bn3, se, nl = paths
+
+    def at(path):
+        assert any(k.startswith(path + ".") for k in keys), path
+        return blk.get_submodule(path)
+
+    p = engine.block_parts(blk)
+    assert p.fused == isinstance(blk, mb.InvertedResidualChannelsFused)
+    assert [id(m) for m in p.expand_convs] == [id(at(q)) for q in exp]
+    assert [id(m) for m in p.bn1s] == [id(at(q)) for q in bn1]
+    assert [(id(c), id(b)) for c, b in p.dws] == [(id(at(c)), id(at(b))) for c, b in dws]
+    assert [id(m) for m in p.project_convs] == [id(at(q)) for q in proj]
+    assert p.bn3 is at(bn3)
+    assert p.se is (None if se is None else at(se))
+    assert p.nl is (None if nl is None else at(nl))
+    assert isinstance(p.bn3, nn.BatchNorm2d) and all(isinstance(b, nn.BatchNorm2d) for b in p.bn1s)

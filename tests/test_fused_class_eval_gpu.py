@@ -1,4 +1,4 @@
-"""GPU parity of the eval path of InvertedResidualChannelsFused (engine.fused_class_eval_forward):
+"""GPU parity of the eval path of InvertedResidualChannelsFused (engine.eval_forward):
 the one-launch block kernel with the Squeeze-and-Excitation gate (pool pass -> SE FCs -> block
 kernel with the gate) and the non-local tail behind it (reference models/mobilenet_base.py:330-342
 in model.eval() under torch.no_grad()).  Shapes from AutoNL-L and AtomNAS-C+ block 1.

@@ -82,17 +82,17 @@ def test_fused_class_eval_dispatch():
     x = torch.zeros(2, 24, 14, 14)
     blk = _in_block(False)
     with torch.no_grad():
-        assert engine.fused_class_eval_supported(blk, x)
-    assert not engine.fused_class_eval_supported(blk, x)      # a gradient is wanted
+        assert engine.eval_supported(blk, x)
+    assert not engine.eval_supported(blk, x)      # a gradient is wanted
     with torch.no_grad():
-        assert not engine.fused_class_eval_supported(_in_block(True), x)
+        assert not engine.eval_supported(_in_block(True), x)
         blk.nl_op.bn.train()                                  # InstanceNorm alone in train mode
-        assert not engine.fused_class_eval_supported(blk, x)
+        assert not engine.eval_supported(blk, x)
         blk.nl_op.bn.eval()
         blk.nl_op.bn = torch.nn.GroupNorm(4, 24).eval()
-        assert not engine.fused_class_eval_supported(blk, x)
+        assert not engine.eval_supported(blk, x)
         blk.nl_op.bn = torch.nn.InstanceNorm2d(24, affine=True).eval()     # untracked
-        assert not engine.fused_class_eval_supported(blk, x)
+        assert not engine.eval_supported(blk, x)
 
 
 def test_unsupported_norms_raise():

@@ -14,6 +14,7 @@ Reference semantics: models/mobilenet_base.py:446-451 (unfused), :330-342 (fused
 torch.autograd backward.  No tensor between the 1x1 convs is ever normalised in HBM: BatchNorm +
 activation are applied by the consumer on load.
 """
+import collections
 import ctypes as C
 import os
 
@@ -200,6 +201,34 @@ class _Bn:
         torch.addcmul(b.detach(), rm, self.scale, value=-1.0, out=self.shift)
 
 
+BlockParts = collections.namedtuple(
+    "BlockParts", "fused expand_convs bn1s dws project_convs bn3 se nl")
+
+
+def _present(op):
+    """The SE / non-local child, or None where the reference placed its Identity placeholder."""
+    return None if type(op).__name__ == "Identity" else op
+
+
+def block_parts(block):
+    """The child modules of either block class (reference models/mobilenet_base.py:206-458):
+    expand convs and BN1s (one per branch for InvertedResidualChannels, one for
+    InvertedResidualChannelsFused, none without the expansion), (conv, BN2) of every branch's
+    depthwise stage, the project convs, BN3, the Squeeze-and-Excitation and non-local modules (None
+    when absent; always None for the unfused class)."""
+    if hasattr(block, "expand_conv"):
+        dws = [list(op.children())[-1] for op in block.depth_ops]
+        exp = [block.expand_conv] if block.expand else []
+        return BlockParts(True, [e[0] for e in exp], [e[1] for e in exp],
+                          [(d[0], d[1]) for d in dws], [block.project_conv[0]],
+                          block.project_conv[1], _present(block.se_op), _present(block.nl_op))
+    exp = [op[0] for op in block.ops] if block.expand else []
+    first = 1 if block.expand else 0       # ops[i] = [ConvBNReLU expand], ConvBNReLU dw, Conv2d
+    return BlockParts(False, [e[0] for e in exp], [e[1] for e in exp],
+                      [(op[first][0], op[first][1]) for op in block.ops],
+                      [op[first + 1] for op in block.ops], block.pw_bn, None, None)
+
+
 def _nl_norm_supported(norm):
     """The non-local block's norms the sm_90a path runs (reference get_nl_norm_fn,
     models/mobilenet_base.py:472-481): BatchNorm2d (`nl_norm: nn.BatchNorm`, the default) and the
@@ -214,7 +243,8 @@ class _NlTail:
     """Non-local block (reference models/mobilenet_base.py:158-173) behind a BatchNorm output l,
     for one shape: y = norm(dw3x3(f)) + l (+ x), f = (W/H) theta (phi^T g).  Owns l, f, h (bf16
     [N*H*W, C]) and F (fp32 [N][c][C]); `forward` is the four launches of the training plan and of
-    the eval path alike.
+    the eval path alike, `backward` the training plan's way back to dl (its buffers are made on
+    the first backward: the eval path never needs them).
 
     The norm (`bn4`) runs in one of three modes, chosen per forward: BatchNorm with batch
     statistics (the depthwise kernel takes them, yamb_bn_apply_fwd applies them), InstanceNorm with
@@ -238,6 +268,8 @@ class _NlTail:
         self.f = torch.empty(self.M, C, device=dev, dtype=bf)
         self.h = torch.empty(self.M, C, device=dev, dtype=bf)
         self.F = _f32(N * self.cr * C, dev)
+        self.df = self.dl = self.dF = None
+        self.in_dh = None
         self.keep = []
 
     def gram(self, X, I, Y, sub, alpha, G, tag):
@@ -348,12 +380,57 @@ class _NlTail:
         self.keep.append(s)
         launch(nat.lib().yamb_instance_norm_bwd, s, "nl_in_bwd", 2 * self.M * Cc * 5)
 
+    def backward(self, dym, grads, bn_bwd_struct):
+        """dy -> dl (gradient of the BN3 output): norm backward, depthwise 3x3 backward, the two
+        products' backward, plus the `+ l` pass-through.  grads: the plan's accumulation targets
+        ('bn4', 'nl_dw'); bn_bwd_struct(bn, count, grads): the yamb_bn_bwd of BN4 (batch or
+        running statistics; unused after an InstanceNorm forward with per-sample statistics)."""
+        lib = nat.lib()
+        Cc, c, bf, dev = self.C, self.cr, torch.bfloat16, self.l.device
+        if self.df is None:
+            self.df = torch.empty(self.M, Cc, device=dev, dtype=bf)
+            self.dl = torch.empty(self.M, Cc, device=dev, dtype=bf)
+            self.dF = _f32(self.N * c * Cc, dev)
+        d = nat.DwBwd()
+        d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.H, self.W, Cc, Cc, 3, 1
+        d.h = self.h.data_ptr()
+        if self.used_instance_stats:
+            # InstanceNorm with per-sample statistics: its backward writes dh (bf16), which the
+            # depthwise backward takes with the identity coefficients ca = 1, cb = cc = 0
+            if self.in_dh is None:
+                self.in_dh = torch.empty(self.M, Cc, device=dev, dtype=bf)
+                self.ones = torch.ones(Cc, device=dev, dtype=torch.float32)
+                self.zeros = _f32(Cc, dev)
+            self.instance_backward(dym, self.in_dh, grads["bn4"])
+            d.dz = self.in_dh.data_ptr()
+            d.ca, d.cb, d.cc = self.ones.data_ptr(), self.zeros.data_ptr(), self.zeros.data_ptr()
+        else:
+            r = nat.BnReduce()
+            r.M, r.C, r.lddy, r.ldh = self.M, Cc, Cc, Cc
+            r.dy, r.h = dym.data_ptr(), self.h.data_ptr()
+            r.bn = C.pointer(bn_bwd_struct(self.bn4, self.M, grads["bn4"]))
+            launch(lib.yamb_bn_reduce_bwd, r, "nl_bn_reduce", 4 * self.M * Cc)
+            d.dz = dym.data_ptr()
+            d.ca, d.cb, d.cc = self.bn4.ca.data_ptr(), self.bn4.cb.data_ptr(), \
+                self.bn4.cc.data_ptr()
+        d.w = self.nl.depthwise_conv.weight.data_ptr()
+        d.dw = grads["nl_dw"].data_ptr()
+        d.x = self.f.data_ptr()
+        d.dx = self.df.data_ptr()
+        self.keep.append(d)
+        launch(lib.yamb_depthwise_bwd, d, "nl_dw_bwd", 8 * Cc * self.M, 4 * self.M * Cc * 9)
+        # dF = (W/H) theta^T df (all pixels);  dl = dy + [dtheta | 0];  sub-sampled rows += dphi, dg
+        self.gram(self.l, c, self.df, 1, self.scale, self.dF, "nl_gram_bwd")
+        self.rowmat(self.df, Cc, self.F, 1, Cc, c, 1, self.scale, self.dl, "nl_dtheta", base=dym)
+        self.rowmat(self.l, Cc, self.dF, 1, Cc, c, self.sub, 1.0, self.dl, "nl_dphi", accumulate=1)
+        self.rowmat(self.l, c, self.dF, Cc, 1, Cc, self.sub, 1.0, self.dl, "nl_dg", accumulate=1)
+        return self.dl
+
 
 class BlockPlan:
     def __init__(self, block, x):
         dev = x.device
         self.dev = dev
-        self.ws = Workspace.get(dev)
         self.lib = nat.lib()
         N, Cin, H, W = x.shape
         self.N, self.H, self.W, self.Cin = N, H, W, Cin
@@ -367,7 +444,8 @@ class BlockPlan:
         self.expand = bool(block.expand)
         self.residual = bool(block.use_res_connect)
         self.act = act_code_of(block.active_fn)
-        self.fused = hasattr(block, "expand_conv")
+        parts = block_parts(block)
+        self.fused = parts.fused
         self.Chid = sum(self.channels)
         if self.Cin % 8 or self.Cout % 8 or any(c % 8 for c in self.channels):
             raise nat.NativeError(
@@ -386,28 +464,8 @@ class BlockPlan:
         self.dz2 = None
         self.dz1 = None
         # ---- modules ----
-        if self.fused:
-            self.conv_exp = [block.expand_conv[0]] if self.expand else []
-            bn1 = [block.expand_conv[1]] if self.expand else []
-            dws = [list(op.children())[-1] for op in block.depth_ops]
-            self.conv_proj = [block.project_conv[0]]
-            bn3 = block.project_conv[1]
-            self.se = block.se_op if type(block.se_op).__name__ != "Identity" else None
-            self.nl = block.nl_op if type(block.nl_op).__name__ != "Identity" else None
-        else:
-            if self.expand:
-                self.conv_exp = [op[0][0] for op in block.ops]
-                bn1 = [op[0][1] for op in block.ops]
-                dws = [op[1] for op in block.ops]
-                self.conv_proj = [op[2] for op in block.ops]
-            else:
-                self.conv_exp, bn1 = [], []
-                dws = [op[0] for op in block.ops]
-                self.conv_proj = [op[1] for op in block.ops]
-            bn3 = block.pw_bn
-        if not self.fused:
-            self.se = None
-            self.nl = None
+        self.conv_exp, self.conv_proj = parts.expand_convs, parts.project_convs
+        self.se, self.nl = parts.se, parts.nl
         if self.nl is not None:
             # non-local block (reference models/mobilenet_base.py:131-178) between BN3 and the skip
             nl = self.nl
@@ -416,14 +474,8 @@ class BlockPlan:
                     "non-local block: the sm_90a path runs nn.BatchNorm2d and "
                     "nn.InstanceNorm2d(affine=True, track_running_stats=True) as nl_norm (got %r)"
                     % nl.bn)
-            self.nl_tail = tail = _NlTail(nl, _Bn([nl.bn], dev), N, self.Ho, self.Wo, Cout, dev)
-            self.nl_cr, self.nl_sub, self.nl_scale = tail.cr, tail.sub, tail.scale
-            self.nl_l, self.nl_f, self.nl_h, self.nl_F = tail.l, tail.f, tail.h, tail.F
-            self.nl_dF = None
-            self.nl_df = None
-            self.nl_dl = None
-            self.nl_in_dh = None
-            self.bn4 = tail.bn4
+            self.nl_tail = _NlTail(nl, _Bn([nl.bn], dev), N, self.Ho, self.Wo, Cout, dev)
+            self.bn4 = self.nl_tail.bn4
             self.g_nl = torch.zeros_like(nl.depthwise_conv.weight, dtype=torch.float32)
         if self.se is not None:
             self.se_act = act_code_of(self.se.active_fn)
@@ -439,10 +491,10 @@ class BlockPlan:
             self.gate = _f32(N * Chid, dev).view(N, Chid)
             self.dgate = _f32(N * Chid, dev).view(N, Chid)
             self.dpool = _f32(N * Chid, dev).view(N, Chid)
-        self.conv_dw = [d[0] for d in dws]
-        self.bn1 = _Bn(bn1, dev) if self.expand else None
-        self.bn2 = _Bn([d[1] for d in dws], dev)
-        self.bn3 = _Bn([bn3], dev)
+        self.conv_dw = [conv for conv, _ in parts.dws]
+        self.bn1 = _Bn(parts.bn1s, dev) if self.expand else None
+        self.bn2 = _Bn([bn for _, bn in parts.dws], dev)
+        self.bn3 = _Bn([parts.bn3], dev)
         # ---- bf16 tensor-core operands + fp32 gradient accumulators ----
         self.w_exp_bf = torch.empty(Chid, Cin, device=dev, dtype=bf) if self.expand else None
         self.w_proj_bf = torch.empty(Cout, Chid, device=dev, dtype=bf)
@@ -541,9 +593,6 @@ class BlockPlan:
             else:
                 self.w_proj_bf.copy_(torch.cat([c.weight.flatten(1) for c in self.conv_proj], 1))
 
-    def _call(self, fn, st, tag="", nbytes=0, flops=0):
-        launch(fn, st, tag, nbytes, flops)
-
     def _fork_event(self):
         if not SIDE_WGRAD or PROFILE is not None:
             return None
@@ -583,18 +632,18 @@ class BlockPlan:
             if self.bn1.batch_stats:
                 if self.bn1.single:
                     g.bn_fwd = C.pointer(self._bn_fwd_struct(self.bn1, self.M_in))
-                    self._call(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
-                               2 * self.M_in * (self.Cin + self.Chid),
-                               2 * self.M_in * self.Cin * self.Chid)
+                    launch(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
+                           2 * self.M_in * (self.Cin + self.Chid),
+                           2 * self.M_in * self.Cin * self.Chid)
                 else:
                     # per-branch BN modules: one finalize per branch slice is done by the GEMM only
                     # for a single module; otherwise run the statistics per slice via N-slices
                     self._gemm_sliced_stats(g, self.bn1, self.M_in)
             else:
                 self.bn1.eval_coeffs()
-                self._call(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
-                           2 * self.M_in * (self.Cin + self.Chid),
-                           2 * self.M_in * self.Cin * self.Chid)
+                launch(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
+                       2 * self.M_in * (self.Cin + self.Chid),
+                       2 * self.M_in * self.Cin * self.Chid)
         # 2. depthwise per branch (BN1+act applied on load) + BN2 statistics
         if not self.bn2.batch_stats:
             self.bn2.eval_coeffs()
@@ -615,8 +664,8 @@ class BlockPlan:
             d.y = self.h2.data_ptr() + c0 * 2
             if self.bn2.batch_stats:
                 d.bn = C.pointer(self._bn_fwd_struct(self.bn2, self.M_out, c0, cb))
-            self._call(lib.yamb_depthwise_fwd, d, "dw_fwd", 2 * cb * (self.M_in + self.M_out),
-                       2 * self.M_out * cb * k * k)
+            launch(lib.yamb_depthwise_fwd, d, "dw_fwd", 2 * cb * (self.M_in + self.M_out),
+                   2 * self.M_out * cb * k * k)
             c0 += cb
         # 2b. Squeeze-and-Excitation gate (reference mobilenet_base.py:110-113): spatial mean of
         #     a2 = act(bn2(h2)) by a kernel, the two fully connected layers + sigmoid by another,
@@ -627,7 +676,7 @@ class BlockPlan:
             sp.h, sp.scale, sp.shift, sp.act = self.h2.data_ptr(), self.bn2.scale.data_ptr(), \
                 self.bn2.shift.data_ptr(), self.act
             sp.pooled = self.pooled.data_ptr()
-            self._call(lib.yamb_se_pool_fwd, sp, "se_pool", 2 * self.M_out * self.Chid)
+            launch(lib.yamb_se_pool_fwd, sp, "se_pool", 2 * self.M_out * self.Chid)
             se = self.se
             # the two fully connected layers on the pooled [N, C] vectors (fp32, like the reference
             # keeps them) + sigmoid: one launch (csrc/se_fc.cu)
@@ -638,8 +687,8 @@ class BlockPlan:
             f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
             f.u, f.v, f.gate = self.se_u.data_ptr(), self.se_v.data_ptr(), self.gate.data_ptr()
             self._keep.append(f)
-            self._call(lib.yamb_se_fc_fwd, f, "se_fc", 4 * self.N * self.Chid * 2,
-                       4 * self.N * self.Chid * self.se_r)
+            launch(lib.yamb_se_fc_fwd, f, "se_fc", 4 * self.N * self.Chid * 2,
+                   4 * self.N * self.Chid * self.se_r)
         # 3. project 1x1 (BN2+act as operand transform) + BN3 statistics
         g = nat.Gemm()
         g.M, g.N, g.K = self.M_out, self.Cout, self.Chid
@@ -654,9 +703,9 @@ class BlockPlan:
             g.bn_fwd = C.pointer(self._bn_fwd_struct(self.bn3, self.M_out))
         else:
             self.bn3.eval_coeffs()
-        self._call(lib.yamb_pointwise_gemm, g, "pw_project_fwd",
-                   2 * self.M_out * (self.Chid + self.Cout),
-                   2 * self.M_out * self.Chid * self.Cout)
+        launch(lib.yamb_pointwise_gemm, g, "pw_project_fwd",
+               2 * self.M_out * (self.Chid + self.Cout),
+               2 * self.M_out * self.Chid * self.Cout)
         # 4. BN3 apply (+ skip connection)
         a = nat.BnApply()
         a.M, a.C = self.M_out, self.Cout
@@ -667,69 +716,13 @@ class BlockPlan:
         if self.nl is None:
             a.residual = xm.data_ptr() if self.residual else None
             a.y = y.data_ptr()
-            self._call(lib.yamb_bn_apply_fwd, a, "bn_apply",
-                       2 * self.M_out * self.Cout * (3 if self.residual else 2))
+            launch(lib.yamb_bn_apply_fwd, a, "bn_apply",
+                   2 * self.M_out * self.Cout * (3 if self.residual else 2))
             return y
-        a.y = self.nl_l.data_ptr()              # l = BN3(h3): the non-local block's input
-        self._call(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * self.M_out * self.Cout)
+        a.y = self.nl_tail.l.data_ptr()         # l = BN3(h3): the non-local block's input
+        launch(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * self.M_out * self.Cout)
         self.nl_tail.forward(xm, y, self.residual, self._bn_fwd_struct)
         return y
-
-    # -- non-local block (reference models/mobilenet_base.py:158-173) ------------------------------
-    def _nl_gram(self, X, I, Y, sub, alpha, G, tag):
-        self.nl_tail.gram(X, I, Y, sub, alpha, G, tag)
-
-    def _nl_rowmat(self, X, K, Mat, sk, so, O, sub, alpha, out, tag, base=None, accumulate=0):
-        self.nl_tail.rowmat(X, K, Mat, sk, so, O, sub, alpha, out, tag, base, accumulate)
-
-    def _nl_backward(self, dym, grads):
-        """dy -> dl (gradient of the BN3 output): BN4 backward, depthwise 3x3 backward, the two
-        products' backward, plus the `+ l` pass-through."""
-        lib = self.lib
-        Cc, c, bf = self.Cout, self.nl_cr, torch.bfloat16
-        if self.nl_df is None:
-            self.nl_df = torch.empty(self.M_out, Cc, device=self.dev, dtype=bf)
-            self.nl_dl = torch.empty(self.M_out, Cc, device=self.dev, dtype=bf)
-            self.nl_dF = _f32(self.N * c * Cc, self.dev)
-        tail = self.nl_tail
-        d = nat.DwBwd()
-        d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.Ho, self.Wo, Cc, Cc, 3, 1
-        if tail.used_instance_stats:
-            # InstanceNorm with per-sample statistics: its backward writes dh (bf16), which the
-            # depthwise backward takes with the identity coefficients ca = 1, cb = cc = 0
-            if self.nl_in_dh is None:
-                self.nl_in_dh = torch.empty(self.M_out, Cc, device=self.dev, dtype=bf)
-                self.nl_ones = torch.ones(Cc, device=self.dev, dtype=torch.float32)
-                self.nl_zeros = _f32(Cc, self.dev)
-            tail.instance_backward(dym, self.nl_in_dh, grads["bn4"])
-            d.dz, d.h = self.nl_in_dh.data_ptr(), self.nl_h.data_ptr()
-            d.ca, d.cb, d.cc = self.nl_ones.data_ptr(), self.nl_zeros.data_ptr(), \
-                self.nl_zeros.data_ptr()
-        else:
-            r = nat.BnReduce()
-            r.M, r.C, r.lddy, r.ldh = self.M_out, Cc, Cc, Cc
-            r.dy, r.h = dym.data_ptr(), self.nl_h.data_ptr()
-            r.bn = C.pointer(self._bn_bwd_struct(self.bn4, self.M_out, grads["bn4"]))
-            self._call(lib.yamb_bn_reduce_bwd, r, "nl_bn_reduce", 4 * self.M_out * Cc)
-            d.dz, d.h = dym.data_ptr(), self.nl_h.data_ptr()
-            d.ca, d.cb, d.cc = self.bn4.ca.data_ptr(), self.bn4.cb.data_ptr(), \
-                self.bn4.cc.data_ptr()
-        d.w = self.nl.depthwise_conv.weight.data_ptr()
-        d.dw = grads["nl_dw"].data_ptr()
-        d.x = self.nl_f.data_ptr()
-        d.dx = self.nl_df.data_ptr()
-        self._keep.append(d)
-        self._call(lib.yamb_depthwise_bwd, d, "nl_dw_bwd", 8 * Cc * self.M_out,
-                   4 * self.M_out * Cc * 9)
-        # dF = (W/H) theta^T df (all pixels);  dl = dy + [dtheta | 0];  sub-sampled rows += dphi, dg
-        self._nl_gram(self.nl_l, c, self.nl_df, 1, self.nl_scale, self.nl_dF, "nl_gram_bwd")
-        self._nl_rowmat(self.nl_df, Cc, self.nl_F, 1, Cc, c, 1, self.nl_scale, self.nl_dl,
-                        "nl_dtheta", base=dym)
-        self._nl_rowmat(self.nl_l, Cc, self.nl_dF, 1, Cc, c, self.nl_sub, 1.0, self.nl_dl,
-                        "nl_dphi", accumulate=1)
-        self._nl_rowmat(self.nl_l, c, self.nl_dF, Cc, 1, Cc, self.nl_sub, 1.0, self.nl_dl,
-                        "nl_dg", accumulate=1)
-        return self.nl_dl
 
     def _gemm_sliced_stats(self, g, bn, count):
         """Expand GEMM whose output channels belong to several BN modules: one GEMM per module
@@ -742,8 +735,8 @@ class BlockPlan:
             gs.B = g.B + c0 * g.ldb * 2
             gs.D = g.D + c0 * 2
             gs.bn_fwd = C.pointer(self._bn_fwd_struct(bn, count, c0, cb))
-            self._call(lib.yamb_pointwise_gemm, gs, "pw_expand_fwd", 2 * gs.M * (gs.K + cb),
-                       2 * gs.M * gs.K * cb)
+            launch(lib.yamb_pointwise_gemm, gs, "pw_expand_fwd", 2 * gs.M * (gs.K + cb),
+                   2 * gs.M * gs.K * cb)
 
     def _se_backward(self, grads):
         """SE backward: dgate by a reduction kernel, the backward of the two fully connected layers
@@ -757,7 +750,7 @@ class BlockPlan:
         r.dy, r.h = self.dz2.data_ptr(), self.h2.data_ptr()
         r.scale, r.shift, r.act = self.bn2.scale.data_ptr(), self.bn2.shift.data_ptr(), self.act
         r.dgate = self.dgate.data_ptr()
-        self._call(lib.yamb_se_bwd_reduce_bwd, r, "se_bwd_reduce", 4 * self.M_out * self.Chid)
+        launch(lib.yamb_se_bwd_reduce_bwd, r, "se_bwd_reduce", 4 * self.M_out * self.Chid)
         b = nat.SeFcBwd()
         b.N, b.C, b.R, b.act, b.inv_hw = self.N, self.Chid, self.se_r, self.se_act, 1.0 / HW
         b.dgate, b.gate = self.dgate.data_ptr(), self.gate.data_ptr()
@@ -767,8 +760,8 @@ class BlockPlan:
         tg = grads["se"]
         b.g_wr, b.g_br, b.g_we, b.g_be = (tg[k].data_ptr() for k in ("wr", "br", "we", "be"))
         self._keep.append(b)
-        self._call(lib.yamb_se_fc_bwd, b, "se_fc_bwd", 4 * self.N * self.Chid * 4,
-                   8 * self.N * self.Chid * self.se_r)
+        launch(lib.yamb_se_fc_bwd, b, "se_fc_bwd", 4 * self.N * self.Chid * 4,
+               8 * self.N * self.Chid * self.se_r)
         for (c0, cb) in self.bn2.slices:
             a = nat.SeBwdApply()
             a.M, a.C, a.ldd, a.ldh, a.ldz = self.M_out, cb, self.Chid, self.Chid, self.Chid
@@ -783,7 +776,7 @@ class BlockPlan:
             a.ldg = self.Chid
             a.dz = self.dz2.data_ptr() + c0 * 2
             a.bn = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"], c0, cb))
-            self._call(lib.yamb_se_bwd_apply_bwd, a, "se_bwd_apply", 6 * self.M_out * cb)
+            launch(lib.yamb_se_bwd_apply_bwd, a, "se_bwd_apply", 6 * self.M_out * cb)
 
     # -- backward --------------------------------------------------------------------------------
     def backward(self, x, dy, grads):
@@ -803,13 +796,13 @@ class BlockPlan:
         dx = torch.empty((self.N, self.Cin, self.H, self.W), device=self.dev, dtype=bf,
                          memory_format=torch.channels_last)
         if self.nl is not None:
-            dym = self._nl_backward(dym, grads)
+            dym = self.nl_tail.backward(dym, grads, self._bn_bwd_struct)
         # 1. BN3 backward reduction -> ca3, cb3, cc3, dgamma3, dbeta3
         r = nat.BnReduce()
         r.M, r.C, r.lddy, r.ldh = self.M_out, self.Cout, self.Cout, self.Cout
         r.dy, r.h = dym.data_ptr(), self.h3.data_ptr()
         r.bn = C.pointer(self._bn_bwd_struct(self.bn3, self.M_out, grads["bn3"]))
-        self._call(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * self.M_out * self.Cout)
+        launch(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * self.M_out * self.Cout)
         fork_ev = self._fork_event()
         # 2. project dgrad: da2 = dh3 * W3, dz2 = da2 * act'(z2), BN2-backward statistics
         g = nat.Gemm()
@@ -824,9 +817,9 @@ class BlockPlan:
         if self.se is not None:
             # SE: the GEMM writes d(a2*gate); the gate / pooling gradients need a reduction over
             # HW first, so act'/BN2-backward happen in se_bwd_apply afterwards
-            self._call(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
-                       2 * self.M_out * (2 * self.Cout + self.Chid),
-                       2 * self.M_out * self.Chid * self.Cout)
+            launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
+                   2 * self.M_out * (2 * self.Cout + self.Chid),
+                   2 * self.M_out * self.Chid * self.Cout)
             self._se_backward(grads)
         else:
             g.epi = 1
@@ -835,9 +828,9 @@ class BlockPlan:
                 self.bn2.shift.data_ptr(), self.act
             if len(self.bn2.mods) == 1:
                 g.bn_bwd = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"]))
-                self._call(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
-                           4 * self.M_out * (self.Cout + self.Chid),
-                           2 * self.M_out * self.Chid * self.Cout)
+                launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
+                       4 * self.M_out * (self.Cout + self.Chid),
+                       2 * self.M_out * self.Chid * self.Cout)
             else:
                 for (c0, cb) in self.bn2.slices:
                     gs = nat.Gemm()
@@ -850,9 +843,9 @@ class BlockPlan:
                     gs.h_shift = g.h_shift + c0 * 4
                     gs.bn_bwd = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"],
                                                               c0, cb))
-                    self._call(lib.yamb_pointwise_gemm, gs, "pw_project_dgrad",
-                               4 * self.M_out * (self.Cout + cb),
-                               2 * self.M_out * cb * self.Cout)
+                    launch(lib.yamb_pointwise_gemm, gs, "pw_project_dgrad",
+                           4 * self.M_out * (self.Cout + cb),
+                           2 * self.M_out * cb * self.Cout)
         # 3. project wgrad: dW3[Cout,Chid] += dh3^T * a2
         g = nat.Gemm()
         g.M, g.N, g.K = self.Cout, self.Chid, self.M_out
@@ -897,8 +890,8 @@ class BlockPlan:
                 d.x = xm.data_ptr()
                 d.dx = dx.data_ptr()
                 d.residual = dym_skip.data_ptr() if self.residual else None
-            self._call(lib.yamb_depthwise_bwd, d, "dw_bwd", 4 * cb * (self.M_in + self.M_out),
-                       4 * self.M_out * cb * k * k)
+            launch(lib.yamb_depthwise_bwd, d, "dw_bwd", 4 * cb * (self.M_in + self.M_out),
+                   4 * self.M_out * cb * k * k)
             c0 += cb
         if not self.expand:
             return dx
@@ -915,9 +908,9 @@ class BlockPlan:
         g.D, g.ldd = dx.data_ptr(), self.Cin
         if self.residual:
             g.residual, g.ldr = dym_skip.data_ptr(), self.Cout
-        self._call(lib.yamb_pointwise_gemm, g, "pw_expand_dgrad",
-                   2 * self.M_in * (2 * self.Chid + self.Cin * (2 if self.residual else 1)),
-                   2 * self.M_in * self.Chid * self.Cin)
+        launch(lib.yamb_pointwise_gemm, g, "pw_expand_dgrad",
+               2 * self.M_in * (2 * self.Chid + self.Cin * (2 if self.residual else 1)),
+               2 * self.M_in * self.Chid * self.Cin)
         # 6. expand wgrad: dW1[Chid,Cin] += dh1^T * x
         g = nat.Gemm()
         g.M, g.N, g.K = self.Chid, self.Cin, self.M_in
@@ -975,11 +968,6 @@ def _plan_for(block, x):
     return p
 
 
-def block_params(block):
-    """Parameters of a block in the fixed order the autograd Function receives them."""
-    return [p for p in block.parameters()]
-
-
 class _BlockFn(torch.autograd.Function):
     """autograd boundary of the fused block: forward/backward run the sm_90a kernel sequences.
 
@@ -1018,106 +1006,105 @@ class _BlockFn(torch.autograd.Function):
 def run_backward(block, plan, x, dy):
     """Backward kernel sequence of one block; returns dx and {id(param): grad} for the parameters
     whose gradient was NOT accumulated straight into `.grad` (flat-arena direct mode)."""
-    if True:
-        dy = to_nhwc_bf16(dy)
-        params = list(block.parameters())
-        direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
+    dy = to_nhwc_bf16(dy)
+    params = list(block.parameters())
+    direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
 
-        def target(p, zero_buf):
-            if direct:
-                return p.grad
-            zero_buf.zero_()
-            return zero_buf
+    def target(p, zero_buf):
+        if direct:
+            return p.grad
+        zero_buf.zero_()
+        return zero_buf
 
-        def bn_targets(bn, key):
-            res = []
-            if bn is None:
-                return res
-            for i, m in enumerate(bn.mods):
-                if direct:
-                    res.append((m.weight.grad, m.bias.grad))
-                else:
-                    bufs = plan.__dict__.setdefault("_bn_gbuf", {})
-                    k2 = (key, i)
-                    if k2 not in bufs:
-                        bufs[k2] = (torch.zeros_like(m.weight), torch.zeros_like(m.bias))
-                    bufs[k2][0].zero_()
-                    bufs[k2][1].zero_()
-                    res.append(bufs[k2])
+    def bn_targets(bn, key):
+        res = []
+        if bn is None:
             return res
-
-        single_exp = plan.expand and len(plan.conv_exp) == 1
-        single_proj = len(plan.conv_proj) == 1
-        g = {}
-        if plan.expand:
-            if single_exp and direct:
-                g["exp"] = plan.conv_exp[0].weight.grad.view(plan.Chid, plan.Cin)
+        for i, m in enumerate(bn.mods):
+            if direct:
+                res.append((m.weight.grad, m.bias.grad))
             else:
-                plan.g_exp.zero_()
-                g["exp"] = plan.g_exp
-        if single_proj and direct:
-            g["proj"] = plan.conv_proj[0].weight.grad.view(plan.Cout, plan.Chid)
+                bufs = plan.__dict__.setdefault("_bn_gbuf", {})
+                k2 = (key, i)
+                if k2 not in bufs:
+                    bufs[k2] = (torch.zeros_like(m.weight), torch.zeros_like(m.bias))
+                bufs[k2][0].zero_()
+                bufs[k2][1].zero_()
+                res.append(bufs[k2])
+        return res
+
+    single_exp = plan.expand and len(plan.conv_exp) == 1
+    single_proj = len(plan.conv_proj) == 1
+    g = {}
+    if plan.expand:
+        if single_exp and direct:
+            g["exp"] = plan.conv_exp[0].weight.grad.view(plan.Chid, plan.Cin)
         else:
-            plan.g_proj.zero_()
-            g["proj"] = plan.g_proj
-        g["dw"] = [target(c.weight, plan.g_dw[i]) for i, c in enumerate(plan.conv_dw)]
-        g["bn1"] = bn_targets(plan.bn1, "bn1")
-        g["bn2"] = bn_targets(plan.bn2, "bn2")
-        g["bn3"] = bn_targets(plan.bn3, "bn3")
-        if plan.se is not None:
-            se = plan.se
-            g["se"] = {"wr": target(se.se_reduce.weight, plan.g_se["wr"]),
-                       "br": target(se.se_reduce.bias, plan.g_se["br"]),
-                       "we": target(se.se_expand.weight, plan.g_se["we"]),
-                       "be": target(se.se_expand.bias, plan.g_se["be"])}
-        if plan.nl is not None:
-            g["bn4"] = bn_targets(plan.bn4, "bn4")
-            g["nl_dw"] = target(plan.nl.depthwise_conv.weight, plan.g_nl)
-        dx = plan.backward(x, dy, g)
-        if not (DEFER_JOIN and direct and single_proj and (single_exp or not plan.expand)):
-            join_side(plan.dev)   # the gradient hand-over below reads what the wgrads wrote
-        # ---- hand gradients to autograd ----
-        gmap = {}
-        if plan.expand:
-            if not (single_exp and direct):
-                c0 = 0
-                for conv in plan.conv_exp:
-                    n = conv.weight.shape[0]
-                    piece = plan.g_exp[c0:c0 + n].reshape(conv.weight.shape)
-                    if direct:
-                        conv.weight.grad.add_(piece)
-                    else:
-                        gmap[id(conv.weight)] = piece
-                    c0 += n
-        if not (single_proj and direct):
+            plan.g_exp.zero_()
+            g["exp"] = plan.g_exp
+    if single_proj and direct:
+        g["proj"] = plan.conv_proj[0].weight.grad.view(plan.Cout, plan.Chid)
+    else:
+        plan.g_proj.zero_()
+        g["proj"] = plan.g_proj
+    g["dw"] = [target(c.weight, plan.g_dw[i]) for i, c in enumerate(plan.conv_dw)]
+    g["bn1"] = bn_targets(plan.bn1, "bn1")
+    g["bn2"] = bn_targets(plan.bn2, "bn2")
+    g["bn3"] = bn_targets(plan.bn3, "bn3")
+    if plan.se is not None:
+        se = plan.se
+        g["se"] = {"wr": target(se.se_reduce.weight, plan.g_se["wr"]),
+                   "br": target(se.se_reduce.bias, plan.g_se["br"]),
+                   "we": target(se.se_expand.weight, plan.g_se["we"]),
+                   "be": target(se.se_expand.bias, plan.g_se["be"])}
+    if plan.nl is not None:
+        g["bn4"] = bn_targets(plan.bn4, "bn4")
+        g["nl_dw"] = target(plan.nl.depthwise_conv.weight, plan.g_nl)
+    dx = plan.backward(x, dy, g)
+    if not (DEFER_JOIN and direct and single_proj and (single_exp or not plan.expand)):
+        join_side(plan.dev)   # the gradient hand-over below reads what the wgrads wrote
+    # ---- hand gradients to autograd ----
+    gmap = {}
+    if plan.expand:
+        if not (single_exp and direct):
             c0 = 0
-            for conv in plan.conv_proj:
-                n = conv.weight.shape[1]
-                piece = plan.g_proj[:, c0:c0 + n].reshape(conv.weight.shape)
+            for conv in plan.conv_exp:
+                n = conv.weight.shape[0]
+                piece = plan.g_exp[c0:c0 + n].reshape(conv.weight.shape)
                 if direct:
                     conv.weight.grad.add_(piece)
                 else:
                     gmap[id(conv.weight)] = piece
                 c0 += n
-        if not direct:
-            for i, c in enumerate(plan.conv_dw):
-                gmap[id(c.weight)] = plan.g_dw[i]
-            if plan.nl is not None:
-                gmap[id(plan.nl.depthwise_conv.weight)] = plan.g_nl
-            for key, bn in (("bn1", plan.bn1), ("bn2", plan.bn2), ("bn3", plan.bn3),
-                            ("bn4", getattr(plan, "bn4", None))):
-                if bn is None:
-                    continue
-                for i, m in enumerate(bn.mods):
-                    dg, db = g[key][i]
-                    gmap[id(m.weight)] = dg
-                    gmap[id(m.bias)] = db
-        if plan.se is not None and not direct:
-            se = plan.se
-            for k, prm in (("wr", se.se_reduce.weight), ("br", se.se_reduce.bias),
-                           ("we", se.se_expand.weight), ("be", se.se_expand.bias)):
-                gmap[id(prm)] = plan.g_se[k]
-        return dx, gmap
+    if not (single_proj and direct):
+        c0 = 0
+        for conv in plan.conv_proj:
+            n = conv.weight.shape[1]
+            piece = plan.g_proj[:, c0:c0 + n].reshape(conv.weight.shape)
+            if direct:
+                conv.weight.grad.add_(piece)
+            else:
+                gmap[id(conv.weight)] = piece
+            c0 += n
+    if not direct:
+        for i, c in enumerate(plan.conv_dw):
+            gmap[id(c.weight)] = plan.g_dw[i]
+        if plan.nl is not None:
+            gmap[id(plan.nl.depthwise_conv.weight)] = plan.g_nl
+        for key, bn in (("bn1", plan.bn1), ("bn2", plan.bn2), ("bn3", plan.bn3),
+                        ("bn4", getattr(plan, "bn4", None))):
+            if bn is None:
+                continue
+            for i, m in enumerate(bn.mods):
+                dg, db = g[key][i]
+                gmap[id(m.weight)] = dg
+                gmap[id(m.bias)] = db
+    if plan.se is not None and not direct:
+        se = plan.se
+        for k, prm in (("wr", se.se_reduce.weight), ("br", se.se_reduce.bias),
+                       ("we", se.se_expand.weight), ("be", se.se_expand.bias)):
+            gmap[id(prm)] = plan.g_se[k]
+    return dx, gmap
 
 
 # ---- channel padding ---------------------------------------------------------------------------
@@ -1138,7 +1125,8 @@ def needs_padding(block):
 class _PadShadow(Scratch):
     def __init__(self, block, device):
         from . import mobilenet_base as mb
-        fused = hasattr(block, "expand_conv")
+        parts = block_parts(block)
+        fused = parts.fused
         base = mb.InvertedResidualChannelsFused if fused else mb.InvertedResidualChannels
         self.real_ch = list(block.channels)
         self.pad_ch = [_ceil8(c) for c in self.real_ch]
@@ -1155,11 +1143,11 @@ class _PadShadow(Scratch):
         self.shadow = base(block.input_dim, block.output_dim, block.stride, self.pad_ch,
                            list(block.kernel_sizes), block.expand, **kw).to(device)
         logging.root.setLevel(lvl)
-        if fused and hasattr(block.nl_op, "bn"):
+        if parts.nl is not None:
             # the non-local norm (output width: never padded) is of the real block's class, which
             # the reference picks from FLAGS.nl_norm at construction time
             import copy
-            self.shadow.nl_op.bn = copy.deepcopy(block.nl_op.bn).to(device)
+            self.shadow.nl_op.bn = copy.deepcopy(parts.nl.bn).to(device)
         for p in self.shadow.parameters():
             p.requires_grad_(False)
         real = dict(block.named_parameters())
@@ -1327,7 +1315,6 @@ class _PadFn(torch.autograd.Function):
 class _BnActState(Scratch):
     def __init__(self, bn, dev):
         self.bn = _Bn([bn], dev)
-        self.ws = Workspace.get(dev)
         self.keep = []
         self.gbuf = None
 
@@ -1447,42 +1434,6 @@ def bn_act_apply(bn, active_fn, h):
 # YAMB_EVAL_FUSED=0 keeps the four-launch sequence (folded coefficients) for every block.
 EVAL_FUSED = os.environ.get("YAMB_EVAL_FUSED", "1") != "0"
 EVAL_FUSED_CALLS = 0     # blocks that went through yamb_block_eval_fwd (tests / bench)
-# (both eval paths: fused_eval_forward for the unfused class, fused_class_eval_forward for
-# InvertedResidualChannelsFused)
-
-
-def fused_eval_supported(block, x):
-    """True when yamb_block_eval_fwd covers this block for this call: no gradient wanted, every
-    BatchNorm normalising with running statistics, unfused single-branch block with a 3x3 / 5x5 /
-    7x7 depthwise, stride 1 or 2, with or without expansion (reference
-    models/mobilenet_base.py:380-421; every block of MobileNetV2-1.0 and of Proxyless-mobile),
-    channel counts the kernel's tiles hold."""
-    if not EVAL_FUSED or torch.is_grad_enabled() or hasattr(block, "expand_conv"):
-        return False
-    if block.stride not in (1, 2) or not hasattr(block, "ops"):
-        return False
-    if len(block.channels) != 1 or list(block.kernel_sizes)[0] not in (3, 5, 7):
-        return False
-    cin, chid, cout = block.input_dim, block.channels[0], block.output_dim
-    if cin % 8 or chid % 8 or cout % 8 or cin > 256 or cout > 320:
-        return False
-    if not block.expand and chid != cin:
-        return False
-    if x.dim() != 4 or x.shape[0] * x.shape[2] * x.shape[3] >= 2 ** 30:
-        return False
-    op = block.ops[0]
-    bns = (op[0][1], op[1][1], block.pw_bn) if block.expand else (op[0][1], block.pw_bn)
-    for bn in bns:
-        if not isinstance(bn, torch.nn.BatchNorm2d) or bn.training or \
-                not bn.track_running_stats or bn.running_mean is None:
-            return False
-    try:
-        act = act_code_of(block.active_fn)
-    except ValueError:
-        return False
-    if block.kernel_sizes[0] != 3 and (not block.expand or act not in (0, 1, 2)):
-        return False        # k = 5 / 7: built with expansion and relu / relu6 only
-    return True
 
 
 def _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p):
@@ -1537,31 +1488,8 @@ def _block_eval_cost(block, x, Ho, Wo, residual, project=True):
     return nbytes, flops
 
 
-def fused_eval_forward(block, x):
-    """y = block(x) in eval mode through ONE kernel launch; x channels_last bf16 on CUDA."""
-    global EVAL_FUSED_CALLS
-    dev = x.device
-    N, Cin, H, W = x.shape
-    op = block.ops[0]
-    if block.expand:
-        conv_e, bn1, conv_d, bn2, conv_p = op[0][0], op[0][1], op[1][0], op[1][1], op[2]
-    else:
-        conv_e, bn1, conv_d, bn2, conv_p = None, None, op[0][0], op[0][1], op[1]
-    bn3 = block.pw_bn
-    Chid, Cout, stride = block.channels[0], block.output_dim, block.stride
-    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    w1, w3 = _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p)
-    y = torch.empty((N, Cout, Ho, Wo), device=dev, dtype=torch.bfloat16,
-                    memory_format=torch.channels_last)
-    a = _block_eval_args(block, x, y, w1, w3, conv_d, (bn1, bn2, bn3), block.use_res_connect)
-    launch(lib_fn("yamb_block_eval_fwd"), a, "block_eval",
-           *_block_eval_cost(block, x, Ho, Wo, block.use_res_connect))
-    EVAL_FUSED_CALLS += 1
-    return y
-
-
-# ---- eval mode of InvertedResidualChannelsFused (AutoNL, AtomNAS): the block kernel with the SE
-# gate and the non-local tail (reference models/mobilenet_base.py:330-342) ----------------------------
+# ---- one eval path for both block classes; InvertedResidualChannelsFused (AutoNL, AtomNAS) adds
+# the SE gate and the non-local tail (reference models/mobilenet_base.py:330-342) -----------------
 # Shape rule of the fused-class path, measured by tests/gpu_eval_bench_fused_class.py on one H100
 # 80GB HBM3 (400 W power limit), N = 256, kernel time per block, new path vs the four-launch
 # sequence.  5x5 blocks measured slower (AutoNL-L block 3, no SE: 1.08 vs 0.97 ms; block 14, SE:
@@ -1587,16 +1515,18 @@ def _nl_norm_eval_ready(norm):
     return _bn_eval_ready(norm)
 
 
-def fused_class_eval_supported(block, x):
-    """True when the eval path of InvertedResidualChannelsFused covers this block for this call: no
-    gradient wanted, every BatchNorm (the non-local block's included, or its tracked InstanceNorm)
-    normalising with running statistics, one branch with a 3x3 / 5x5 / 7x7 depthwise (no expansion: 3x3 only), stride 1 or
-    2, widths that are multiples of 8 with Cin <= 256 and Cout <= 320, any activation, with or
-    without Squeeze-and-Excitation and a non-local block (every block of AutoNL-L, block 1 of
-    AtomNAS-C+), minus the shapes FUSED_CLASS_SHAPE_RULE keeps on the four-launch sequence (8
-    AutoNL-L blocks take the path with it).  The unfused class has its own rule,
-    fused_eval_supported."""
-    if not EVAL_FUSED or torch.is_grad_enabled() or not hasattr(block, "expand_conv"):
+def eval_supported(block, x):
+    """True when the eval path covers this block for this call: no gradient wanted, every
+    BatchNorm (the non-local block's included, or its tracked InstanceNorm) normalising with
+    running statistics, one branch with a 3x3 / 5x5 / 7x7 depthwise (no expansion: 3x3 only),
+    stride 1 or 2, widths that are multiples of 8 with Cin <= 256 and Cout <= 320.  Per class:
+    InvertedResidualChannels (reference models/mobilenet_base.py:380-421) with k = 5 / 7 only for
+    relu / relu6 / no activation (every block of MobileNetV2-1.0 and of Proxyless-mobile);
+    InvertedResidualChannelsFused with any activation, with or without Squeeze-and-Excitation and
+    a non-local block (every block of AutoNL-L, block 1 of AtomNAS-C+), minus the shapes
+    FUSED_CLASS_SHAPE_RULE keeps on the four-launch sequence (8 AutoNL-L blocks take the path with
+    it)."""
+    if not EVAL_FUSED or torch.is_grad_enabled():
         return False
     if block.stride not in (1, 2) or len(block.channels) != 1:
         return False
@@ -1606,45 +1536,42 @@ def fused_class_eval_supported(block, x):
         return False
     if not block.expand and (k != 3 or chid != cin):
         return False
-    if FUSED_CLASS_SHAPE_RULE and (k != 3 or not block.expand):
-        return False        # measured slower than the four-launch sequence (see above)
     if x.dim() != 4 or x.shape[0] * x.shape[2] * x.shape[3] >= 2 ** 30:
         return False
-    stage = list(block.depth_ops[0].children())[-1]
-    bns = [stage[1], block.project_conv[1]] + ([block.expand_conv[1]] if block.expand else [])
-    nl = block.nl_op if type(block.nl_op).__name__ != "Identity" else None
-    if nl is not None:
-        if not _nl_norm_eval_ready(nl.bn):
-            return False
-        c = int(nl.nl_c * cout)
-        if c <= 0 or c % 2 or int(nl.nl_s) < 1:
-            return False
-    if not all(_bn_eval_ready(bn) for bn in bns):
+    parts = block_parts(block)
+    if not all(_bn_eval_ready(bn) for bn in parts.bn1s + [parts.dws[0][1], parts.bn3]):
         return False
     try:
-        act_code_of(block.active_fn)
-        if hasattr(block.se_op, "se_reduce"):
-            act_code_of(block.se_op.active_fn)
+        act = act_code_of(block.active_fn)
+        if parts.se is not None:
+            act_code_of(parts.se.active_fn)
     except ValueError:
         return False
+    if not parts.fused:
+        return k == 3 or act in (0, 1, 2)     # k = 5 / 7: built with relu / relu6 only
+    if FUSED_CLASS_SHAPE_RULE and (k != 3 or not block.expand):
+        return False        # measured slower than the four-launch sequence (see above)
+    nl = parts.nl
+    if nl is not None:
+        c = int(nl.nl_c * cout)
+        if not _nl_norm_eval_ready(nl.bn) or c <= 0 or c % 2 or int(nl.nl_s) < 1:
+            return False
     return True
 
 
-def fused_class_eval_forward(block, x):
-    """y = block(x) of an InvertedResidualChannelsFused in eval mode; x channels_last bf16 on CUDA.
-    C-ABI calls: the block kernel (1); with SE the pool pass and the gate FCs first (3); with a
-    non-local block the kernel writes l = BN3(h3) and the non-local tail follows (+4)."""
+def eval_forward(block, x):
+    """y = block(x) in eval mode; x channels_last bf16 on CUDA.  C-ABI calls: the block kernel
+    (1); with SE the pool pass and the gate FCs first (3); with a non-local block the kernel writes
+    l = BN3(h3) and the non-local tail follows (+4)."""
     global EVAL_FUSED_CALLS
     dev = x.device
     N, Cin, H, W = x.shape
-    conv_e, bn1 = (block.expand_conv[0], block.expand_conv[1]) if block.expand else (None, None)
-    stage = list(block.depth_ops[0].children())[-1]
-    conv_d, bn2 = stage[0], stage[1]
-    conv_p, bn3 = block.project_conv[0], block.project_conv[1]
+    parts = block_parts(block)
+    conv_e, bn1 = (parts.expand_convs[0], parts.bn1s[0]) if block.expand else (None, None)
+    (conv_d, bn2), conv_p, bn3 = parts.dws[0], parts.project_convs[0], parts.bn3
+    se, nl = parts.se, parts.nl
     Chid, Cout, stride = block.channels[0], block.output_dim, block.stride
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    se = block.se_op if hasattr(block.se_op, "se_reduce") else None
-    nl = block.nl_op if type(block.nl_op).__name__ != "Identity" else None
     w1, w3 = _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p)
     bf = torch.bfloat16
     y = torch.empty((N, Cout, Ho, Wo), device=dev, dtype=bf, memory_format=torch.channels_last)
@@ -1693,10 +1620,8 @@ def block_apply(block, x):
             "the inverted-residual block runs only on CUDA sm_90a (no CPU fallback); got a %s "
             "tensor" % x.device)
     x = to_nhwc_bf16(x)
-    if fused_eval_supported(block, x):
-        return fused_eval_forward(block, x)
-    if fused_class_eval_supported(block, x):
-        return fused_class_eval_forward(block, x)
+    if eval_supported(block, x):
+        return eval_forward(block, x)
     params = list(block.parameters())
     if needs_padding(block):
         return _PadFn.apply(x, block, *params)

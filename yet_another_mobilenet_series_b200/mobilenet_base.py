@@ -112,7 +112,7 @@ class ZeroInitBN(nn.BatchNorm2d):
 class Nonlocal(nn.Module):
     """Lightweight non-local block (reference :131-178): parameter holder with the reference's
     module tree (`depthwise_conv`, `bn`).  Inside a fused block on CUDA its arithmetic runs in the
-    block's kernel sequence (engine.BlockPlan._nl_forward / _nl_backward: yamb_nl_gram,
+    block's kernel sequence (engine._NlTail.forward / backward: yamb_nl_gram,
     yamb_nl_rowmat, the depthwise and BatchNorm kernels); this `forward` is the stand-alone
     stock-torch statement of the same function (CPU, oracle, `as_reference`).
 

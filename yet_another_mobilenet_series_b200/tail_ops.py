@@ -29,7 +29,6 @@ class _PwState(engine.Scratch):
 
     def __init__(self, conv, bn, dev):
         self.bn = engine._Bn([bn], dev)
-        self.ws = engine.Workspace.get(dev)
         self.w_own = torch.empty(conv.out_channels, conv.in_channels, device=dev,
                                  dtype=torch.bfloat16)
         self.g_own = None
