@@ -265,32 +265,60 @@ struct BnBwdApplyDev {
   const float *ca, *cb, *cc;
   __nv_bfloat16* dh;
 };
+// Thread layout of bn_reduce: a thread owns one 8-channel group (its coefficients stay in registers)
+// and walks pixel rows with 4 rows (8 independent 16-byte loads) in flight; one load pair per
+// iteration left the kernel latency-bound.  The arithmetic is that of the GEMM loaders' two-source
+// transform (gxform_panel<2>: fmaf(ca, dy, fmaf(cb, h, cc)), RN to bf16), so a GEMM that reads
+// this dh gets the operand bits the transform would have formed.
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __grid_constant__ BnBwdApplyDev p) {
   const int CG = p.C / 8;
-  const long long total = p.M * CG;
+  const int PX = 256 / CG > 0 ? 256 / CG : 1;
   const ActParam zap = make_act(p.z_scale ? p.z_act : ACT_NONE);
-  const long long stride = (long long)gridDim.x * blockDim.x;   // incremental (row, group), see bn_apply
-  const long long d_row = stride / CG;
-  const int d_cg = (int)(stride % CG);
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  long long row = i / CG;
-  int cgi = (int)(i % CG);
-  for (; i < total; i += stride, row += d_row, cgi += d_cg) {
-    if (cgi >= CG) { cgi -= CG; ++row; }
-    const int c0 = cgi * 8;
-    float d[8], hv[8];
-    unpack8(__ldg(reinterpret_cast<const uint4*>(p.dy + row * p.lddy + c0)), d);
-    unpack8(__ldg(reinterpret_cast<const uint4*>(p.h + row * p.ldh + c0)), hv);
-    if (p.z_scale) {
-      float z[8];
+  // channel groups beyond 256 are covered by looping cg
+  for (int cgb = 0; cgb < CG; cgb += 256) {
+    const int cg = cgb + (CG >= 256 ? threadIdx.x : threadIdx.x % CG);
+    const int px = CG >= 256 ? 0 : threadIdx.x / CG;
+    if (cg >= CG || px >= PX) continue;
+    const int c0 = cg * 8;
+    float ca[8], cb[8], cc[8], zs[8], zt[8];
 #pragma unroll
-      for (int e = 0; e < 8; ++e) z[e] = fmaf(__ldg(p.z_scale + c0 + e), hv[e], __ldg(p.z_shift + c0 + e));
-      act_bwd_vec<8>(d, z, zap, p.z_act);
+    for (int e = 0; e < 8; ++e) {
+      ca[e] = __ldg(p.ca + c0 + e);
+      cb[e] = __ldg(p.cb + c0 + e);
+      cc[e] = __ldg(p.cc + c0 + e);
+      zs[e] = p.z_scale ? __ldg(p.z_scale + c0 + e) : 1.f;
+      zt[e] = p.z_scale ? __ldg(p.z_shift + c0 + e) : 0.f;
     }
+    const long long rstep = (long long)gridDim.x * PX;
+    for (long long row = (long long)blockIdx.x * PX + px; row < p.M; row += 4 * rstep) {
+      uint4 ud[4], uh[4];
 #pragma unroll
-    for (int e = 0; e < 8; ++e)
-      d[e] = fmaf(__ldg(p.ca + c0 + e), d[e], fmaf(__ldg(p.cb + c0 + e), hv[e], __ldg(p.cc + c0 + e)));
-    *reinterpret_cast<uint4*>(p.dh + row * p.lddh + c0) = pack8(d);
+      for (int j = 0; j < 4; ++j) {
+        const long long r2 = row + j * rstep;
+        ud[j] = make_uint4(0u, 0u, 0u, 0u);
+        uh[j] = make_uint4(0u, 0u, 0u, 0u);
+        if (r2 < p.M) {
+          ud[j] = __ldg(reinterpret_cast<const uint4*>(p.dy + r2 * p.lddy + c0));
+          uh[j] = __ldg(reinterpret_cast<const uint4*>(p.h + r2 * p.ldh + c0));
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const long long r2 = row + j * rstep;
+        float d[8], hv[8];
+        unpack8(ud[j], d);
+        unpack8(uh[j], hv);
+        if (p.z_scale) {
+          float z[8];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) z[e] = fmaf(zs[e], hv[e], zt[e]);
+          act_bwd_vec<8>(d, z, zap, p.z_act);
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) d[e] = fmaf(ca[e], d[e], fmaf(cb[e], hv[e], cc[e]));
+        if (r2 < p.M) *reinterpret_cast<uint4*>(p.dh + r2 * p.lddh + c0) = pack8(d);
+      }
+    }
   }
 }
 
@@ -540,9 +568,11 @@ int bn_bwd_apply_launch(const yamb_bn_bwd_apply* a, cudaStream_t st) {
   p.dy = (const __nv_bfloat16*)a->dy; p.h = (const __nv_bfloat16*)a->h;
   p.z_scale = a->z_scale; p.z_shift = a->z_shift; p.z_act = a->z_act;
   p.ca = a->ca; p.cb = a->cb; p.cc = a->cc; p.dh = (__nv_bfloat16*)a->dh;
-  const long long total = a->M * (a->C / 8);
-  long long want = (total + 255) / 256;
-  int grid = (int)(want < (long long)16 * max_ctas() ? want : 16 * max_ctas());
+  const int CG = a->C / 8;
+  const int PX = 256 / CG > 0 ? 256 / CG : 1;
+  // one 4-row batch per pixel lane and CTA at least; up to 8 CTAs per SM (the SM's thread limit)
+  long long want = (a->M + 4LL * PX - 1) / (4LL * PX);
+  int grid = (int)(want < (long long)8 * max_ctas() ? want : 8 * max_ctas());
   bn_bwd_apply_kernel<<<grid, 256, 0, st>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "bn_bwd_apply: %s", cudaGetErrorString(e));

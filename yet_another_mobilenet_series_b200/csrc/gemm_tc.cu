@@ -1204,8 +1204,8 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
                                                                       : pick_tc<0, 16, 0, 0>(xf);
   else if (a->epi == 0 && !p.a_mn)         // dgrad (+ residual)
     fn = pick_tc<0, 64, 0, 1>(xf);
-  else if (a->epi == 1 && !p.a_mn && p.b_mn)   // dgrad + dz: the layers always transform A, so one
-    fn = &launch_tc<true, 1, 64, 0, 1>;        // variant (it runs a plain A with the transform off)
+  else if (a->epi == 1 && !p.a_mn && p.b_mn)   // dgrad + dz: plain A (dh3) or two-source A, one
+    fn = &launch_tc<true, 1, 64, 0, 1>;        // variant (XF = false spills 68 B at 128 registers)
   else if (a->epi == 2 && p.a_mn && p.b_mn)    // wgrad
     fn = pick_tc<2, 64, 1, 1>(xf);
   if (!fn)

@@ -461,6 +461,7 @@ class BlockPlan:
         self.h1 = torch.empty(self.M_in, Chid, device=dev, dtype=bf) if self.expand else None
         self.h2 = torch.empty(self.M_out, Chid, device=dev, dtype=bf)
         self.h3 = torch.empty(self.M_out, Cout, device=dev, dtype=bf)
+        self.dh3 = None
         self.dz2 = None
         self.dz1 = None
         # ---- modules ----
@@ -787,6 +788,7 @@ class BlockPlan:
         self._keep = []
         bf = torch.bfloat16
         if self.dz2 is None:
+            self.dh3 = torch.empty(self.M_out, self.Cout, device=self.dev, dtype=bf)
             self.dz2 = torch.empty(self.M_out, self.Chid, device=self.dev, dtype=bf)
             if self.expand:
                 self.dz1 = torch.empty(self.M_in, self.Chid, device=self.dev, dtype=bf)
@@ -803,22 +805,26 @@ class BlockPlan:
         r.dy, r.h = dym.data_ptr(), self.h3.data_ptr()
         r.bn = C.pointer(self._bn_bwd_struct(self.bn3, self.M_out, grads["bn3"]))
         launch(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * self.M_out * self.Cout)
+        # 1b. dh3 = ca3*dy + cb3*h3 + cc3, formed once: both project GEMMs read it as a plain
+        #     operand (as a loader transform it was re-read and re-formed for every n-block)
+        a = nat.BnBwdApply()
+        a.M, a.C, a.lddy, a.ldh, a.lddh = self.M_out, self.Cout, self.Cout, self.Cout, self.Cout
+        a.dy, a.h = dym.data_ptr(), self.h3.data_ptr()
+        a.ca, a.cb, a.cc = self.bn3.ca.data_ptr(), self.bn3.cb.data_ptr(), self.bn3.cc.data_ptr()
+        a.dh = self.dh3.data_ptr()
+        launch(lib.yamb_bn_bwd_apply_bwd, a, "bn3_bwd_apply", 6 * self.M_out * self.Cout)
         fork_ev = self._fork_event()
         # 2. project dgrad: da2 = dh3 * W3, dz2 = da2 * act'(z2), BN2-backward statistics
         g = nat.Gemm()
         g.M, g.N, g.K = self.M_out, self.Chid, self.Cout
-        g.A, g.lda = dym.data_ptr(), self.Cout
-        g.a_xform = 2
-        g.a_scale, g.a_scale2, g.a_shift = self.bn3.ca.data_ptr(), self.bn3.cb.data_ptr(), \
-            self.bn3.cc.data_ptr()
-        g.A2, g.lda2 = self.h3.data_ptr(), self.Cout
+        g.A, g.lda = self.dh3.data_ptr(), self.Cout
         g.B, g.ldb, g.b_mn_major = self.w_proj_bf.data_ptr(), self.Chid, 1
         g.D, g.ldd = self.dz2.data_ptr(), self.Chid
         if self.se is not None:
             # SE: the GEMM writes d(a2*gate); the gate / pooling gradients need a reduction over
             # HW first, so act'/BN2-backward happen in se_bwd_apply afterwards
             launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
-                   2 * self.M_out * (2 * self.Cout + self.Chid),
+                   2 * self.M_out * (self.Cout + self.Chid),
                    2 * self.M_out * self.Chid * self.Cout)
             self._se_backward(grads)
         else:
@@ -829,7 +835,7 @@ class BlockPlan:
             if len(self.bn2.mods) == 1:
                 g.bn_bwd = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"]))
                 launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
-                       4 * self.M_out * (self.Cout + self.Chid),
+                       2 * self.M_out * (self.Cout + 2 * self.Chid),
                        2 * self.M_out * self.Chid * self.Cout)
             else:
                 for (c0, cb) in self.bn2.slices:
@@ -844,17 +850,13 @@ class BlockPlan:
                     gs.bn_bwd = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"],
                                                               c0, cb))
                     launch(lib.yamb_pointwise_gemm, gs, "pw_project_dgrad",
-                           4 * self.M_out * (self.Cout + cb),
+                           2 * self.M_out * (self.Cout + 2 * cb),
                            2 * self.M_out * cb * self.Cout)
         # 3. project wgrad: dW3[Cout,Chid] += dh3^T * a2
         g = nat.Gemm()
         g.M, g.N, g.K = self.Cout, self.Chid, self.M_out
         g.a_mn_major = g.b_mn_major = 1
-        g.A, g.lda = dym.data_ptr(), self.Cout
-        g.a_xform = 2
-        g.a_scale, g.a_scale2, g.a_shift = self.bn3.ca.data_ptr(), self.bn3.cb.data_ptr(), \
-            self.bn3.cc.data_ptr()
-        g.A2, g.lda2 = self.h3.data_ptr(), self.Cout
+        g.A, g.lda = self.dh3.data_ptr(), self.Cout
         g.B, g.ldb = self.h2.data_ptr(), self.Chid
         g.b_xform, g.b_act = 1, self.act
         g.b_scale, g.b_shift = self.bn2.scale.data_ptr(), self.bn2.shift.data_ptr()
@@ -862,10 +864,10 @@ class BlockPlan:
             g.b_gate, g.gate_rows_per_sample = self.gate.data_ptr(), self.Ho * self.Wo
         g.D, g.ldd = grads["proj"].data_ptr(), self.Chid
         g.epi = 2
-        # needs only the BN3-backward coefficients (step 1) -> off the critical chain
+        # needs only dh3 (step 1b) -> off the critical chain
         self._call_side(lib.yamb_pointwise_gemm, g, "pw_project_wgrad",
-                        2 * self.M_out * (2 * self.Cout + self.Chid),
-                        2 * self.M_out * self.Chid * self.Cout, fork_ev, (dy,))
+                        2 * self.M_out * (self.Cout + self.Chid),
+                        2 * self.M_out * self.Chid * self.Cout, fork_ev, (self.dh3,))
         # 4. depthwise backward per branch
         c0 = 0
         for b, (cb, k) in enumerate(zip(self.channels, self.ks)):
