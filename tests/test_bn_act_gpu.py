@@ -12,7 +12,8 @@ def _rel(a, b):
 
 
 @pytest.mark.parametrize("C,H,act,train", [(32, 24, "ReLU6", True), (1280, 3, "ReLU", True),
-                                           (64, 9, "Swish", True), (32, 16, "ReLU6", False)])
+                                           (64, 9, "Swish", True), (32, 16, "ReLU6", False),
+                                           (2048, 3, "ReLU", True)])
 def test_bn_act_matches_torch(built_lib, C, H, act, train):
     from yet_another_mobilenet_series_b200 import engine, mobilenet_base as mb
     torch.manual_seed(0)

@@ -24,7 +24,9 @@ def _bn_randomise(m, g):
             mod.bias.data.normal_(0, 0.3, generator=g)
 
 
-@pytest.mark.parametrize("cin,cout,hw,act", [(320, 1280, 7, "nn.ReLU"), (64, 136, 5, "nn.Swish")])
+# (640, 2560): the head of a width-2.0 network (last_channel = 1280 * width_mult)
+@pytest.mark.parametrize("cin,cout,hw,act", [(320, 1280, 7, "nn.ReLU"), (64, 136, 5, "nn.Swish"),
+                                             (640, 2560, 7, "nn.ReLU")])
 def test_head_pointwise_conv_bn_act(built_lib, cin, cout, hw, act):
     from yet_another_mobilenet_series_b200 import mobilenet_base as mb
     torch.backends.cudnn.allow_tf32 = False

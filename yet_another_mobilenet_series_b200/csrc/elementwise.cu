@@ -8,6 +8,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include <mutex>
+
 #include "bn_finalize.cuh"
 #include "host_util.h"
 #include "prims.cuh"
@@ -504,8 +506,67 @@ __global__ void __launch_bounds__(256) se_bwd_apply_kernel(const __grid_constant
   }
 }
 
+// ---- launchers -----------------------------------------------------------------------------------
+// A bf16 [rows][ld] operand that the kernels read or write 16 bytes (8 channels) at a time: present,
+// ld >= C, rows of whole 16-byte vectors and a 16-byte aligned base.
+static int check_bf16(const char* fn, const char* name, const void* p, int ld, int C) {
+  if (!p) return set_error(YAMB_EINVAL, "%s: %s is NULL", fn, name);
+  if (ld < C || ld % 8)
+    return set_error(YAMB_EINVAL, "%s: row pitch of %s is %d, needs >= C = %d and a multiple of 8", fn,
+                     name, ld, C);
+  if (reinterpret_cast<uintptr_t>(p) & 15)
+    return set_error(YAMB_EINVAL, "%s: %s must be 16-byte aligned", fn, name);
+  return 0;
+}
+
+// bn_stats, bn_reduce and se_bwd_apply take 2*C doubles of dynamic shared memory (the CTA's
+// statistics slots) on top of cta_stats_merge's static staging.  Past the 48 KiB default (C >= 1984)
+// the kernel has to opt in; the limit is per device, so it is raised (never lowered) per device.
+// A C whose total exceeds the device's opt-in maximum is refused.
+enum { kStatsKernels = 3, kStatsDevices = 64 };
+static int stats_smem(int which, const void* kern, const char* fn, int C, size_t* smem_out) {
+  struct Ent { size_t static_smem; int optin; size_t raised; bool init; };
+  static Ent cache[kStatsKernels][kStatsDevices];
+  static std::mutex mu;
+  const size_t smem = 2 * (size_t)C * sizeof(stat_t);
+  *smem_out = smem;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "%s: %s", fn, cudaGetErrorString(e));
+  std::lock_guard<std::mutex> lock(mu);
+  Ent spare = Ent{0, 0, 0, false};
+  Ent& c = dev < kStatsDevices ? cache[which][dev] : spare;
+  if (!c.init) {
+    cudaFuncAttributes fa;
+    e = cudaFuncGetAttributes(&fa, kern);
+    if (e == cudaSuccess)
+      e = cudaDeviceGetAttribute(&c.optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "%s: %s", fn, cudaGetErrorString(e));
+    c.static_smem = fa.sharedSizeBytes;
+    c.init = true;
+  }
+  if (c.static_smem + smem > (size_t)c.optin)
+    return set_error(YAMB_EINVAL, "%s: C = %d needs %zu B of shared memory, the device allows %d B",
+                     fn, C, c.static_smem + smem, c.optin);
+  if (smem > c.raised && c.static_smem + smem > 48 * 1024) {
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "%s attr: %s", fn, cudaGetErrorString(e));
+    c.raised = smem;
+  }
+  return 0;
+}
+
 int bn_apply_launch(const yamb_bn_apply* a, cudaStream_t st) {
   if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8)) return set_error(YAMB_EINVAL, "bn_apply shape");
+  int rc;
+  if ((rc = check_bf16("bn_apply", "h", a->h, a->ldh, a->C)) ||
+      (rc = check_bf16("bn_apply", "y", a->y, a->ldy, a->C)) ||
+      (a->residual && (rc = check_bf16("bn_apply", "residual", a->residual, a->ldr, a->C))) ||
+      (a->residual2 && (rc = check_bf16("bn_apply", "residual2", a->residual2, a->ldr2, a->C))))
+    return rc;
+  if (!a->scale || !a->shift ||
+      ((reinterpret_cast<uintptr_t>(a->scale) | reinterpret_cast<uintptr_t>(a->shift)) & 15))
+    return set_error(YAMB_EINVAL, "bn_apply: scale / shift must be 16-byte aligned");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   BnApplyDev p;
   p.M = a->M; p.C = a->C; p.ldh = a->ldh; p.ldr = a->ldr; p.ldy = a->ldy;
@@ -525,43 +586,59 @@ int bn_apply_launch(const yamb_bn_apply* a, cudaStream_t st) {
 int bn_reduce_launch(const yamb_bn_reduce* a, cudaStream_t st) {
   if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8) || !a->bn)
     return set_error(YAMB_EINVAL, "bn_reduce shape");
+  int rc;
+  if ((rc = check_bf16("bn_reduce", "dy", a->dy, a->lddy, a->C)) ||
+      (rc = check_bf16("bn_reduce", "h", a->h, a->ldh, a->C)))
+    return rc;
+  if (a->z_scale && !a->z_shift) return set_error(YAMB_EINVAL, "bn_reduce: z_scale without z_shift");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   BnReduceDev p;
   p.M = a->M; p.C = a->C; p.lddy = a->lddy; p.ldh = a->ldh;
   p.dy = (const __nv_bfloat16*)a->dy; p.h = (const __nv_bfloat16*)a->h; p.bn = *a->bn;
   p.z_scale = a->z_scale; p.z_shift = a->z_scale ? a->z_shift : nullptr; p.z_act = a->z_act;
-  if (a->z_scale && !a->z_shift) return set_error(YAMB_EINVAL, "bn_reduce: z_scale without z_shift");
+  size_t smem;
+  if ((rc = stats_smem(0, (const void*)bn_reduce_kernel, "bn_reduce", a->C, &smem))) return rc;
   const int CG = a->C / 8;
   const int PX = 256 / CG > 0 ? 256 / CG : 1;
   long long want = (a->M + PX - 1) / PX;
   int grid = (int)(want < (long long)2 * max_ctas() ? want : 2 * max_ctas());
-  bn_reduce_kernel<<<grid, 256, 2 * a->C * sizeof(stat_t), st>>>(p);
+  bn_reduce_kernel<<<grid, 256, smem, st>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "bn_reduce: %s", cudaGetErrorString(e));
   return 0;
 }
 
 int bn_stats_launch(const yamb_bn_stats* a, cudaStream_t st) {
-  if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8) || (a->ldh % 8) || !a->h || !a->bn)
+  if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8) || !a->bn)
     return set_error(YAMB_EINVAL, "bn_stats args");
+  int rc;
+  if ((rc = check_bf16("bn_stats", "h", a->h, a->ldh, a->C))) return rc;
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   BnStatsDev p;
   p.M = a->M; p.C = a->C; p.ldh = a->ldh;
   p.h = (const __nv_bfloat16*)a->h; p.bn = *a->bn;
+  size_t smem;
+  if ((rc = stats_smem(1, (const void*)bn_stats_kernel, "bn_stats", a->C, &smem))) return rc;
   const int CG = a->C / 8;
   const int PX = 256 / CG > 0 ? 256 / CG : 1;
   long long want = (a->M + PX - 1) / PX;
   int grid = (int)(want < (long long)4 * max_ctas() ? want : 4 * max_ctas());
-  bn_stats_kernel<<<grid, 256, 2 * a->C * sizeof(stat_t), st>>>(p);
+  bn_stats_kernel<<<grid, 256, smem, st>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "bn_stats: %s", cudaGetErrorString(e));
   return 0;
 }
 
 int bn_bwd_apply_launch(const yamb_bn_bwd_apply* a, cudaStream_t st) {
-  if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8) || (a->ldh % 8) || (a->lddy % 8) || (a->lddh % 8) ||
-      !a->dy || !a->h || !a->dh || !a->ca || !a->cb || !a->cc)
+  if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8) || !a->ca || !a->cb || !a->cc)
     return set_error(YAMB_EINVAL, "bn_bwd_apply args");
+  int rc;
+  if ((rc = check_bf16("bn_bwd_apply", "dy", a->dy, a->lddy, a->C)) ||
+      (rc = check_bf16("bn_bwd_apply", "h", a->h, a->ldh, a->C)) ||
+      (rc = check_bf16("bn_bwd_apply", "dh", a->dh, a->lddh, a->C)))
+    return rc;
+  if (a->z_scale && !a->z_shift)
+    return set_error(YAMB_EINVAL, "bn_bwd_apply: z_scale without z_shift");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   BnBwdApplyDev p;
   p.M = a->M; p.C = a->C; p.lddy = a->lddy; p.ldh = a->ldh; p.lddh = a->lddh;
@@ -613,13 +690,15 @@ static int se_slabs_done(float* part, int chunks, int N, int C, float* out, cuda
 int se_pool_launch(const yamb_se_pool* a, cudaStream_t st) {
   if (!a || a->N <= 0 || a->HW <= 0 || a->C <= 0 || (a->C % 8))
     return set_error(YAMB_EINVAL, "se_pool shape");
+  int rc;
+  if ((rc = check_bf16("se_pool", "h", a->h, a->ldh, a->C))) return rc;
+  if (a->N > 65535) return set_error(YAMB_EINVAL, "se_pool: N <= 65535");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   SePoolDev p;
   p.N = a->N; p.HW = a->HW; p.C = a->C; p.ldh = a->ldh;
   p.h = (const __nv_bfloat16*)a->h; p.scale = a->scale; p.shift = a->shift; p.act = a->act;
-  if (a->N > 65535) return set_error(YAMB_EINVAL, "se_pool: N <= 65535");
   int chunks;
-  int rc = se_slabs(a->N, a->HW, a->C, a->pooled, st, &chunks, &p.pooled);
+  rc = se_slabs(a->N, a->HW, a->C, a->pooled, st, &chunks, &p.pooled);
   if (rc) return rc;
   p.out_ld = a->C;
   p.slab = (long long)a->N * a->C;
@@ -636,14 +715,18 @@ int se_pool_launch(const yamb_se_pool* a, cudaStream_t st) {
 int se_bwd_reduce_launch(const yamb_se_bwd_reduce* a, cudaStream_t st) {
   if (!a || a->N <= 0 || a->HW <= 0 || a->C <= 0 || (a->C % 8))
     return set_error(YAMB_EINVAL, "se_bwd_reduce shape");
+  int rc;
+  if ((rc = check_bf16("se_bwd_reduce", "dy", a->dy, a->ldd, a->C)) ||
+      (rc = check_bf16("se_bwd_reduce", "h", a->h, a->ldh, a->C)))
+    return rc;
+  if (a->N > 65535) return set_error(YAMB_EINVAL, "se_bwd_reduce: N <= 65535");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   SeBwdReduceDev p;
   p.N = a->N; p.HW = a->HW; p.C = a->C; p.ldd = a->ldd; p.ldh = a->ldh;
   p.dy = (const __nv_bfloat16*)a->dy; p.h = (const __nv_bfloat16*)a->h;
   p.scale = a->scale; p.shift = a->shift; p.act = a->act;
-  if (a->N > 65535) return set_error(YAMB_EINVAL, "se_bwd_reduce: N <= 65535");
   int chunks;
-  int rc = se_slabs(a->N, a->HW, a->C, a->dgate, st, &chunks, &p.dgate);
+  rc = se_slabs(a->N, a->HW, a->C, a->dgate, st, &chunks, &p.dgate);
   if (rc) return rc;
   p.out_ld = a->C;
   p.slab = (long long)a->N * a->C;
@@ -661,21 +744,31 @@ int se_bwd_reduce_launch(const yamb_se_bwd_reduce* a, cudaStream_t st) {
 int se_bwd_apply_launch(const yamb_se_bwd_apply* a, cudaStream_t st) {
   if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8) || !a->bn || a->rows_per_sample <= 0)
     return set_error(YAMB_EINVAL, "se_bwd_apply shape");
+  int rc;
+  if ((rc = check_bf16("se_bwd_apply", "dy", a->dy, a->ldd, a->C)) ||
+      (rc = check_bf16("se_bwd_apply", "h", a->h, a->ldh, a->C)) ||
+      (rc = check_bf16("se_bwd_apply", "dz", a->dz, a->ldz, a->C)))
+    return rc;
+  const int ldg = a->ldg > 0 ? a->ldg : a->C;
+  if (!a->gate || !a->dpool ||
+      ((reinterpret_cast<uintptr_t>(a->gate) | reinterpret_cast<uintptr_t>(a->dpool)) & 15) ||
+      (ldg % 4))
+    return set_error(YAMB_EINVAL, "se_bwd_apply: gate / dpool must be 16-byte aligned, pitch % 4 == 0");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   SeBwdApplyDev p;
   p.M = a->M; p.C = a->C; p.ldd = a->ldd; p.ldh = a->ldh; p.ldz = a->ldz;
   p.rows_per_sample = a->rows_per_sample;
   p.dy = (const __nv_bfloat16*)a->dy; p.h = (const __nv_bfloat16*)a->h;
   p.scale = a->scale; p.shift = a->shift; p.act = a->act;
-  p.gate = a->gate; p.dpool = a->dpool; p.ldg = a->ldg > 0 ? a->ldg : a->C;
-  if (((reinterpret_cast<uintptr_t>(a->gate) | reinterpret_cast<uintptr_t>(a->dpool)) & 15) || (p.ldg % 4))
-    return set_error(YAMB_EINVAL, "se_bwd_apply: gate / dpool must be 16-byte aligned, pitch % 4 == 0");
+  p.gate = a->gate; p.dpool = a->dpool; p.ldg = ldg;
   p.dz = (__nv_bfloat16*)a->dz; p.bn = *a->bn;
+  size_t smem;
+  if ((rc = stats_smem(2, (const void*)se_bwd_apply_kernel, "se_bwd_apply", a->C, &smem))) return rc;
   const int CG = a->C / 8;
   const int PX = 256 / CG > 0 ? 256 / CG : 1;
   long long want = (a->M + PX - 1) / PX;
   int grid = (int)(want < (long long)2 * max_ctas() ? want : 2 * max_ctas());
-  se_bwd_apply_kernel<<<grid, 256, 2 * a->C * sizeof(stat_t), st>>>(p);
+  se_bwd_apply_kernel<<<grid, 256, smem, st>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_bwd_apply: %s", cudaGetErrorString(e));
   return 0;

@@ -94,10 +94,11 @@ def act_code_of(active_fn):
 
 
 class Workspace:
-    """Scratch of the statistics-producing kernels: the global fp32 accumulator of the per-channel
-    sums (2*C floats, zero between launches — the last CTA of every launch returns it to zero) and
-    the arrival counter.  The kernels of ONE stream serialise on it, so there is one per
-    (device, stream): blocks driven from two streams at the same time (VERDICT r1) do not share."""
+    """Scratch of the statistics-producing kernels: the global accumulator of the per-channel sums
+    (2*C doubles for a BatchNorm of C channels, room for C <= max_c; zero between launches — the
+    last CTA of every launch returns it to zero) and the arrival counter.  The kernels of ONE
+    stream serialise on it, so there is one per (device, stream): blocks driven from two streams at
+    the same time (VERDICT r1) do not share."""
     _per_stream = {}
 
     def __init__(self, device):
@@ -106,8 +107,16 @@ class Workspace:
         if self.max_ctas <= 0:
             raise nat.NativeError("no CUDA device visible to libyamb200 (there is no CPU path)")
         self.max_c = 4096
+        # 2 * max_c doubles, kept in a float32 tensor
         self.partials = torch.zeros(4 * self.max_c, device=device, dtype=torch.float32)
         self.counter = torch.zeros(4, device=device, dtype=torch.int32)
+
+    def stats(self, C):
+        """(partials, counter) device pointers for a statistics kernel over C channels."""
+        if C > self.max_c:
+            raise nat.NativeError("BatchNorm of %d channels: the statistics accumulator holds %d"
+                                  % (C, self.max_c))
+        return self.partials.data_ptr(), self.counter.data_ptr()
 
     @classmethod
     def get(cls, device):
@@ -513,8 +522,7 @@ class BlockPlan:
         C = bn.C if C is None else C
         s = nat.BnFwd()
         ws = Workspace.get(self.dev)     # of the stream this launch goes to
-        s.partials = ws.partials.data_ptr()
-        s.counter = ws.counter.data_ptr()
+        s.partials, s.counter = ws.stats(C)
         if bn.single:
             m = bn.mods[0]
             g, b = m.weight, m.bias
@@ -550,8 +558,7 @@ class BlockPlan:
         C = bn.C if C is None else C
         s = nat.BnBwd()
         ws = Workspace.get(self.dev)     # of the stream this launch goes to
-        s.partials = ws.partials.data_ptr()
-        s.counter = ws.counter.data_ptr()
+        s.partials, s.counter = ws.stats(C)
         f4 = 4
         if bn.single:
             mi, off = 0, c0
@@ -1342,7 +1349,7 @@ class _BnActFn(torch.autograd.Function):
         if b.batch_stats:
             f = nat.BnFwd()
             ws = Workspace.get(h.device)
-            f.partials, f.counter = ws.partials.data_ptr(), ws.counter.data_ptr()
+            f.partials, f.counter = ws.stats(Cc)
             f.gamma, f.beta = nat.ptr(bn.weight), nat.ptr(bn.bias)
             f.eps, f.momentum = b.eps, b.momentum_value()
             if bn.track_running_stats and bn.running_mean is not None:
@@ -1398,7 +1405,7 @@ class _BnActFn(torch.autograd.Function):
             dg, db = st.gbuf
         g = nat.BnBwd()
         ws = Workspace.get(h.device)
-        g.partials, g.counter = ws.partials.data_ptr(), ws.counter.data_ptr()
+        g.partials, g.counter = ws.stats(Cc)
         g.gamma = nat.ptr(bn.weight)
         g.mean, g.invstd = c_mean, c_invstd
         g.dgamma, g.dbeta = dg.data_ptr(), db.data_ptr()

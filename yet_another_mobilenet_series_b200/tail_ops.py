@@ -77,7 +77,7 @@ class _PwConvBnActFn(torch.autograd.Function):
         if b.batch_stats:
             f = nat.BnFwd()
             ws = engine.Workspace.get(x.device)
-            f.partials, f.counter = ws.partials.data_ptr(), ws.counter.data_ptr()
+            f.partials, f.counter = ws.stats(Cout)
             f.gamma, f.beta = nat.ptr(bn.weight), nat.ptr(bn.bias)
             f.eps, f.momentum = b.eps, b.momentum_value()
             if bn.track_running_stats and bn.running_mean is not None:
@@ -135,7 +135,7 @@ class _PwConvBnActFn(torch.autograd.Function):
         # BatchNorm-backward statistics of dz = dy * act'(z), then dh = ca*dz + cb*h + cc
         q = nat.BnBwd()
         ws = engine.Workspace.get(x.device)
-        q.partials, q.counter = ws.partials.data_ptr(), ws.counter.data_ptr()
+        q.partials, q.counter = ws.stats(Cout)
         q.gamma = nat.ptr(bn.weight)
         q.mean, q.invstd = c_mean, c_invstd
         q.dgamma, q.dbeta = dg.data_ptr(), db.data_ptr()
