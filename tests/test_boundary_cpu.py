@@ -214,23 +214,28 @@ def test_kernel_scratch_does_not_travel_with_a_deepcopy():
 
     blk = mb.InvertedResidualChannels(16, 16, 1, [32], [3], True, active_fn=mb.get_active_fn("nn.ReLU"),
                                       batch_norm_kwargs={"momentum": 0.01, "eps": 1e-3})
-    seq = nn.Sequential(blk, nn.Linear(4, 4))
+    head = mb.ConvBNReLU(16, 32, kernel_size=1, active_fn=mb.get_active_fn("nn.ReLU"))
+    seq = nn.Sequential(blk, nn.Linear(4, 4), head)
     plans = engine._ScratchDict()
     plans["k"] = Holder()
     blk.__dict__["_yamb_plans"] = plans
     blk.__dict__["_yamb_eval"] = engine._ScratchDict(a=torch.zeros(1))
     blk.pw_bn.__dict__["_yamb_bnact"] = Holder()
     seq[1].__dict__["_yamb_lin"] = Holder()
+    head[0].__dict__["_yamb_pw"] = Holder()
     assert issubclass(tail_ops._PwState, engine.Scratch)
     assert issubclass(tail_ops._LinearState, engine.Scratch)
     assert issubclass(engine._BnActState, engine.Scratch)
     c = copy.deepcopy(seq)
     assert "_yamb_plans" not in c[0].__dict__ and "_yamb_eval" not in c[0].__dict__
     assert c[0].pw_bn.__dict__["_yamb_bnact"] is None and c[1].__dict__["_yamb_lin"] is None
+    assert c[2][0].__dict__["_yamb_pw"] is None
     for (k, a), (_, b) in zip(seq.state_dict().items(), c.state_dict().items()):
         assert torch.equal(a, b), k
     r = pickle.loads(pickle.dumps(seq[1]))
     assert r.__dict__["_yamb_lin"] is None
+    r = pickle.loads(pickle.dumps(head))
+    assert r[0].__dict__["_yamb_pw"] is None
 
 
 def test_one_launch_eval_dispatch_rules():

@@ -76,6 +76,55 @@ def test_head_pointwise_conv_bn_act(built_lib, cin, cout, hw, act):
     assert int(mod[1].num_batches_tracked) == 1
 
 
+@pytest.mark.parametrize("layer", ["head", "stem"])
+def test_backward_reads_its_own_forward_statistics(built_lib, layer):
+    """Forward A, forward B on another batch, then A's backward: dx and the parameter gradients
+    equal, bit for bit, those of a copy that ran A's forward and backward alone (the BatchNorm
+    backward reads the statistics its own forward took, not those of the latest forward).  As in
+    training, the parameters live in the fused optimizer's flat arena: the head's bf16 weight
+    operand is the optimizer's mirror, which forward B leaves alone (forward B rewrites a
+    module-owned copy, and autograd then refuses A's backward)."""
+    from yet_another_mobilenet_series_b200 import mobilenet_base as mb
+    from yet_another_mobilenet_series_b200.fused_rmsprop import RMSprop
+    g = torch.Generator().manual_seed(6)
+    bnk = {"momentum": 0.01, "eps": 1e-3}
+    relu = mb.get_active_fn("nn.ReLU")
+    # module construction draws from the global generator: leave it as the later tests find it
+    with torch.random.fork_rng(devices=[]):
+        if layer == "head":
+            mod = mb.ConvBNReLU(320, 1280, kernel_size=1, batch_norm_kwargs=bnk, active_fn=relu)
+            shape = (16, 320, 7, 7)
+        else:
+            mod = mb.ConvBNReLU(3, 32, stride=2, batch_norm_kwargs=bnk, active_fn=relu)
+            shape = (4, 3, 64, 64)
+        mod.apply(mb.init_weights_mnas)
+    _bn_randomise(mod, g)
+    alone = copy.deepcopy(mod).cuda().train()
+    mod = mod.cuda().train()
+    opts = [RMSprop(m.parameters(), lr=0.016, alpha=0.9, momentum=0.9, eps=1e-3,
+                    eps_inside_sqrt=True) for m in (alone, mod)]
+    for o in opts:
+        o.arenas()
+    xa = torch.randn(shape, generator=g).cuda()
+    xb = (torch.randn(shape, generator=g) * 3 + 1).cuda()
+
+    def grads(m, others):
+        x = xa.clone().requires_grad_(layer == "head")     # the stem has no input gradient
+        y = m(x)
+        for o in others:
+            m(o)
+        y.backward(torch.randn(y.shape, generator=torch.Generator().manual_seed(7)).cuda()
+                   .to(y.dtype))
+        torch.cuda.synchronize()
+        return ([x.grad] if layer == "head" else []) + [p.grad for p in m.parameters()]
+
+    want = grads(alone, [])
+    got = grads(mod, [xb])
+    assert len(got) == len(want) == (4 if layer == "head" else 3)
+    for a, b in zip(got, want):
+        assert torch.equal(a, b)
+
+
 def test_classifier_linear(built_lib):
     from yet_another_mobilenet_series_b200 import tail_ops
     torch.backends.cuda.matmul.allow_tf32 = False

@@ -158,6 +158,17 @@ def _f32(n, dev):
     return torch.zeros(n, device=dev, dtype=torch.float32)
 
 
+def _at(t, c0):
+    """Device pointer of channel c0 of an fp32 per-channel tensor (None -> NULL)."""
+    return None if t is None else t.data_ptr() + 4 * c0
+
+
+def direct_grads(params):
+    """True when every parameter carries a pre-allocated `.grad` that the flat-arena optimizer marked
+    `_yamb_direct`: the kernels then accumulate into those gradients and autograd gets None."""
+    return all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
+
+
 class _Bn:
     """Device-side state of one BatchNorm stage (possibly several reference BN modules whose
     channels are concatenated: per-branch BNs of the unfused block)."""
@@ -208,6 +219,50 @@ class _Bn:
         torch.mul(g.detach(), self.invstd, out=self.scale)
         self.mean.copy_(rm)
         torch.addcmul(b.detach(), rm, self.scale, value=-1.0, out=self.shift)
+
+    def _module(self, c0, C):
+        """(index, channel offset) of the reference module that holds channels [c0, c0+C): any
+        range of a single module, exactly one module's channels otherwise."""
+        if self.single:
+            return 0, c0
+        for i, (s0, n) in enumerate(self.slices):
+            if (s0, n) == (c0, C):
+                return i, 0
+        raise nat.NativeError("BatchNorm slice does not match a reference module")
+
+    def fwd_struct(self, count, c0=0, C=None):
+        """yamb_bn_fwd of channels [c0, c0+C) (all by default) over `count` rows, with the
+        statistics workspace of the current stream: build it right before its launch."""
+        C = self.C if C is None else C
+        i, off = self._module(c0, C)
+        m = self.mods[i]
+        s = nat.BnFwd()
+        s.partials, s.counter = Workspace.get(self.dev).stats(C)
+        s.gamma, s.beta = _at(m.weight, off), _at(m.bias, off)
+        s.eps, s.momentum = self.eps, self.momentum_value()
+        if m.track_running_stats and m.running_mean is not None:
+            s.running_mean, s.running_var = _at(m.running_mean, off), _at(m.running_var, off)
+            s.num_batches_tracked = nat.ptr(m.num_batches_tracked)
+        s.scale, s.shift = _at(self.scale, c0), _at(self.shift, c0)
+        s.mean, s.invstd = _at(self.mean, c0), _at(self.invstd, c0)
+        s.count = count
+        return s
+
+    def bwd_struct(self, count, grads, c0=0, C=None):
+        """yamb_bn_bwd of channels [c0, c0+C) (all by default) over `count` rows; grads: the
+        (dgamma, dbeta) accumulation targets of every module.  Built like `fwd_struct`."""
+        C = self.C if C is None else C
+        i, off = self._module(c0, C)
+        s = nat.BnBwd()
+        s.partials, s.counter = Workspace.get(self.dev).stats(C)
+        s.gamma = _at(self.mods[i].weight, off)
+        s.mean, s.invstd = _at(self.mean, c0), _at(self.invstd, c0)
+        dg, db = grads[i]
+        s.dgamma, s.dbeta = _at(dg, off), _at(db, off)
+        s.ca, s.cb, s.cc = _at(self.ca, c0), _at(self.cb, c0), _at(self.cc, c0)
+        s.count = count
+        s.use_batch_stats = 1 if self.batch_stats else 0
+        return s
 
 
 BlockParts = collections.namedtuple(
@@ -279,7 +334,6 @@ class _NlTail:
         self.F = _f32(N * self.cr * C, dev)
         self.df = self.dl = self.dF = None
         self.in_dh = None
-        self.keep = []
 
     def gram(self, X, I, Y, sub, alpha, G, tag):
         g = nat.NlGram()
@@ -287,7 +341,6 @@ class _NlTail:
         g.X, g.ldx, g.I = X.data_ptr(), self.C, I
         g.Y, g.ldy, g.J = Y.data_ptr(), self.C, self.C
         g.alpha, g.G = alpha, G.data_ptr()
-        self.keep.append(g)
         launch(lib_fn("yamb_nl_gram_fwd"), g, tag, 4 * self.M * self.C // (sub * sub))
 
     def rowmat(self, X, K, Mat, sk, so, O, sub, alpha, out, tag, base=None, accumulate=0):
@@ -300,14 +353,11 @@ class _NlTail:
             r.base, r.ldb, r.O_copy = base.data_ptr(), self.C, self.C
         r.accumulate = accumulate
         r.out, r.ldo = out.data_ptr(), self.C
-        self.keep.append(r)
         launch(lib_fn("yamb_nl_rowmat_fwd"), r, tag, 4 * self.M * self.C // (sub * sub))
 
-    def forward(self, xm, y, residual, bn_fwd_struct=None):
-        """self.l -> y.  bn_fwd_struct(bn, count): the yamb_bn_fwd of BN4 when it normalises with
-        batch statistics (train mode); otherwise BN4 is folded from its running statistics."""
+    def forward(self, xm, y, residual):
+        """self.l -> y."""
         lib = nat.lib()
-        self.keep = []
         Cc, c = self.C, self.cr
         instance = self.instance and self.bn4.batch_stats
         if instance and self.H * self.W == 1:
@@ -326,7 +376,7 @@ class _NlTail:
         if instance:
             pass                               # statistics per sample: yamb_instance_norm_fwd
         elif self.bn4.batch_stats:
-            d.bn = C.pointer(bn_fwd_struct(self.bn4, self.M))
+            d.bn = C.pointer(self.bn4.fwd_struct(self.M))
         else:
             self.bn4.eval_coeffs()
         launch(lib.yamb_depthwise_fwd, d, "nl_dw_fwd", 4 * Cc * self.M, 2 * self.M * Cc * 9)
@@ -344,7 +394,6 @@ class _NlTail:
         if residual:
             a.residual2, a.ldr2 = xm.data_ptr(), Cc
         a.y = y.data_ptr()
-        self.keep += [d, a]
         launch(lib.yamb_bn_apply_fwd, a, "nl_bn_apply", 2 * self.M * Cc * (4 if residual else 3))
 
     def _instance_forward(self, xm, y, residual):
@@ -368,7 +417,6 @@ class _NlTail:
             s.residual2, s.ldr2 = xm.data_ptr(), Cc
         s.y, s.ldy = y.data_ptr(), Cc
         s.counter = Workspace.get(self.l.device).counter.data_ptr()
-        self.keep.append(s)
         launch(nat.lib().yamb_instance_norm_fwd, s, "nl_in_fwd",
                2 * self.M * Cc * (5 if residual else 4))
 
@@ -386,14 +434,12 @@ class _NlTail:
         s.dgamma, s.dbeta = nat.ptr(dg), nat.ptr(db)
         s.dh = dh.data_ptr()
         s.counter = Workspace.get(self.l.device).counter.data_ptr()
-        self.keep.append(s)
         launch(nat.lib().yamb_instance_norm_bwd, s, "nl_in_bwd", 2 * self.M * Cc * 5)
 
-    def backward(self, dym, grads, bn_bwd_struct):
+    def backward(self, dym, grads):
         """dy -> dl (gradient of the BN3 output): norm backward, depthwise 3x3 backward, the two
         products' backward, plus the `+ l` pass-through.  grads: the plan's accumulation targets
-        ('bn4', 'nl_dw'); bn_bwd_struct(bn, count, grads): the yamb_bn_bwd of BN4 (batch or
-        running statistics; unused after an InstanceNorm forward with per-sample statistics)."""
+        ('bn4', 'nl_dw')."""
         lib = nat.lib()
         Cc, c, bf, dev = self.C, self.cr, torch.bfloat16, self.l.device
         if self.df is None:
@@ -417,7 +463,7 @@ class _NlTail:
             r = nat.BnReduce()
             r.M, r.C, r.lddy, r.ldh = self.M, Cc, Cc, Cc
             r.dy, r.h = dym.data_ptr(), self.h.data_ptr()
-            r.bn = C.pointer(bn_bwd_struct(self.bn4, self.M, grads["bn4"]))
+            r.bn = C.pointer(self.bn4.bwd_struct(self.M, grads["bn4"]))
             launch(lib.yamb_bn_reduce_bwd, r, "nl_bn_reduce", 4 * self.M * Cc)
             d.dz = dym.data_ptr()
             d.ca, d.cb, d.cc = self.bn4.ca.data_ptr(), self.bn4.cb.data_ptr(), \
@@ -426,7 +472,6 @@ class _NlTail:
         d.dw = grads["nl_dw"].data_ptr()
         d.x = self.f.data_ptr()
         d.dx = self.df.data_ptr()
-        self.keep.append(d)
         launch(lib.yamb_depthwise_bwd, d, "nl_dw_bwd", 8 * Cc * self.M, 4 * self.M * Cc * 9)
         # dF = (W/H) theta^T df (all pixels);  dl = dy + [dtheta | 0];  sub-sampled rows += dphi, dg
         self.gram(self.l, c, self.df, 1, self.scale, self.dF, "nl_gram_bwd")
@@ -514,72 +559,8 @@ class BlockPlan:
         self.g_dw = [torch.zeros_like(c.weight, dtype=torch.float32) for c in self.conv_dw]
         self.generation = 0
         self.pinned = False
-        self._keep = []
 
     # -- helpers -------------------------------------------------------------------------------
-    def _bn_fwd_struct(self, bn, count, c0=0, C=None):
-        """yamb_bn_fwd for channels [c0, c0+C) of stage `bn` (per-branch slice for depthwise)."""
-        C = bn.C if C is None else C
-        s = nat.BnFwd()
-        ws = Workspace.get(self.dev)     # of the stream this launch goes to
-        s.partials, s.counter = ws.stats(C)
-        if bn.single:
-            m = bn.mods[0]
-            g, b = m.weight, m.bias
-            rm, rv, nbt = m.running_mean, m.running_var, m.num_batches_tracked
-            off = c0
-        else:
-            # slice == exactly one reference BN module
-            idx = [i for i, (s0, n) in enumerate(bn.slices) if s0 == c0 and n == C]
-            if len(idx) != 1:
-                raise nat.NativeError("BatchNorm slice does not match a reference module")
-            m = bn.mods[idx[0]]
-            g, b = m.weight, m.bias
-            rm, rv, nbt = m.running_mean, m.running_var, m.num_batches_tracked
-            off = 0
-        f4 = 4
-        s.gamma = g.data_ptr() + off * f4 if g is not None else None
-        s.beta = b.data_ptr() + off * f4 if b is not None else None
-        s.eps = bn.eps
-        s.momentum = bn.momentum_value()
-        if m.track_running_stats and rm is not None:
-            s.running_mean = rm.data_ptr() + off * f4
-            s.running_var = rv.data_ptr() + off * f4
-            s.num_batches_tracked = nbt.data_ptr() if nbt is not None else None
-        s.scale = bn.scale.data_ptr() + c0 * f4
-        s.shift = bn.shift.data_ptr() + c0 * f4
-        s.mean = bn.mean.data_ptr() + c0 * f4
-        s.invstd = bn.invstd.data_ptr() + c0 * f4
-        s.count = count
-        self._keep.append(s)
-        return s
-
-    def _bn_bwd_struct(self, bn, count, grads, c0=0, C=None):
-        C = bn.C if C is None else C
-        s = nat.BnBwd()
-        ws = Workspace.get(self.dev)     # of the stream this launch goes to
-        s.partials, s.counter = ws.stats(C)
-        f4 = 4
-        if bn.single:
-            mi, off = 0, c0
-        else:
-            mi = [i for i, (s0, n) in enumerate(bn.slices) if s0 == c0 and n == C][0]
-            off = 0
-        m = bn.mods[mi]
-        s.gamma = m.weight.data_ptr() + off * f4 if m.weight is not None else None
-        s.mean = bn.mean.data_ptr() + c0 * f4
-        s.invstd = bn.invstd.data_ptr() + c0 * f4
-        dg, db = grads[mi]
-        s.dgamma = dg.data_ptr() + off * f4 if dg is not None else None
-        s.dbeta = db.data_ptr() + off * f4 if db is not None else None
-        s.ca = bn.ca.data_ptr() + c0 * f4
-        s.cb = bn.cb.data_ptr() + c0 * f4
-        s.cc = bn.cc.data_ptr() + c0 * f4
-        s.count = count
-        s.use_batch_stats = 1 if bn.batch_stats else 0
-        self._keep.append(s)
-        return s
-
     def _refresh_weights(self):
         """fp32 master -> bf16 tensor-core operands (merged over branches).
 
@@ -624,7 +605,6 @@ class BlockPlan:
     def forward(self, x):
         """x: channels_last bf16 [N,Cin,H,W]; returns channels_last bf16 [N,Cout,Ho,Wo]."""
         lib = self.lib
-        self._keep = []
         self.generation += 1
         self._refresh_weights()
         xm = x.permute(0, 2, 3, 1).reshape(self.M_in, self.Cin)  # view, NHWC matrix
@@ -639,7 +619,7 @@ class BlockPlan:
             g.D, g.ldd = self.h1.data_ptr(), self.Chid
             if self.bn1.batch_stats:
                 if self.bn1.single:
-                    g.bn_fwd = C.pointer(self._bn_fwd_struct(self.bn1, self.M_in))
+                    g.bn_fwd = C.pointer(self.bn1.fwd_struct(self.M_in))
                     launch(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
                            2 * self.M_in * (self.Cin + self.Chid),
                            2 * self.M_in * self.Cin * self.Chid)
@@ -671,7 +651,7 @@ class BlockPlan:
             d.w = self.conv_dw[b].weight.data_ptr()
             d.y = self.h2.data_ptr() + c0 * 2
             if self.bn2.batch_stats:
-                d.bn = C.pointer(self._bn_fwd_struct(self.bn2, self.M_out, c0, cb))
+                d.bn = C.pointer(self.bn2.fwd_struct(self.M_out, c0, cb))
             launch(lib.yamb_depthwise_fwd, d, "dw_fwd", 2 * cb * (self.M_in + self.M_out),
                    2 * self.M_out * cb * k * k)
             c0 += cb
@@ -694,7 +674,6 @@ class BlockPlan:
             f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
             f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
             f.u, f.v, f.gate = self.se_u.data_ptr(), self.se_v.data_ptr(), self.gate.data_ptr()
-            self._keep.append(f)
             launch(lib.yamb_se_fc_fwd, f, "se_fc", 4 * self.N * self.Chid * 2,
                    4 * self.N * self.Chid * self.se_r)
         # 3. project 1x1 (BN2+act as operand transform) + BN3 statistics
@@ -708,7 +687,7 @@ class BlockPlan:
         if self.se is not None:
             g.a_gate, g.gate_rows_per_sample = self.gate.data_ptr(), self.Ho * self.Wo
         if self.bn3.batch_stats:
-            g.bn_fwd = C.pointer(self._bn_fwd_struct(self.bn3, self.M_out))
+            g.bn_fwd = C.pointer(self.bn3.fwd_struct(self.M_out))
         else:
             self.bn3.eval_coeffs()
         launch(lib.yamb_pointwise_gemm, g, "pw_project_fwd",
@@ -729,7 +708,7 @@ class BlockPlan:
             return y
         a.y = self.nl_tail.l.data_ptr()         # l = BN3(h3): the non-local block's input
         launch(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * self.M_out * self.Cout)
-        self.nl_tail.forward(xm, y, self.residual, self._bn_fwd_struct)
+        self.nl_tail.forward(xm, y, self.residual)
         return y
 
     def _gemm_sliced_stats(self, g, bn, count):
@@ -742,7 +721,7 @@ class BlockPlan:
             gs.N = cb
             gs.B = g.B + c0 * g.ldb * 2
             gs.D = g.D + c0 * 2
-            gs.bn_fwd = C.pointer(self._bn_fwd_struct(bn, count, c0, cb))
+            gs.bn_fwd = C.pointer(bn.fwd_struct(count, c0, cb))
             launch(lib.yamb_pointwise_gemm, gs, "pw_expand_fwd", 2 * gs.M * (gs.K + cb),
                    2 * gs.M * gs.K * cb)
 
@@ -767,7 +746,6 @@ class BlockPlan:
         b.dpool, b.dt, b.du = self.dpool.data_ptr(), self.se_dt.data_ptr(), self.se_du.data_ptr()
         tg = grads["se"]
         b.g_wr, b.g_br, b.g_we, b.g_be = (tg[k].data_ptr() for k in ("wr", "br", "we", "be"))
-        self._keep.append(b)
         launch(lib.yamb_se_fc_bwd, b, "se_fc_bwd", 4 * self.N * self.Chid * 4,
                8 * self.N * self.Chid * self.se_r)
         for (c0, cb) in self.bn2.slices:
@@ -783,7 +761,7 @@ class BlockPlan:
             a.dpool = self.dpool.data_ptr() + c0 * 4
             a.ldg = self.Chid
             a.dz = self.dz2.data_ptr() + c0 * 2
-            a.bn = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"], c0, cb))
+            a.bn = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
             launch(lib.yamb_se_bwd_apply_bwd, a, "se_bwd_apply", 6 * self.M_out * cb)
 
     # -- backward --------------------------------------------------------------------------------
@@ -792,7 +770,6 @@ class BlockPlan:
            'exp' [Chid,Cin], 'proj' [Cout,Chid], 'dw' list[[C,1,k,k]], 'bn1'/'bn2'/'bn3' lists of
            (dgamma, dbeta) per reference BN module.  Returns dx (channels_last bf16)."""
         lib = self.lib
-        self._keep = []
         bf = torch.bfloat16
         if self.dz2 is None:
             self.dh3 = torch.empty(self.M_out, self.Cout, device=self.dev, dtype=bf)
@@ -805,12 +782,12 @@ class BlockPlan:
         dx = torch.empty((self.N, self.Cin, self.H, self.W), device=self.dev, dtype=bf,
                          memory_format=torch.channels_last)
         if self.nl is not None:
-            dym = self.nl_tail.backward(dym, grads, self._bn_bwd_struct)
+            dym = self.nl_tail.backward(dym, grads)
         # 1. BN3 backward reduction -> ca3, cb3, cc3, dgamma3, dbeta3
         r = nat.BnReduce()
         r.M, r.C, r.lddy, r.ldh = self.M_out, self.Cout, self.Cout, self.Cout
         r.dy, r.h = dym.data_ptr(), self.h3.data_ptr()
-        r.bn = C.pointer(self._bn_bwd_struct(self.bn3, self.M_out, grads["bn3"]))
+        r.bn = C.pointer(self.bn3.bwd_struct(self.M_out, grads["bn3"]))
         launch(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * self.M_out * self.Cout)
         # 1b. dh3 = ca3*dy + cb3*h3 + cc3, formed once: both project GEMMs read it as a plain
         #     operand (as a loader transform it was re-read and re-formed for every n-block)
@@ -840,7 +817,7 @@ class BlockPlan:
             g.h_scale, g.h_shift, g.h_act = self.bn2.scale.data_ptr(), \
                 self.bn2.shift.data_ptr(), self.act
             if len(self.bn2.mods) == 1:
-                g.bn_bwd = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"]))
+                g.bn_bwd = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"]))
                 launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
                        2 * self.M_out * (self.Cout + 2 * self.Chid),
                        2 * self.M_out * self.Chid * self.Cout)
@@ -854,8 +831,7 @@ class BlockPlan:
                     gs.H = g.H + c0 * 2
                     gs.h_scale = g.h_scale + c0 * 4
                     gs.h_shift = g.h_shift + c0 * 4
-                    gs.bn_bwd = C.pointer(self._bn_bwd_struct(self.bn2, self.M_out, grads["bn2"],
-                                                              c0, cb))
+                    gs.bn_bwd = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
                     launch(lib.yamb_pointwise_gemm, gs, "pw_project_dgrad",
                            2 * self.M_out * (self.Cout + 2 * cb),
                            2 * self.M_out * cb * self.Cout)
@@ -894,7 +870,7 @@ class BlockPlan:
                 d.in_shift = self.bn1.shift.data_ptr() + c0 * 4
                 d.in_act = self.act
                 d.dx = self.dz1.data_ptr() + c0 * 2
-                d.bn = C.pointer(self._bn_bwd_struct(self.bn1, self.M_in, grads["bn1"], c0, cb))
+                d.bn = C.pointer(self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb))
             else:
                 d.x = xm.data_ptr()
                 d.dx = dx.data_ptr()
@@ -1016,8 +992,7 @@ def run_backward(block, plan, x, dy):
     """Backward kernel sequence of one block; returns dx and {id(param): grad} for the parameters
     whose gradient was NOT accumulated straight into `.grad` (flat-arena direct mode)."""
     dy = to_nhwc_bf16(dy)
-    params = list(block.parameters())
-    direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
+    direct = direct_grads(block.parameters())
 
     def target(p, zero_buf):
         if direct:
@@ -1309,22 +1284,22 @@ class _PadFn(torch.autograd.Function):
         dx, gmap = run_backward(sh.shadow, plan, x, dy)
         grads = sh.gather_grads(gmap, block)
         params = list(block.parameters())
-        if all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params):
+        if direct_grads(params):
             torch._foreach_add_([p.grad for p in params], grads)   # straight into the flat arena
             return (dx, None) + (None,) * len(params)
         return (dx, None) + tuple(grads)
 
 
 # ------------------------------------------------------------------------------------------------
-# Stand-alone BatchNorm + activation behind a convolution torch runs (stem 3x3 / head 1x1
-# ConvBNReLU, reference models/mobilenet_base.py:181-203): raw conv output h [N,H,W,C] bf16 ->
-# statistics kernel (+ finalize) -> y = act(scale*h + shift); backward: statistics of
-# dz = dy*act'(z) (+ finalize: dgamma, dbeta, ca/cb/cc) -> dh = ca*dz + cb*h + cc.
+# Stand-alone BatchNorm + activation of a ConvBNReLU (reference models/mobilenet_base.py:181-203)
+# behind the stem 3x3 / head 1x1 convolution kernels or a convolution torch runs: raw conv output
+# h [N,H,W,C] bf16 -> statistics kernel (+ finalize; skipped when the kernel that wrote h took the
+# statistics) -> y = act(scale*h + shift); backward: statistics of dz = dy*act'(z) (+ finalize:
+# dgamma, dbeta, ca/cb/cc) -> dh = ca*dz + cb*h + cc.
 # ------------------------------------------------------------------------------------------------
 class _BnActState(Scratch):
     def __init__(self, bn, dev):
         self.bn = _Bn([bn], dev)
-        self.keep = []
         self.gbuf = None
 
 
@@ -1338,39 +1313,25 @@ def _bn_act_state(bn, dev):
 
 class _BnActFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, h, bn, act, weight, bias):
+    def forward(ctx, h, bn, act, weight, bias, stats_taken):
         lib = nat.lib()
         st = _bn_act_state(bn, h.device)
-        st.keep = []
         b = st.bn
         N, Cc, H, W = h.shape
         M = N * H * W
         hm = h.permute(0, 2, 3, 1).reshape(M, Cc)        # view of the channels_last storage
-        if b.batch_stats:
-            f = nat.BnFwd()
-            ws = Workspace.get(h.device)
-            f.partials, f.counter = ws.stats(Cc)
-            f.gamma, f.beta = nat.ptr(bn.weight), nat.ptr(bn.bias)
-            f.eps, f.momentum = b.eps, b.momentum_value()
-            if bn.track_running_stats and bn.running_mean is not None:
-                f.running_mean, f.running_var = bn.running_mean.data_ptr(), bn.running_var.data_ptr()
-                f.num_batches_tracked = nat.ptr(bn.num_batches_tracked)
-            f.scale, f.shift = b.scale.data_ptr(), b.shift.data_ptr()
-            f.mean, f.invstd = b.mean.data_ptr(), b.invstd.data_ptr()
-            f.count = M
-            s = nat.BnStats()
-            s.M, s.C, s.ldh, s.h, s.bn = M, Cc, Cc, hm.data_ptr(), C.pointer(f)
-            st.keep += [f, s]
-            launch(lib.yamb_bn_stats_fwd, s, "bn_stats", 2 * M * Cc)
-        else:
+        if not b.batch_stats:
             with torch.no_grad():
                 b.eval_coeffs()
+        elif not stats_taken:
+            s = nat.BnStats()
+            s.M, s.C, s.ldh, s.h, s.bn = M, Cc, Cc, hm.data_ptr(), C.pointer(b.fwd_struct(M))
+            launch(lib.yamb_bn_stats_fwd, s, "bn_stats", 2 * M * Cc)
         y = torch.empty_like(h, memory_format=torch.channels_last)
         a = nat.BnApply()
         a.M, a.C, a.ldh, a.ldr, a.ldy = M, Cc, Cc, Cc, Cc
         a.h, a.scale, a.shift, a.act = hm.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), act
         a.y = y.data_ptr()
-        st.keep.append(a)
         launch(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * M * Cc)
         ctx.bn, ctx.act, ctx.st = bn, act, st
         # per-call copy of [scale, shift, mean, invstd]: another forward through this module before
@@ -1393,8 +1354,7 @@ class _BnActFn(torch.autograd.Function):
         M = N * H * W
         hm = h.permute(0, 2, 3, 1).reshape(M, Cc)
         dym = dy.permute(0, 2, 3, 1).reshape(M, Cc)
-        params = [p for p in (bn.weight, bn.bias) if p is not None]
-        direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
+        direct = direct_grads((bn.weight, bn.bias))
         if direct:
             dg, db = bn.weight.grad, bn.bias.grad
         else:
@@ -1403,15 +1363,8 @@ class _BnActFn(torch.autograd.Function):
             st.gbuf[0].zero_()
             st.gbuf[1].zero_()
             dg, db = st.gbuf
-        g = nat.BnBwd()
-        ws = Workspace.get(h.device)
-        g.partials, g.counter = ws.stats(Cc)
-        g.gamma = nat.ptr(bn.weight)
-        g.mean, g.invstd = c_mean, c_invstd
-        g.dgamma, g.dbeta = dg.data_ptr(), db.data_ptr()
-        g.ca, g.cb, g.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
-        g.count = M
-        g.use_batch_stats = 1 if b.batch_stats else 0
+        g = b.bwd_struct(M, [(dg, db)])
+        g.mean, g.invstd = c_mean, c_invstd      # this call's statistics, not the live buffers
         r = nat.BnReduce()
         r.M, r.C, r.lddy, r.ldh = M, Cc, Cc, Cc
         r.dy, r.h, r.bn = dym.data_ptr(), hm.data_ptr(), C.pointer(g)
@@ -1424,19 +1377,20 @@ class _BnActFn(torch.autograd.Function):
         a.z_scale, a.z_shift, a.z_act = c_scale, c_shift, act
         a.ca, a.cb, a.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
         a.dh = dh.data_ptr()
-        st.keep += [g, r, a]
         launch(lib.yamb_bn_bwd_apply_bwd, a, "bn_bwd_apply", 6 * M * Cc)
         if direct:
-            return dh, None, None, None, None
-        return dh, None, None, dg.clone(), db.clone()
+            return dh, None, None, None, None, None
+        return dh, None, None, dg.clone(), db.clone(), None
 
 
-def bn_act_apply(bn, active_fn, h):
-    """y = act(BatchNorm(h)) for a raw convolution output on CUDA (training or eval)."""
+def bn_act_apply(bn, active_fn, h, stats_taken=False):
+    """y = act(BatchNorm(h)) for a raw convolution output on CUDA (training or eval).
+    stats_taken: the kernel that wrote h already took its batch statistics (a GEMM epilogue given
+    `_bn_act_state(bn, dev).bn.fwd_struct`); ignored when `bn` folds its running statistics."""
     h = to_nhwc_bf16(h)
     if h.shape[1] % 8:
         raise nat.NativeError("bn_act: channel count must be a multiple of 8")
-    return _BnActFn.apply(h, bn, act_code_of(active_fn), bn.weight, bn.bias)
+    return _BnActFn.apply(h, bn, act_code_of(active_fn), bn.weight, bn.bias, stats_taken)
 
 
 # ---- eval mode: the whole block in one launch (csrc/block_eval.cu) ---------------------------------

@@ -25,24 +25,13 @@ def _mat(t):
 
 
 class _PwState(engine.Scratch):
-    """Per-module device state of a 1x1 ConvBNReLU: BatchNorm coefficients, bf16 weight copy."""
+    """Per-module device state of a 1x1 convolution: bf16 weight copy, fp32 weight gradient."""
 
-    def __init__(self, conv, bn, dev):
-        self.bn = engine._Bn([bn], dev)
+    def __init__(self, conv, dev):
         self.w_own = torch.empty(conv.out_channels, conv.in_channels, device=dev,
                                  dtype=torch.bfloat16)
         self.g_own = None
-        self.gbuf = None
-        self.keep = []
         self.dev = dev
-
-
-def _pw_state(mod, dev):
-    st = mod.__dict__.get("_yamb_pw")
-    if st is None or st.dev != dev:
-        st = _PwState(mod[0], mod[1], dev)
-        mod.__dict__["_yamb_pw"] = st
-    return st
 
 
 def _gemm(M, N, K, A, lda, B, ldb, D, ldd, **kw):
@@ -54,107 +43,50 @@ def _gemm(M, N, K, A, lda, B, ldb, D, ldd, **kw):
     return g
 
 
-class _PwConvBnActFn(torch.autograd.Function):
-    """y = act(BatchNorm(conv1x1(x))) — GEMM (+ statistics) -> BN apply; backward: BN-backward
-    reduction -> dh -> dgrad GEMM + split-K wgrad GEMM."""
+class _PwConvFn(torch.autograd.Function):
+    """Raw output h = conv1x1(x) of a ConvBNReLU by the GEMM, which takes the batch statistics of
+    the BatchNorm `bn` behind it in its epilogue when `bn` normalises with them; backward: dgrad
+    GEMM + split-K wgrad GEMM."""
 
     @staticmethod
-    def forward(ctx, x, mod, act, weight, gamma, beta):
-        lib = nat.lib()
-        conv, bn = mod[0], mod[1]
-        st = _pw_state(mod, x.device)
-        st.keep = []
-        b = st.bn
+    def forward(ctx, x, conv, bn, weight):
+        st = conv.__dict__.get("_yamb_pw")
+        if st is None or st.dev != x.device:
+            st = conv.__dict__["_yamb_pw"] = _PwState(conv, x.device)
         N, Cin, H, W = x.shape
         Cout = conv.out_channels
         M = N * H * W
-        xm = _mat(x)
         with torch.no_grad():
             wbf = engine._bf16_operand(conv.weight, st.w_own, (Cout, Cin))
         h = torch.empty((N, Cout, H, W), device=x.device, dtype=torch.bfloat16,
                         memory_format=torch.channels_last)
-        g = _gemm(M, Cout, Cin, xm.data_ptr(), Cin, wbf.data_ptr(), Cin, h.data_ptr(), Cout)
+        g = _gemm(M, Cout, Cin, _mat(x).data_ptr(), Cin, wbf.data_ptr(), Cin, h.data_ptr(), Cout)
+        b = engine._bn_act_state(bn, x.device).bn
         if b.batch_stats:
-            f = nat.BnFwd()
-            ws = engine.Workspace.get(x.device)
-            f.partials, f.counter = ws.stats(Cout)
-            f.gamma, f.beta = nat.ptr(bn.weight), nat.ptr(bn.bias)
-            f.eps, f.momentum = b.eps, b.momentum_value()
-            if bn.track_running_stats and bn.running_mean is not None:
-                f.running_mean, f.running_var = bn.running_mean.data_ptr(), \
-                    bn.running_var.data_ptr()
-                f.num_batches_tracked = nat.ptr(bn.num_batches_tracked)
-            f.scale, f.shift = b.scale.data_ptr(), b.shift.data_ptr()
-            f.mean, f.invstd = b.mean.data_ptr(), b.invstd.data_ptr()
-            f.count = M
-            g.bn_fwd = C.pointer(f)
-            st.keep.append(f)
-        else:
-            with torch.no_grad():
-                b.eval_coeffs()
-        st.keep.append(g)
-        engine.launch(lib.yamb_pointwise_gemm, g, "head_conv_fwd", 2 * M * (Cin + Cout),
+            g.bn_fwd = C.pointer(b.fwd_struct(M))
+        engine.launch(nat.lib().yamb_pointwise_gemm, g, "head_conv_fwd", 2 * M * (Cin + Cout),
                       2 * M * Cin * Cout)
-        y = torch.empty_like(h, memory_format=torch.channels_last)
-        a = nat.BnApply()
-        a.M, a.C, a.ldh, a.ldr, a.ldy = M, Cout, Cout, Cout, Cout
-        a.h, a.scale, a.shift, a.act = h.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), act
-        a.y = y.data_ptr()
-        st.keep.append(a)
-        engine.launch(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * M * Cout)
-        coef = torch.stack((b.scale, b.shift, b.mean, b.invstd)) if any(ctx.needs_input_grad) \
-            else None
-        ctx.mod, ctx.act, ctx.st = mod, act, st
-        ctx.save_for_backward(x, h, coef, wbf)
-        return y
+        ctx.conv, ctx.st = conv, st
+        ctx.save_for_backward(x, wbf)
+        return h
 
     @staticmethod
-    def backward(ctx, dy):
+    def backward(ctx, dh):
         lib = nat.lib()
-        x, h, coef, wbf = ctx.saved_tensors
-        mod, act, st = ctx.mod, ctx.act, ctx.st
-        conv, bn = mod[0], mod[1]
-        b = st.bn
-        dy = engine.to_nhwc_bf16(dy)
+        x, wbf = ctx.saved_tensors
+        conv, st = ctx.conv, ctx.st
+        dh = engine.to_nhwc_bf16(dh)
         N, Cin, H, W = x.shape
         Cout = conv.out_channels
         M = N * H * W
-        xm, hm, dym = _mat(x), _mat(h), _mat(dy)
-        c_scale, c_shift, c_mean, c_invstd = (coef[i].data_ptr() for i in range(4))
-        params = [conv.weight, bn.weight, bn.bias]
-        direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
+        direct = engine.direct_grads((conv.weight,))
         if direct:
-            dg, db, gw = bn.weight.grad, bn.bias.grad, conv.weight.grad
+            gw = conv.weight.grad
         else:
-            if st.gbuf is None:
-                st.gbuf = (torch.zeros_like(bn.weight), torch.zeros_like(bn.bias))
+            if st.g_own is None:
                 st.g_own = torch.zeros(Cout, Cin, device=x.device, dtype=torch.float32)
-            for t in st.gbuf + (st.g_own,):
-                t.zero_()
-            dg, db, gw = st.gbuf[0], st.gbuf[1], st.g_own
-        # BatchNorm-backward statistics of dz = dy * act'(z), then dh = ca*dz + cb*h + cc
-        q = nat.BnBwd()
-        ws = engine.Workspace.get(x.device)
-        q.partials, q.counter = ws.stats(Cout)
-        q.gamma = nat.ptr(bn.weight)
-        q.mean, q.invstd = c_mean, c_invstd
-        q.dgamma, q.dbeta = dg.data_ptr(), db.data_ptr()
-        q.ca, q.cb, q.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
-        q.count = M
-        q.use_batch_stats = 1 if b.batch_stats else 0
-        r = nat.BnReduce()
-        r.M, r.C, r.lddy, r.ldh = M, Cout, Cout, Cout
-        r.dy, r.h, r.bn = dym.data_ptr(), hm.data_ptr(), C.pointer(q)
-        r.z_scale, r.z_shift, r.z_act = c_scale, c_shift, act
-        engine.launch(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * M * Cout)
-        dh = torch.empty(M, Cout, device=x.device, dtype=torch.bfloat16)
-        a = nat.BnBwdApply()
-        a.M, a.C, a.lddy, a.ldh, a.lddh = M, Cout, Cout, Cout, Cout
-        a.dy, a.h = dym.data_ptr(), hm.data_ptr()
-        a.z_scale, a.z_shift, a.z_act = c_scale, c_shift, act
-        a.ca, a.cb, a.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
-        a.dh = dh.data_ptr()
-        engine.launch(lib.yamb_bn_bwd_apply_bwd, a, "bn_bwd_apply", 6 * M * Cout)
+            st.g_own.zero_()
+            gw = st.g_own
         # dgrad: dx[M, Cin] = dh[M, Cout] * W[Cout, Cin]   (weight read MN-major)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -165,20 +97,21 @@ class _PwConvBnActFn(torch.autograd.Function):
             engine.launch(lib.yamb_pointwise_gemm, g, "head_conv_dgrad", 2 * M * (Cin + Cout),
                           2 * M * Cin * Cout)
         # wgrad: dW[Cout, Cin] += dh^T x   (pixels on K, split-K, slabs added in a fixed order)
-        g2 = _gemm(Cout, Cin, M, dh.data_ptr(), Cout, xm.data_ptr(), Cin, gw.data_ptr(), Cin,
+        g2 = _gemm(Cout, Cin, M, dh.data_ptr(), Cout, _mat(x).data_ptr(), Cin, gw.data_ptr(), Cin,
                    a_mn_major=1, b_mn_major=1, epi=2)
         engine.launch(lib.yamb_pointwise_gemm, g2, "head_conv_wgrad", 2 * M * (Cin + Cout),
                       2 * M * Cin * Cout)
-        if direct:
-            return dx, None, None, None, None, None
-        return dx, None, None, gw.view_as(conv.weight).clone(), dg.clone(), db.clone()
+        return dx, None, None, (None if direct else gw.view_as(conv.weight).clone())
 
 
 def pw_conv_bn_act(mod, x):
-    """ConvBNReLU with a 1x1 convolution (reference models/mobilenet_base.py:181-203) on CUDA."""
+    """ConvBNReLU with a 1x1 convolution (reference models/mobilenet_base.py:181-203) on CUDA:
+    pointwise GEMM (+ BatchNorm statistics in its epilogue) -> BatchNorm apply + activation
+    (engine.bn_act_apply)."""
     x = engine.to_nhwc_bf16(x)
     conv, bn, act = mod[0], mod[1], mod[2]
-    return _PwConvBnActFn.apply(x, mod, engine.act_code_of(act), conv.weight, bn.weight, bn.bias)
+    h = _PwConvFn.apply(x, conv, bn, conv.weight)
+    return engine.bn_act_apply(bn, act, h, stats_taken=True)
 
 
 def pw_conv_supported(mod, x):
@@ -233,8 +166,7 @@ class _LinearFn(torch.autograd.Function):
         dy = dy.contiguous()
         if dy.dtype != torch.bfloat16:
             dy = dy.to(torch.bfloat16)
-        direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None
-                     for p in (lin.weight, lin.bias))
+        direct = engine.direct_grads((lin.weight, lin.bias))
         if direct:
             gw = lin.weight.grad
         else:
@@ -361,7 +293,7 @@ class _StemConvFn(torch.autograd.Function):
         N, _, H, W = x.shape
         Cout = conv.out_channels
         w = conv.weight
-        direct = getattr(w, "_yamb_direct", False) and w.grad is not None
+        direct = engine.direct_grads((w,))
         gw = w.grad if direct else torch.zeros_like(w, dtype=torch.float32)
         a = nat.StemConv()
         a.N, a.H, a.W, a.Cout = N, H, W, Cout
