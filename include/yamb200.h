@@ -361,6 +361,41 @@ typedef struct yamb_stem_conv {
 int yamb_stem_conv_fwd(const yamb_stem_conv* args, yamb_stream_t stream);
 int yamb_stem_conv_wgrad(const yamb_stem_conv* args, yamb_stream_t stream);
 
+/* Eval-mode stem ConvBNReLU in ONE launch: the forward kernel of yamb_stem_conv_fwd with the folded
+ * BatchNorm and the activation applied before the store,
+ *   y = bf16(act(scale[c] * bf16(conv) + shift[c]))
+ * with exactly the expression of yamb_bn_apply_fwd, so y is bitwise equal to yamb_stem_conv_fwd
+ * followed by yamb_bn_apply_fwd with the same scale / shift.  Shapes as yamb_stem_conv_fwd
+ * (conv.dh / conv.dw unused). */
+typedef struct yamb_stem_conv_eval {
+  yamb_stem_conv conv;
+  const float* scale;   /* [Cout] gamma * rsqrt(running_var + eps) */
+  const float* shift;   /* [Cout] beta - running_mean * scale */
+  int32_t act;          /* YAMB_ACT_* */
+} yamb_stem_conv_eval;
+
+int yamb_stem_conv_eval_fwd(const yamb_stem_conv_eval* args, yamb_stream_t stream);
+
+/* ---- eval-mode head: 1x1 ConvBNReLU + full-extent average pool, ONE launch ------------------------
+ * Replaces, in eval mode, the head ConvBNReLU (reference models/mobilenet_supernet.py:152-158) and
+ * the AvgPool2d over the whole final feature map (:159):
+ *   pooled[n][c] = bf16((1/HW) * sum_p bf16(act(scale[c] * bf16(x[n,p,:] . w[c,:]) + shift[c])))
+ * The per-element rounding points are those of yamb_pointwise_gemm -> yamb_bn_apply_fwd; the sum
+ * over p is fp32 in a fixed order (the same bits on every run).  The conv output and the activation
+ * never reach HBM; `pooled` is the bf16 [N][Cout] operand of the classifier GEMM.  wgmma tensor
+ * cores; Cin, Cout multiples of 8, Cin <= 512, any HW >= 1.  Other shapes return YAMB_EINVAL. */
+typedef struct yamb_head_pool_eval {
+  int32_t N, HW, Cin, Cout;
+  const void* x;        /* bf16 [N][HW][Cin] (NHWC), 16-byte aligned */
+  const void* w;        /* bf16 [Cout][Cin], 16-byte aligned */
+  const float* scale;   /* [Cout] */
+  const float* shift;   /* [Cout] */
+  int32_t act;          /* YAMB_ACT_* */
+  void* pooled;         /* out bf16 [N][Cout] */
+} yamb_head_pool_eval;
+
+int yamb_head_pool_eval_fwd(const yamb_head_pool_eval* args, yamb_stream_t stream);
+
 /* ---- label-smoothed softmax cross entropy + top-k -------------------------------------------------
  * Replaces CrossEntropyLabelSmooth(reduction='none') (reference utils/optim.py:150-158), the
  * top-1 / top-5 `correct_k` bookkeeping of forward_loss (common.py:73-79) and their backward.
@@ -489,8 +524,8 @@ int yamb_max_ctas(void);
 /* sizeof() of the ABI structs (0 bn_fwd, 1 bn_bwd, 2 gemm, 3 dw_fwd, 4 dw_bwd, 5 bn_apply,
  * 6 bn_reduce, 7 se_pool, 8 rmsprop, 9 se_bwd_reduce, 10 se_bwd_apply, 11 bn_stats,
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
- * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd) so bindings
- * can self-check */
+ * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
+ * 25 stem_conv_eval, 26 head_pool_eval) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

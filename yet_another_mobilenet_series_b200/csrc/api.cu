@@ -77,6 +77,8 @@ int yamb_struct_size(int which) {
     case 22: return (int)sizeof(yamb_in_fwd);
     case 23: return (int)sizeof(yamb_in_bwd);
     case 24: return (int)sizeof(yamb_sgd);
+    case 25: return (int)sizeof(yamb_stem_conv_eval);
+    case 26: return (int)sizeof(yamb_head_pool_eval);
     default: return -1;
   }
 }
@@ -105,6 +107,8 @@ int yamb_colsum_bf16(const void* X, int64_t M, int32_t C, int64_t ld, float* out
 }
 int yamb_stem_conv_fwd(const yamb_stem_conv* a, yamb_stream_t s) { return yamb::stem_conv_fwd_launch(a, YAMB_ST(s)); }
 int yamb_stem_conv_wgrad(const yamb_stem_conv* a, yamb_stream_t s) { return yamb::stem_conv_wgrad_launch(a, YAMB_ST(s)); }
+int yamb_stem_conv_eval_fwd(const yamb_stem_conv_eval* a, yamb_stream_t s) { return yamb::stem_conv_eval_fwd_launch(a, YAMB_ST(s)); }
+int yamb_head_pool_eval_fwd(const yamb_head_pool_eval* a, yamb_stream_t s) { return yamb::head_pool_eval_launch(a, YAMB_ST(s)); }
 int yamb_nl_gram_fwd(const yamb_nl_gram* a, yamb_stream_t s) { return yamb::nl_gram_launch(a, YAMB_ST(s)); }
 int yamb_nl_rowmat_fwd(const yamb_nl_rowmat* a, yamb_stream_t s) { return yamb::nl_rowmat_launch(a, YAMB_ST(s)); }
 int yamb_block_eval_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_launch(a, YAMB_ST(s)); }

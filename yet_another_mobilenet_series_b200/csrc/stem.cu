@@ -9,6 +9,8 @@
 //
 // forward : thread = 2 horizontally adjacent output pixels x all output channels (8 at a time);
 //           the 3x5x3 input patch sits in registers, the weights are broadcast from shared memory.
+//           Eval variant (yamb_stem_conv_eval_fwd): the same kernel with the folded BatchNorm +
+//           activation applied before the store, so h never reaches HBM.
 // wgrad   : dW[co][ci][ky][kx] = sum_pixels dh[p][co] * x[2p+tap][ci]; thread = (pair of output
 //           channels, 2 of the 27 (tap, ci) positions); tiles of 16 x 32 output pixels are staged in
 //           shared memory; per-thread register accumulators over the CTA's tiles, one fp32
@@ -34,6 +36,9 @@ struct StemDev {
   float* dw;                  // [Cout][3][3][3] +=       (wgrad)
   float* part;                // [CTA x pixel subset][Cout][27] wgrad partials
   int tiles_h, tiles_w, num_tiles;
+  const float* scale;         // [Cout] eval forward: y = act(scale * bf16(conv) + shift)
+  const float* shift;
+  int act;
 };
 
 // The staged input tile starts ONE pixel left of the halo (column ix0 - 1) so that, with the tile
@@ -76,6 +81,10 @@ __device__ __forceinline__ void stem_stage_wait() {
   asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// EVAL: the BatchNorm (running statistics folded into scale / shift) and the activation are applied
+// between the accumulators and the staging, with the expression and rounding points of
+// bn_apply_kernel (elementwise.cu): y = bf16(act(fmaf(scale, bf16(conv), shift))).
+template <bool EVAL>
 __global__ void __launch_bounds__(256) stem_fwd_kernel(const __grid_constant__ StemDev p) {
   extern __shared__ __align__(16) unsigned char stem_smem[];
   float* s_w = reinterpret_cast<float*>(stem_smem);                // [tap*3+ci][co], 27*64 floats
@@ -146,6 +155,24 @@ __global__ void __launch_bounds__(256) stem_fwd_kernel(const __grid_constant__ S
               acc[1][e] = ffma2(a1, wv[e], acc[1][e]);
             }
           }
+      if (EVAL) {
+        const ActParam ap = make_act(p.act);
+        float z0[8], z1[8];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          z0[2 * e] = fmaf(p.scale[c0 + 2 * e], round_bf16(acc[0][e].x), p.shift[c0 + 2 * e]);
+          z0[2 * e + 1] = fmaf(p.scale[c0 + 2 * e + 1], round_bf16(acc[0][e].y), p.shift[c0 + 2 * e + 1]);
+          z1[2 * e] = fmaf(p.scale[c0 + 2 * e], round_bf16(acc[1][e].x), p.shift[c0 + 2 * e]);
+          z1[2 * e + 1] = fmaf(p.scale[c0 + 2 * e + 1], round_bf16(acc[1][e].y), p.shift[c0 + 2 * e + 1]);
+        }
+        act_vec<8>(z0, ap);
+        act_vec<8>(z1, ap);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          acc[0][e] = make_float2(z0[2 * e], z0[2 * e + 1]);
+          acc[1][e] = make_float2(z1[2 * e], z1[2 * e + 1]);
+        }
+      }
       // staging layout: [row hp][pixel 0..31][V vectors]
       uint4* so = s_out + (hp * 32 + 2 * cp) * V + (c0 >> 3);
       so[0] = make_uint4(pack_bf16(acc[0][0].x, acc[0][0].y), pack_bf16(acc[0][1].x, acc[0][1].y),
@@ -273,31 +300,53 @@ static int stem_fill(const yamb_stem_conv* a, StemDev& p) {
   return 0;
 }
 
+template <bool EVAL>
+static int stem_fwd_run(const StemDev& p, int Cout, cudaStream_t st) {
+  const size_t smem = 27 * 64 * 4 + (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
+                      (size_t)8 * 64 * (Cout / 8) * 16;
+  static size_t attr_f = 0;   // process-wide: only ever raise the limit
+  cudaError_t e;
+  if (smem > attr_f) {
+    e = cudaFuncSetAttribute(stem_fwd_kernel<EVAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem fwd attr: %s", cudaGetErrorString(e));
+    attr_f = smem;
+  }
+  static int per_sm_f = 0;
+  if (per_sm_f == 0 &&
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_f, stem_fwd_kernel<EVAL>, 256, smem) != cudaSuccess)
+    per_sm_f = 2;
+  const int res_f = max_ctas() * (per_sm_f > 0 ? per_sm_f : 1);   // one resident wave: no tail
+  stem_fwd_kernel<EVAL><<<p.num_tiles < res_f ? p.num_tiles : res_f, 256, smem, st>>>(p);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv fwd: %s", cudaGetErrorString(e));
+  return 0;
+}
+
 int stem_conv_fwd_launch(const yamb_stem_conv* a, cudaStream_t st) {
   StemDev p;
   int rc = stem_fill(a, p);
   if (rc) return rc;
   if (!a->w || !a->y || (reinterpret_cast<uintptr_t>(a->y) & 15))
     return set_error(YAMB_EINVAL, "stem conv fwd: w / y (16-byte aligned) required");
-  const int cap = 4 * max_ctas();
-  const size_t smem = 27 * 64 * 4 + (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
-                      (size_t)8 * 64 * (a->Cout / 8) * 16;
-  static size_t attr_f = 0;   // process-wide: only ever raise the limit
-  cudaError_t e;
-  if (smem > attr_f) {
-    e = cudaFuncSetAttribute(stem_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem fwd attr: %s", cudaGetErrorString(e));
-    attr_f = smem;
-  }
-  static int per_sm_f = 0;
-  if (per_sm_f == 0 &&
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_f, stem_fwd_kernel, 256, smem) != cudaSuccess)
-    per_sm_f = 2;
-  const int res_f = max_ctas() * (per_sm_f > 0 ? per_sm_f : 1);   // one resident wave: no tail
-  stem_fwd_kernel<<<p.num_tiles < res_f ? p.num_tiles : res_f, 256, smem, st>>>(p);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv fwd: %s", cudaGetErrorString(e));
-  return 0;
+  p.scale = p.shift = nullptr;
+  p.act = 0;
+  return stem_fwd_run<false>(p, a->Cout, st);
+}
+
+int stem_conv_eval_fwd_launch(const yamb_stem_conv_eval* a, cudaStream_t st) {
+  if (!a) return set_error(YAMB_EINVAL, "stem conv eval: bad arguments");
+  StemDev p;
+  int rc = stem_fill(&a->conv, p);
+  if (rc) return rc;
+  if (!a->conv.w || !a->conv.y || (reinterpret_cast<uintptr_t>(a->conv.y) & 15) || !a->scale ||
+      !a->shift)
+    return set_error(YAMB_EINVAL, "stem conv eval: w / y (16-byte aligned) / scale / shift required");
+  if (a->act < YAMB_ACT_NONE || a->act > YAMB_ACT_HSWISH)
+    return set_error(YAMB_EINVAL, "stem conv eval: act=%d", a->act);
+  p.scale = a->scale;
+  p.shift = a->shift;
+  p.act = a->act;
+  return stem_fwd_run<true>(p, a->conv.Cout, st);
 }
 
 int stem_conv_wgrad_launch(const yamb_stem_conv* a, cudaStream_t st) {

@@ -47,6 +47,26 @@ def launch(fn, st, tag="", nbytes=0, flops=0):
     PROFILE.append((tag, nbytes, flops, e0, e1))
 
 
+def try_launch(fn, st, tag="", nbytes=0, flops=0):
+    """`launch` for an entry point that may decline a shape: False, with nothing enqueued, when
+    it returns YAMB_EINVAL (the caller then runs its unfused sequence); other errors raise."""
+    global LAUNCHES
+    e0 = None
+    if PROFILE is not None:
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+    rc = fn(C.byref(st), nat.stream_handle())
+    if rc == nat.EINVAL:
+        return False
+    nat.check(rc)
+    LAUNCHES += 1
+    if PROFILE is not None:
+        e1 = torch.cuda.Event(enable_timing=True)
+        e1.record()
+        PROFILE.append((tag, nbytes, flops, e0, e1))
+    return True
+
+
 # ---- weight-gradient side stream -------------------------------------------------------------------
 # The split-K wgrad GEMMs feed nothing but the optimizer, so they leave the dgrad -> depthwise ->
 # dgrad dependency chain: they are enqueued on a second stream right after the kernel that produces
@@ -1397,6 +1417,15 @@ def bn_act_apply(bn, active_fn, h, stats_taken=False):
 # YAMB_EVAL_FUSED=0 keeps the four-launch sequence (folded coefficients) for every block.
 EVAL_FUSED = os.environ.get("YAMB_EVAL_FUSED", "1") != "0"
 EVAL_FUSED_CALLS = 0     # blocks that went through yamb_block_eval_fwd (tests / bench)
+
+# ---- eval mode: the layers around the blocks (tail_ops.stem_eval / head_pool_eval) ----------------
+# Off by default, so that a plain model.eval() forward launches what it always launched.  When True
+# (trainer.EvalStep turns it on for its own forwards) the stem ConvBNReLU runs as one launch
+# (yamb_stem_conv_eval_fwd) and the head ConvBNReLU + full-extent average pool as one launch
+# (yamb_head_pool_eval_fwd), whenever no gradient is wanted, their BatchNorms use running statistics
+# and the kernels cover the shape; otherwise the unfused sequence runs.
+EVAL_TAIL_FUSED = False
+EVAL_TAIL_CALLS = 0      # stem / head calls that went through the one-launch kernels (tests)
 
 
 def _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p):

@@ -53,9 +53,23 @@ def _full_extent(pool, x):
 def run_features(model, x):
     """Shared forward of both builders: bf16 channels_last through stem, blocks, head, pool."""
     if x.is_cuda:
+        from . import tail_ops
         x = engine.to_nhwc_bf16(x)
+        layers = list(model.features)
         with torch.autocast("cuda", dtype=torch.bfloat16):
-            for layer in model.features:
+            skip = False
+            for i, layer in enumerate(layers):
+                if skip:
+                    skip = False
+                    continue
+                nxt = layers[i + 1] if i + 1 < len(layers) else None
+                if (engine.EVAL_TAIL_FUSED and isinstance(layer, ConvBNReLU)
+                        and isinstance(nxt, nn.AvgPool2d) and _full_extent(nxt, x)):
+                    # eval: head 1x1 ConvBNReLU + global average pool in one launch (when covered)
+                    y = tail_ops.head_pool_eval(layer, x)
+                    if y is not None:
+                        x, skip = y, True
+                        continue
                 if (isinstance(layer, nn.AvgPool2d) and _full_extent(layer, x)):
                     # global average pool: same numbers as nn.AvgPool2d(H), but torch's NHWC
                     # avg_pool2d backward kernel took 0.24 ms for this 16 M-element tensor

@@ -34,6 +34,13 @@ class _PwState(engine.Scratch):
         self.dev = dev
 
 
+def _pw_state(conv, dev):
+    st = conv.__dict__.get("_yamb_pw")
+    if st is None or st.dev != dev:
+        st = conv.__dict__["_yamb_pw"] = _PwState(conv, dev)
+    return st
+
+
 def _gemm(M, N, K, A, lda, B, ldb, D, ldd, **kw):
     g = nat.Gemm()
     g.M, g.N, g.K = M, N, K
@@ -50,9 +57,7 @@ class _PwConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, conv, bn, weight):
-        st = conv.__dict__.get("_yamb_pw")
-        if st is None or st.dev != x.device:
-            st = conv.__dict__["_yamb_pw"] = _PwState(conv, x.device)
+        st = _pw_state(conv, x.device)
         N, Cin, H, W = x.shape
         Cout = conv.out_channels
         M = N * H * W
@@ -112,6 +117,39 @@ def pw_conv_bn_act(mod, x):
     conv, bn, act = mod[0], mod[1], mod[2]
     h = _PwConvFn.apply(x, conv, bn, conv.weight)
     return engine.bn_act_apply(bn, act, h, stats_taken=True)
+
+
+def _tail_eval_wanted(bn):
+    return engine.EVAL_TAIL_FUSED and not torch.is_grad_enabled() and engine._bn_eval_ready(bn)
+
+
+def head_pool_eval(mod, x):
+    """Eval-mode head ConvBNReLU 1x1 followed by the full-extent average pool in one launch
+    (yamb_head_pool_eval_fwd): bf16 [N, Cout, 1, 1], or None when the call is not covered
+    (switch off, gradient wanted, BatchNorm on batch statistics, shape) and the caller runs the
+    unfused sequence."""
+    conv, bn, act = mod[0], mod[1], mod[2]
+    if not (_tail_eval_wanted(bn) and pw_conv_supported(mod, x)):
+        return None
+    x = engine.to_nhwc_bf16(x)
+    N, Cin, H, W = x.shape
+    Cout = conv.out_channels
+    st = _pw_state(conv, x.device)
+    b = engine._bn_act_state(bn, x.device).bn
+    with torch.no_grad():
+        wbf = engine._bf16_operand(conv.weight, st.w_own, (Cout, Cin))
+        b.eval_coeffs()
+    pooled = torch.empty(N, Cout, device=x.device, dtype=torch.bfloat16)
+    a = nat.HeadPoolEval()
+    a.N, a.HW, a.Cin, a.Cout = N, H * W, Cin, Cout
+    a.x, a.w = x.data_ptr(), wbf.data_ptr()
+    a.scale, a.shift, a.act = b.scale.data_ptr(), b.shift.data_ptr(), engine.act_code_of(act)
+    a.pooled = pooled.data_ptr()
+    if not engine.try_launch(nat.lib().yamb_head_pool_eval_fwd, a, "head_pool_eval",
+                             2 * (N * H * W * Cin + Cout * Cin + N * Cout), 2 * N * H * W * Cin * Cout):
+        return None
+    engine.EVAL_TAIL_CALLS += 1
+    return pooled.view(N, Cout, 1, 1)
 
 
 def pw_conv_supported(mod, x):
@@ -319,5 +357,31 @@ def stem_conv_bn_act(mod, x):
     BatchNorm apply + activation (engine.bn_act_apply)."""
     x = engine.to_nhwc_bf16(x)
     conv, bn, act = mod[0], mod[1], mod[2]
+    if _tail_eval_wanted(bn):
+        y = _stem_eval(conv, bn, act, x)
+        if y is not None:
+            return y
     h = _StemConvFn.apply(x, conv, conv.weight)
     return engine.bn_act_apply(bn, act, h)
+
+
+def _stem_eval(conv, bn, act, x):
+    """Eval-mode stem in one launch (yamb_stem_conv_eval_fwd), bitwise equal to the stem kernel
+    followed by bn_act_apply; None when the kernel declines the shape."""
+    N, _, H, W = x.shape
+    Cout = conv.out_channels
+    Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    b = engine._bn_act_state(bn, x.device).bn
+    with torch.no_grad():
+        b.eval_coeffs()
+    y = torch.empty((N, Cout, Ho, Wo), device=x.device, dtype=torch.bfloat16,
+                    memory_format=torch.channels_last)
+    a = nat.StemConvEval()
+    a.conv.N, a.conv.H, a.conv.W, a.conv.Cout = N, H, W, Cout
+    a.conv.x, a.conv.w, a.conv.y = x.data_ptr(), conv.weight.data_ptr(), y.data_ptr()
+    a.scale, a.shift, a.act = b.scale.data_ptr(), b.shift.data_ptr(), engine.act_code_of(act)
+    if not engine.try_launch(nat.lib().yamb_stem_conv_eval_fwd, a, "stem_conv_eval",
+                             2 * N * (H * W * 3 + Ho * Wo * Cout), 2 * N * Ho * Wo * Cout * 27):
+        return None
+    engine.EVAL_TAIL_CALLS += 1
+    return y

@@ -13,7 +13,14 @@ Forward+backward are captured once into a CUDA graph (static input buffers) and 
 arrive through `load(x, target)` which accepts HOST (ideally pinned) or device tensors and copies
 them on a side stream so the H2D copy of step i+1 overlaps the compute of step i (the role of the
 reference's DataPrefetcher, utils/dataflow.py:13-58).
+
+The other half of an epoch, the reference's `validate()` (train.py:273-309), is
+`TrainStep.validate`: `ema_model()` (get_ema_model, common.py:155-172) -> `EvalStep.calibrate`
+(bn_calibration, utils/common.py:175-187) -> `EvalStep.evaluate` (forward_loss, common.py:67-80,
+with the metrics summed on the device).
 """
+import copy
+
 import torch
 import torch.distributed as dist
 
@@ -88,6 +95,8 @@ class TrainStep:
         self.global_step = 0
         self.launches_per_step = None
         self._warm = 0
+        self._ema_model = None
+        self._eval_step = None
 
     # ---- input path ----------------------------------------------------------------------------
     def load(self, x, target):
@@ -158,3 +167,202 @@ class TrainStep:
     def __call__(self, x, target):
         self.load(x, target)
         return self.run()
+
+    # ---- validation ----------------------------------------------------------------------------
+    def ema_model(self):
+        """The model with the EMA weights and EMA running statistics (reference get_ema_model,
+        common.py:155-172).  Built once by `copy.deepcopy` (kernel scratch does not travel, and a
+        copied Parameter has no `_yamb_bf16`, so the copy never reads the live bf16 mirror); later
+        calls refresh the same copy in place, so its addresses, and any graph captured on it,
+        stay valid.  The live model and the optimizer are only read."""
+        if self.ema_decay is None:
+            raise RuntimeError("ema_model: this TrainStep keeps no EMA (ema_decay=0)")
+        if self._ema_model is None:
+            m = copy.deepcopy(self.model)
+            self._ema_pairs = list(zip(m.parameters(), self.model.parameters()))
+            bufs = dict(m.named_buffers())
+            self._ema_stats = [bufs[n] for n, _ in self.model.named_buffers()
+                               if "running_mean" in n or "running_var" in n]
+            self._ema_model = m
+        with torch.no_grad():
+            for q, p in self._ema_pairs:
+                q.copy_(self.opt.ema_shadow(p))
+            for b, s in zip(self._ema_stats, self.stat_shadow):
+                b.copy_(s)
+        return self._ema_model
+
+    def validate(self, val_batches, calib_batches=None, calib_steps=None, calib_batch=None):
+        """The reference's validate() (train.py:273-309): the EMA model, calibrated on
+        `calib_batches` (at most `calib_steps` of them) when given, evaluated on `val_batches`.
+        Returns {'loss', 'top1_error', 'top5_error'} (means over the samples of every rank)."""
+        model = self.ema_model()
+        if self._eval_step is None:
+            self._eval_step = EvalStep(model, self.batch, image_size=self.x.shape[-1],
+                                       calib_batch=calib_batch, use_graph=self.use_graph,
+                                       input_dtype=self.x.dtype)
+        es = self._eval_step
+        if calib_batches is not None:
+            es.calibrate(calib_batches, calib_steps)
+        return es.evaluate(val_batches)
+
+
+def metrics_from_sums(loss_sum, correct1, correct5, count):
+    """The reference's validation results (forward_loss meters averaged over the samples,
+    common.py:67-80) from the sums over every sample of every rank."""
+    n = float(count)
+    if n <= 0:
+        raise ValueError("no samples were evaluated")
+    return {"loss": float(loss_sum) / n, "top1_error": 1.0 - float(correct1) / n,
+            "top5_error": 1.0 - float(correct5) / n}
+
+
+class _Phase:
+    """Static input buffers, staging copies and the captured graph of one EvalStep phase for its
+    full batch shape."""
+
+    def __init__(self, batch, image_size, dtype, dev):
+        self.x = torch.zeros(batch, 3, image_size, image_size, device=dev,
+                             dtype=dtype).contiguous(memory_format=torch.channels_last)
+        self.t = torch.zeros(batch, dtype=torch.long, device=dev)
+        self.x_stage = torch.zeros_like(self.x)
+        self.t_stage = torch.zeros_like(self.t)
+        self.graph = None
+        self.warm = 0
+
+
+class EvalStep:
+    """Evaluation counterpart of TrainStep on the sm_90a path: bn_calibration and the validation
+    pass of the reference (train.py:273-309) over a model that stays where it is (typically
+    `TrainStep.ema_model()`).
+
+    Each phase (calibration, evaluation) captures one CUDA graph for its full batch shape and
+    replays it; a batch of another shape (a partial last batch) runs the same kernels eagerly.
+    Everything weight-dependent (bf16 operands, folded BatchNorm coefficients, the classifier's
+    bf16 bias) is recomputed inside the graph, so in-place weight updates between replays are
+    seen.  A model whose parameters carry an optimizer's bf16 mirror needs that optimizer
+    (`optimizer=`): its `sync_mirror()` runs before every replay.
+
+    Evaluation sums the per-sample loss (fp64) and the correct@1 / correct@5 / sample counts
+    (int64) on the device in batch order; there is no host sync per batch, and one all-reduce
+    SUM at the end when the world is larger than one."""
+
+    def __init__(self, model, per_gpu_batch, image_size=224, calib_batch=None, use_graph=True,
+                 input_dtype=torch.bfloat16, optimizer=None):
+        dev = next(model.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("EvalStep needs the model on a CUDA device (no CPU path)")
+        self.model = model
+        self.dev = dev
+        self.world = udist.get_world_size_fallback()
+        self.optimizer = optimizer
+        self.use_graph = use_graph
+        self.phases = {"eval": _Phase(per_gpu_batch, image_size, input_dtype, dev),
+                       "calib": _Phase(calib_batch or per_gpu_batch, image_size, input_dtype, dev)}
+        self.loss_sum = torch.zeros((), device=dev, dtype=torch.float64)
+        self.counts = torch.zeros(3, device=dev, dtype=torch.int64)   # correct@1, correct@5, samples
+        self.logits = None           # logits of the last evaluated batch (fp32, device)
+        self.copy_stream = torch.cuda.Stream(device=dev)
+        self.copied = torch.cuda.Event()
+        self.consumed = torch.cuda.Event()
+        self.consumed.record()
+
+    # ---- input path (as TrainStep.load) --------------------------------------------------------
+    def load(self, x, target, phase="eval"):
+        """Stage the next full batch of `phase` into its static buffers (async on the copy
+        stream)."""
+        ph = self.phases[phase]
+        with torch.cuda.stream(self.copy_stream):
+            self.copy_stream.wait_event(self.consumed)
+            ph.x_stage.copy_(x, non_blocking=True)
+            ph.t_stage.copy_(target, non_blocking=True)
+            self.copied.record(self.copy_stream)
+
+    def _publish(self, ph):
+        cur = torch.cuda.current_stream()
+        cur.wait_event(self.copied)
+        ph.x.copy_(ph.x_stage)
+        ph.t.copy_(ph.t_stage)
+        self.consumed.record(cur)
+
+    # ---- phase bodies ----------------------------------------------------------------------------
+    def _calib_body(self, x, t):
+        self.model(x)
+
+    def _eval_body(self, x, t):
+        engine.EVAL_TAIL_FUSED = True
+        try:
+            logits = self.model(x)
+        finally:
+            engine.EVAL_TAIL_FUSED = False
+        loss, c1, c5 = tail_ops.softmax_ce(logits, t.to(self.dev), 0.0)
+        self.loss_sum.add_(loss.double().sum())
+        self.counts[0].add_(c1.sum().long())
+        self.counts[1].add_(c5.sum().long())
+        self.counts[2].add_(loss.shape[0])
+        self.logits = logits
+
+    def _run(self, phase, body, x, t):
+        """One batch: a graph replay when it has the phase's full shape, else eagerly."""
+        ph = self.phases[phase]
+        if tuple(x.shape) != tuple(ph.x.shape):
+            body(engine.to_nhwc_bf16(x.to(self.dev, non_blocking=True)), t)
+            return
+        self.load(x, t, phase)
+        self._publish(ph)
+        if self.optimizer is not None:
+            self.optimizer.sync_mirror()
+        if self.use_graph and ph.graph is None and ph.warm >= 1:
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                body(ph.x, ph.t)
+            ph.graph = g
+            ph.logits = self.logits          # the eval graph's static output
+        if ph.graph is not None:
+            ph.graph.replay()
+            if phase == "eval":
+                self.logits = ph.logits
+        else:
+            body(ph.x, ph.t)
+            ph.warm += 1
+
+    # ---- the two phases --------------------------------------------------------------------------
+    @torch.no_grad()
+    def calibrate(self, batches, steps=None):
+        """bn_calibration (reference utils/common.py:175-187, train.py:279-296): reset the
+        running statistics of every nn.BatchNorm2d (ZeroInitBN included), give them momentum None
+        (a cumulative average), put only them in train mode (a non-local InstanceNorm stays in
+        eval mode), run `steps` forwards (all batches when None), all-reduce the statistics when
+        the world is larger than one, and return the model to eval mode."""
+        model = self.model
+        model.eval()
+        for m in model.modules():
+            if isinstance(m, torch.nn.BatchNorm2d):
+                m.reset_running_stats()
+                m.momentum = None
+                m.train()
+        try:
+            for i, (x, t) in enumerate(batches):
+                if steps is not None and i >= steps:
+                    break
+                self._run("calib", self._calib_body, x, t)
+        finally:
+            model.eval()
+        if self.world > 1:
+            udist.allreduce_bn(model)
+
+    @torch.no_grad()
+    def evaluate(self, batches):
+        """Eval pass (reference forward_loss with the plain cross entropy, common.py:67-80):
+        returns {'loss', 'top1_error', 'top5_error'} over every sample of every rank.  The
+        per-rank sums stay in `loss_sum` / `counts`."""
+        self.model.eval()
+        self.loss_sum.zero_()
+        self.counts.zero_()
+        for x, t in batches:
+            self._run("eval", self._eval_body, x, t)
+        if self.world > 1:
+            dist.all_reduce(self.loss_sum)
+            dist.all_reduce(self.counts)
+        c = self.counts.tolist()
+        return metrics_from_sums(float(self.loss_sum), c[0], c[1], c[2])
