@@ -202,6 +202,58 @@ def test_stem_conv(built_lib):
         assert _rel(mod[1].running_var, ref[1].running_var) < 5e-3
 
 
+_STEM_CHILD = r"""
+import ctypes as C, sys
+import torch
+sys.path.insert(0, sys.argv[1])
+from yet_another_mobilenet_series_b200 import native as nat
+
+def stem(cout, fwd):
+    # 64 x 224 x 224: 1792 tiles, more than one resident wave, so the wgrad grid (and with it the
+    # partial slabs and the order of their sum) is the occupancy at this Cout's shared memory
+    g = torch.Generator().manual_seed(cout)
+    N, H, W, Ho, Wo = 64, 224, 224, 112, 112
+    x = torch.randn(N, H, W, 3, generator=g).bfloat16().cuda()
+    w = torch.randn(cout, 3, 3, 3, generator=g).cuda()
+    dh = torch.randn(N, Ho, Wo, cout, generator=g).bfloat16().cuda()
+    y = torch.empty(N, Ho, Wo, cout, dtype=torch.bfloat16, device="cuda")
+    dw = torch.zeros(cout, 3, 3, 3, device="cuda")
+    a = nat.StemConv()
+    a.N, a.H, a.W, a.Cout = N, H, W, cout
+    a.x, a.w, a.y, a.dh, a.dw = x.data_ptr(), w.data_ptr(), y.data_ptr(), dh.data_ptr(), dw.data_ptr()
+    if fwd:
+        nat.check(nat.lib().yamb_stem_conv_fwd(C.byref(a), nat.stream_handle()))
+    nat.check(nat.lib().yamb_stem_conv_wgrad(C.byref(a), nat.stream_handle()))
+    torch.cuda.synchronize()
+    return dw
+
+if sys.argv[3] == "after16":
+    stem(16, True)
+print(stem(int(sys.argv[2]), False).cpu().numpy().tobytes().hex())
+"""
+
+
+# on an H100 the wgrad kernel has 3 CTAs per SM at Cout = 16 and 32 (registers), 2 at Cout = 64
+# (shared memory)
+@pytest.mark.parametrize("cout", [32, 64])
+def test_stem_wgrad_bits_do_not_depend_on_earlier_widths(built_lib, cout):
+    """The stem weight gradient at `cout` in a fresh process, and in one that first ran the stem
+    at Cout = 16: each width's grid comes from its own occupancy, so the bits are the same."""
+    import os
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", _STEM_CHILD, root,
+                                                                           str(cout)]
+    out = {}
+    for order in ("fresh", "after16"):
+        r = subprocess.run(cmd + [order], capture_output=True, text=True, timeout=600)
+        assert r.returncode == 0, r.stderr[-4000:]
+        out[order] = r.stdout.strip().splitlines()[-1]
+    assert len(out["fresh"]) == 2 * 4 * cout * 27
+    assert out["fresh"] == out["after16"]
+
+
 def test_data_prefetcher_surface_and_values(built_lib):
     """DataPrefetcher (reference utils/dataflow.py:13-58): iterator surface, device placement,
     bf16 channels_last conversion, buffer recycling without tearing."""

@@ -4,6 +4,10 @@
 #include <stdarg.h>
 #include <stdio.h>
 
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "host_util.h"
 
 namespace yamb {
@@ -29,6 +33,61 @@ int max_ctas() {
     return cached = -1;
   }
   return cached = sms;
+}
+
+int smem_optin(const char* fn, const void* kern, size_t smem, int* per_sm, int block,
+               bool max_carveout) {
+  struct State {
+    size_t static_smem;
+    int optin;
+    size_t raised;                          // the kernel's dynamic limit on this device, 0: default
+    std::map<std::pair<int, size_t>, int> per_sm;   // (block, smem) -> resident CTAs per SM
+  };
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, State> states;   // (kernel, device)
+  auto fail = [fn](cudaError_t e) {
+    cudaGetLastError();
+    return set_error(YAMB_ECUDA, "%s: %s", fn, cudaGetErrorString(e));
+  };
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return fail(e);
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = states.find({kern, dev});
+  if (it == states.end()) {
+    State s{0, 0, 0, {}};
+    cudaFuncAttributes fa;
+    e = cudaFuncGetAttributes(&fa, kern);
+    if (e == cudaSuccess)
+      e = cudaDeviceGetAttribute(&s.optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (e == cudaSuccess && max_carveout)
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
+                               (int)cudaSharedmemCarveoutMaxShared);
+    if (e != cudaSuccess) return fail(e);
+    s.static_smem = fa.sharedSizeBytes;
+    it = states.emplace(std::make_pair(kern, dev), s).first;
+  }
+  State& s = it->second;
+  const size_t total = s.static_smem + smem;
+  if (total > (size_t)s.optin)
+    return set_error(YAMB_EINVAL, "%s: needs %zu B of shared memory, the device allows %d B", fn,
+                     total, s.optin);
+  if (smem > s.raised && total > 48 * 1024) {
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return fail(e);
+    s.raised = smem;
+  }
+  if (per_sm) {
+    auto o = s.per_sm.find({block, smem});
+    if (o == s.per_sm.end()) {
+      int n = 0;
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, block, smem);
+      if (e != cudaSuccess) return fail(e);
+      o = s.per_sm.emplace(std::make_pair(block, smem), n).first;
+    }
+    *per_sm = o->second;
+  }
+  return 0;
 }
 
 PFN_encodeTiled get_encode_tiled() {

@@ -50,8 +50,6 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <mutex>
-
 #include "host_util.h"
 #include "prims.cuh"
 
@@ -578,22 +576,9 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
     int rc = make_map(&tmW3, a->w_project, 2, dims, str, box);
     if (rc) return rc;
   }
-  // the dynamic-smem limit is process-wide state: only ever raise it
-  static std::mutex mu;
-  static int attr = 0;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    if (attr < smem) {
-      cudaError_t e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN, MODE>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(block_eval_kernel<G, EXPAND, LEAN, MODE>,
-                                 cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 (int)cudaSharedmemCarveoutMaxShared);
-      if (e != cudaSuccess) return set_error(YAMB_ECUDA, "block_eval attr: %s", cudaGetErrorString(e));
-      attr = smem;
-    }
-  }
+  int rc = smem_optin("block_eval", (const void*)block_eval_kernel<G, EXPAND, LEAN, MODE>, smem,
+                      nullptr, 256, /*max_carveout=*/true);
+  if (rc) return rc;
   // One resident CTA per SM: the project accumulators, the stencil and the expand fragments take
   // more than the 128 registers per thread that two CTAs of 256 threads could have.
   const long long cap = (long long)max_ctas();
@@ -612,8 +597,7 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
   // written by exactly one tile; pooled = 0, then += the slabs in slab order (deterministic)
   const int nslab = p.tiles_h * p.tiles_w;
   const long long n_out = (long long)p.N * p.Chid;
-  int rc = det_alloc((size_t)nslab * n_out * sizeof(float), st, &p.part);
-  if (rc) return rc;
+  if ((rc = det_alloc((size_t)nslab * n_out * sizeof(float), st, &p.part))) return rc;
   p.inv_hw = 1.f / ((float)p.Ho * (float)p.Wo);
   cudaError_t e = cudaMemsetAsync(a->pooled, 0, (size_t)n_out * sizeof(float), st);
   if (e == cudaSuccess) {

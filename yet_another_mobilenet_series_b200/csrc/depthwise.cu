@@ -65,23 +65,16 @@ int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
   const int ih = (toh - 1) * s + k, iw = (tow - 1) * s + k;
   const size_t smem = (size_t)ih * iw * ct * sizeof(float) + 2 * (size_t)ct * sizeof(stat_t);
   if (smem > 220 * 1024) return set_error(YAMB_EINVAL, "depthwise fwd: tile too large");
-  cudaError_t e;
-  if (ct <= 16) {
-    e = dw_fwd_dispatch_narrow(p, k, s, ct, tw, smem, st);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "dw fwd launch: %s", cudaGetErrorString(e));
-    return 0;
-  }
+  if (ct <= 16) return dw_fwd_dispatch_narrow(p, k, s, ct, tw, smem, st);
 #define YAMB_FWD_CASE(KK, SS, CC, TT) \
-  if (k == KK && s == SS && ct == CC && tw == TT) e = launch_k(dw_fwd_kernel<KK, SS, CC, TT>, p, smem, p.num_tiles, st)
-  e = cudaErrorInvalidValue;
+  if (k == KK && s == SS && ct == CC && tw == TT) return launch_k(dw_fwd_kernel<KK, SS, CC, TT>, p, smem, p.num_tiles, st)
   YAMB_FWD_CASE(3, 1, 64, 1); YAMB_FWD_CASE(3, 1, 64, 2); YAMB_FWD_CASE(3, 2, 64, 1); YAMB_FWD_CASE(3, 2, 64, 2);
   YAMB_FWD_CASE(3, 1, 32, 1); YAMB_FWD_CASE(3, 1, 32, 2); YAMB_FWD_CASE(3, 2, 32, 1); YAMB_FWD_CASE(3, 2, 32, 2);
   YAMB_FWD_CASE(5, 1, 64, 1); YAMB_FWD_CASE(5, 1, 64, 2); YAMB_FWD_CASE(5, 2, 64, 1); YAMB_FWD_CASE(5, 2, 64, 2);
   YAMB_FWD_CASE(5, 1, 32, 1); YAMB_FWD_CASE(5, 1, 32, 2); YAMB_FWD_CASE(5, 2, 32, 1); YAMB_FWD_CASE(5, 2, 32, 2);
   YAMB_FWD_CASE(7, 1, 64, 1); YAMB_FWD_CASE(7, 2, 64, 1); YAMB_FWD_CASE(7, 1, 32, 1); YAMB_FWD_CASE(7, 2, 32, 1);
 #undef YAMB_FWD_CASE
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "dw fwd launch: %s", cudaGetErrorString(e));
-  return 0;
+  return set_error(YAMB_ECUDA, "dw fwd launch: no kernel for k=%d stride=%d ct=%d tw=%d", k, s, ct, tw);
 }
 
 int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
@@ -128,8 +121,7 @@ int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
       ((size_t)(2 * rh * rw + tih * tiw) * ct + (size_t)(7 + 2 * k * k) * ct) * sizeof(float) +
       2 * (size_t)ct * sizeof(stat_t);
   if (smem > 220 * 1024) return set_error(YAMB_EINVAL, "depthwise bwd: slice too wide for smem");
-  cudaError_t e;
-  if (ct <= 16) e = dw_bwd_dispatch_narrow(p, k, s, ct, smem, st);
+  if (ct <= 16) rc = dw_bwd_dispatch_narrow(p, k, s, ct, smem, st);
   else if (k == 3 && s == 1 && ct == 64) YAMB_DW_BWD(3, 1, 64, p, smem, p.num_tiles, st);
   else if (k == 3 && s == 2 && ct == 64) YAMB_DW_BWD(3, 2, 64, p, smem, p.num_tiles, st);
   else if (k == 3 && s == 1) YAMB_DW_BWD(3, 1, 32, p, smem, p.num_tiles, st);
@@ -142,8 +134,7 @@ int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
   else if (k == 7 && s == 2 && ct == 64) YAMB_DW_BWD(7, 2, 64, p, smem, p.num_tiles, st);
   else if (k == 7 && s == 1) YAMB_DW_BWD(7, 1, 32, p, smem, p.num_tiles, st);
   else YAMB_DW_BWD(7, 2, 32, p, smem, p.num_tiles, st);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "dw bwd launch: %s", cudaGetErrorString(e));
-  return 0;
+  return rc;
 }
 
 }  // namespace yamb

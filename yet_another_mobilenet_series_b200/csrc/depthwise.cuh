@@ -25,8 +25,6 @@
 #include <stdlib.h>
 #include <cuda_runtime.h>
 
-#include <mutex>
-
 #include "bn_finalize.cuh"
 #include "host_util.h"
 #include "prims.cuh"
@@ -748,34 +746,12 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_
 
 // Grid of kernel `kern` for `tiles` tiles at `smem` bytes of dynamic shared memory.
 template <typename Kern, typename Dev>
-static cudaError_t grid_k(Kern kern, const Dev& p, size_t smem, long long tiles, int* grid_out) {
-  // The dynamic-smem limit of a kernel is process-wide state: only ever RAISE it (forward and
-  // backward run on different host threads); occupancy is cached per (kernel, smem size).
-  struct Ent { const void* k; size_t smem; int per_sm; };
-  static Ent cache[128];
-  static int n_cache = 0;
-  static std::mutex mu;
+static int grid_k(const char* fn, Kern kern, const Dev& p, size_t smem, long long tiles,
+                  int* grid_out) {
   int per_sm = 0;
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    size_t limit = 0;
-    for (int i = 0; i < n_cache; ++i)
-      if (cache[i].k == (const void*)kern) {
-        if (cache[i].smem > limit) limit = cache[i].smem;
-        if (cache[i].smem == smem) per_sm = cache[i].per_sm;
-      }
-    if (per_sm == 0) {
-      cudaError_t e;
-      if (smem > limit) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-      }
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, smem);
-      if (e != cudaSuccess) return e;
-      if (per_sm < 1) return cudaErrorLaunchOutOfResources;
-      if (n_cache < 128) cache[n_cache++] = Ent{(const void*)kern, smem, per_sm};
-    }
-  }
+  int rc = smem_optin(fn, (const void*)kern, smem, &per_sm);
+  if (rc) return rc;
+  if (per_sm < 1) return set_error(YAMB_ECUDA, "%s: no CTA fits on an SM", fn);
   long long cap = (long long)max_ctas() * (per_sm > 4 ? 4 : per_sm);  // partials sized for 4/SM
   int grid = (int)(tiles < cap ? tiles : cap);
   // Tiles are ordered channel-chunk-major and every CTA walks a contiguous range.  With a grid that
@@ -786,33 +762,36 @@ static cudaError_t grid_k(Kern kern, const Dev& p, size_t smem, long long tiles,
   if (p.chunks > 1 && grid > p.chunks) grid = grid / p.chunks * p.chunks;
   if (grid < 1) grid = 1;
   *grid_out = grid;
-  return cudaSuccess;
+  return 0;
 }
 
+// The launchers below return 0 or a YAMB_* code with the message set.
 template <typename Kern, typename Dev>
-static cudaError_t launch_k(Kern kern, const Dev& p, size_t smem, long long tiles, cudaStream_t st) {
+static int launch_k(Kern kern, const Dev& p, size_t smem, long long tiles, cudaStream_t st) {
   int grid = 0;
-  cudaError_t e = grid_k(kern, p, smem, tiles, &grid);
-  if (e != cudaSuccess) return e;
+  int rc = grid_k("dw fwd launch", kern, p, smem, tiles, &grid);
+  if (rc) return rc;
   kern<<<grid, 256, smem, st>>>(p);
-  return cudaGetLastError();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "dw fwd launch: %s", cudaGetErrorString(e));
+  return 0;
 }
 
 template <int KK, int SS, int CC, typename Dev>
-static cudaError_t launch_bwd(const Dev& p0, size_t smem, long long tiles, cudaStream_t st) {
+static int launch_bwd(const Dev& p0, size_t smem, long long tiles, cudaStream_t st) {
   // weight gradient: per-CTA partials (zero where a CTA has no tile of a channel chunk), then
   // added in CTA order
   auto k0 = dw_bwd_kernel<KK, SS, CC, 0, (KK == 7 ? 25 : KK * KK), true>;
   int g0 = 0, g1 = 0;
-  cudaError_t e = grid_k(k0, p0, smem, tiles, &g0);
+  int rc = grid_k("dw bwd launch", k0, p0, smem, tiles, &g0);
   if constexpr (KK == 7)   // the taps past 25 in a second kernel
-    if (e == cudaSuccess) e = grid_k(dw_bwd_kernel<KK, SS, CC, 25, KK * KK, false>, p0, smem, tiles, &g1);
-  if (e != cudaSuccess) return e;
+    if (!rc) rc = grid_k("dw bwd launch", dw_bwd_kernel<KK, SS, CC, 25, KK * KK, false>, p0, smem, tiles, &g1);
+  if (rc) return rc;
   const int slabs = g0 > g1 ? g0 : g1;
   const long long n = (long long)p0.C * KK * KK;
   Dev p = p0;
-  if (det_alloc((size_t)(slabs * n) * sizeof(float), st, &p.part)) return cudaErrorMemoryAllocation;
-  e = cudaMemsetAsync(p.part, 0, (size_t)(slabs * n) * sizeof(float), st);
+  if ((rc = det_alloc((size_t)(slabs * n) * sizeof(float), st, &p.part))) return rc;
+  cudaError_t e = cudaMemsetAsync(p.part, 0, (size_t)(slabs * n) * sizeof(float), st);
   if (e == cudaSuccess) {
     k0<<<g0, 256, smem, st>>>(p);
     e = cudaGetLastError();
@@ -825,18 +804,16 @@ static cudaError_t launch_bwd(const Dev& p0, size_t smem, long long tiles, cudaS
   }
   if (e != cudaSuccess) {
     det_free(p.part, st);
-    return e;
+    return set_error(YAMB_ECUDA, "dw bwd launch: %s", cudaGetErrorString(e));
   }
-  if (det_reduce_launch(p.part, slabs, n, p.dw, st)) return cudaErrorLaunchFailure;
-  return cudaSuccess;
+  return det_reduce_launch(p.part, slabs, n, p.dw, st);
 }
-#define YAMB_DW_BWD(KK, SS, CC, ...) e = launch_bwd<KK, SS, CC>(__VA_ARGS__)
+#define YAMB_DW_BWD(KK, SS, CC, ...) rc = launch_bwd<KK, SS, CC>(__VA_ARGS__)
 
 
-// 8 / 16-channel tiles (depthwise_narrow.cu); cudaErrorInvalidValue when the combination is not built
-cudaError_t dw_fwd_dispatch_narrow(const DwFwdDev& p, int k, int s, int ct, int tw, size_t smem,
-                                   cudaStream_t st);
-cudaError_t dw_bwd_dispatch_narrow(const DwBwdDev& p, int k, int s, int ct, size_t smem,
-                                   cudaStream_t st);
+// 8 / 16-channel tiles (depthwise_narrow.cu); YAMB_ECUDA when the combination is not built
+int dw_fwd_dispatch_narrow(const DwFwdDev& p, int k, int s, int ct, int tw, size_t smem,
+                           cudaStream_t st);
+int dw_bwd_dispatch_narrow(const DwBwdDev& p, int k, int s, int ct, size_t smem, cudaStream_t st);
 
 }  // namespace yamb

@@ -8,8 +8,6 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
-#include <mutex>
-
 #include "bn_finalize.cuh"
 #include "host_util.h"
 #include "prims.cuh"
@@ -520,41 +518,8 @@ static int check_bf16(const char* fn, const char* name, const void* p, int ld, i
 }
 
 // bn_stats, bn_reduce and se_bwd_apply take 2*C doubles of dynamic shared memory (the CTA's
-// statistics slots) on top of cta_stats_merge's static staging.  Past the 48 KiB default (C >= 1984)
-// the kernel has to opt in; the limit is per device, so it is raised (never lowered) per device.
-// A C whose total exceeds the device's opt-in maximum is refused.
-enum { kStatsKernels = 3, kStatsDevices = 64 };
-static int stats_smem(int which, const void* kern, const char* fn, int C, size_t* smem_out) {
-  struct Ent { size_t static_smem; int optin; size_t raised; bool init; };
-  static Ent cache[kStatsKernels][kStatsDevices];
-  static std::mutex mu;
-  const size_t smem = 2 * (size_t)C * sizeof(stat_t);
-  *smem_out = smem;
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "%s: %s", fn, cudaGetErrorString(e));
-  std::lock_guard<std::mutex> lock(mu);
-  Ent spare = Ent{0, 0, 0, false};
-  Ent& c = dev < kStatsDevices ? cache[which][dev] : spare;
-  if (!c.init) {
-    cudaFuncAttributes fa;
-    e = cudaFuncGetAttributes(&fa, kern);
-    if (e == cudaSuccess)
-      e = cudaDeviceGetAttribute(&c.optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "%s: %s", fn, cudaGetErrorString(e));
-    c.static_smem = fa.sharedSizeBytes;
-    c.init = true;
-  }
-  if (c.static_smem + smem > (size_t)c.optin)
-    return set_error(YAMB_EINVAL, "%s: C = %d needs %zu B of shared memory, the device allows %d B",
-                     fn, C, c.static_smem + smem, c.optin);
-  if (smem > c.raised && c.static_smem + smem > 48 * 1024) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "%s attr: %s", fn, cudaGetErrorString(e));
-    c.raised = smem;
-  }
-  return 0;
-}
+// statistics slots) on top of cta_stats_merge's static staging: from C = 1984 on they opt in.
+static size_t stats_smem(int C) { return 2 * (size_t)C * sizeof(stat_t); }
 
 int bn_apply_launch(const yamb_bn_apply* a, cudaStream_t st) {
   if (!a || a->M <= 0 || a->C <= 0 || (a->C % 8)) return set_error(YAMB_EINVAL, "bn_apply shape");
@@ -596,8 +561,8 @@ int bn_reduce_launch(const yamb_bn_reduce* a, cudaStream_t st) {
   p.M = a->M; p.C = a->C; p.lddy = a->lddy; p.ldh = a->ldh;
   p.dy = (const __nv_bfloat16*)a->dy; p.h = (const __nv_bfloat16*)a->h; p.bn = *a->bn;
   p.z_scale = a->z_scale; p.z_shift = a->z_scale ? a->z_shift : nullptr; p.z_act = a->z_act;
-  size_t smem;
-  if ((rc = stats_smem(0, (const void*)bn_reduce_kernel, "bn_reduce", a->C, &smem))) return rc;
+  const size_t smem = stats_smem(a->C);
+  if ((rc = smem_optin("bn_reduce", (const void*)bn_reduce_kernel, smem))) return rc;
   const int CG = a->C / 8;
   const int PX = 256 / CG > 0 ? 256 / CG : 1;
   long long want = (a->M + PX - 1) / PX;
@@ -617,8 +582,8 @@ int bn_stats_launch(const yamb_bn_stats* a, cudaStream_t st) {
   BnStatsDev p;
   p.M = a->M; p.C = a->C; p.ldh = a->ldh;
   p.h = (const __nv_bfloat16*)a->h; p.bn = *a->bn;
-  size_t smem;
-  if ((rc = stats_smem(1, (const void*)bn_stats_kernel, "bn_stats", a->C, &smem))) return rc;
+  const size_t smem = stats_smem(a->C);
+  if ((rc = smem_optin("bn_stats", (const void*)bn_stats_kernel, smem))) return rc;
   const int CG = a->C / 8;
   const int PX = 256 / CG > 0 ? 256 / CG : 1;
   long long want = (a->M + PX - 1) / PX;
@@ -762,8 +727,8 @@ int se_bwd_apply_launch(const yamb_se_bwd_apply* a, cudaStream_t st) {
   p.scale = a->scale; p.shift = a->shift; p.act = a->act;
   p.gate = a->gate; p.dpool = a->dpool; p.ldg = ldg;
   p.dz = (__nv_bfloat16*)a->dz; p.bn = *a->bn;
-  size_t smem;
-  if ((rc = stats_smem(2, (const void*)se_bwd_apply_kernel, "se_bwd_apply", a->C, &smem))) return rc;
+  const size_t smem = stats_smem(a->C);
+  if ((rc = smem_optin("se_bwd_apply", (const void*)se_bwd_apply_kernel, smem))) return rc;
   const int CG = a->C / 8;
   const int PX = 256 / CG > 0 ? 256 / CG : 1;
   long long want = (a->M + PX - 1) / PX;

@@ -983,24 +983,19 @@ static int pick_block_n(int N, bool b_mn) {
   return N <= 16 ? 16 : 32;
 }
 
-// Launch of one instantiation.  The dynamic shared-memory limit of a kernel is process-wide: one
-// counter per instantiation, the limit is only ever raised.
-using LaunchFn = cudaError_t (*)(int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&,
-                                 const CUtensorMap&, const CUtensorMap&, const CUtensorMap&,
-                                 const GemmDev&);
+// Launch of one instantiation: 0 or a YAMB_* code with the message set.
+using LaunchFn = int (*)(int, int, cudaStream_t, const CUtensorMap&, const CUtensorMap&,
+                         const CUtensorMap&, const CUtensorMap&, const CUtensorMap&, const GemmDev&);
 template <bool XF, int EP, int BN, int AMN, int BMN>
-static cudaError_t launch_tc(int grid, int smem, cudaStream_t stream, const CUtensorMap& tmA,
-                             const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
-                             const CUtensorMap& tmD, const GemmDev& p) {
-  static int attr_smem = 0;
-  if (attr_smem < smem) {
-    const cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<XF, EP, BN, AMN, BMN>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_smem = smem;
-  }
+static int launch_tc(int grid, int smem, cudaStream_t stream, const CUtensorMap& tmA,
+                     const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
+                     const CUtensorMap& tmD, const GemmDev& p) {
+  int rc = smem_optin("gemm launch", (const void*)gemm_tc_kernel<XF, EP, BN, AMN, BMN>, smem);
+  if (rc) return rc;
   gemm_tc_kernel<XF, EP, BN, AMN, BMN><<<grid, 512, smem, stream>>>(tmA, tmB, tmA2, tmB2, tmD, p);
-  return cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "gemm launch: %s", cudaGetErrorString(e));
+  return 0;
 }
 template <int EP, int BN, int AMN, int BMN>
 static LaunchFn pick_tc(bool xf) {
@@ -1221,8 +1216,10 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
     if (p.part) det_free(p.part, stream);
     return set_error(YAMB_ECUDA, "%s: %s", what, cudaGetErrorString(err));
   };
-  e = fn(grid, smem_total, stream, tmA, tmB, tmA2, tmB2, tmD, p);
-  if (e != cudaSuccess) return fail("gemm launch", e);
+  if ((rc = fn(grid, smem_total, stream, tmA, tmB, tmA2, tmB2, tmD, p))) {
+    if (p.part) det_free(p.part, stream);
+    return rc;
+  }
   if (a->epi == 2) {
     const long long total = (long long)a->M * a->N;
     const long long cap = 4LL * dev_ctas, blocks = (total + 255) / 256;

@@ -163,16 +163,10 @@ int head_pool_eval_launch(const yamb_head_pool_eval* a, cudaStream_t st) {
   p.inv_hw = 1.f / (float)a->HW;
   p.pooled = (__nv_bfloat16*)a->pooled;
   const size_t smem = 1024 + (size_t)2 * p.kpanels * 8192 + 4 * 64 * sizeof(float);
-  static size_t attr = 0;   // process-wide: only ever raise the limit
-  cudaError_t e;
-  if (smem > attr) {
-    e = cudaFuncSetAttribute(head_pool_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "head pool eval attr: %s", cudaGetErrorString(e));
-    attr = smem;
-  }
+  const int rc = smem_optin("head pool eval", (const void*)head_pool_eval_kernel, smem);
+  if (rc) return rc;
   head_pool_eval_kernel<<<dim3(a->N, (a->Cout + 63) / 64), 128, smem, st>>>(p);
-  e = cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "head pool eval: %s", cudaGetErrorString(e));
   return 0;
 }

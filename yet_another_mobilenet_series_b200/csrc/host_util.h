@@ -10,6 +10,16 @@ namespace yamb {
 int set_error(int code, const char* fmt, ...);
 int max_ctas();  // SM count of the current device, <= 0 without a device
 
+// Dynamic shared memory for a launch of `kern` with `smem` bytes on the current device.  Refuses
+// (YAMB_EINVAL, "`fn`: ... shared memory ...") when the kernel's static shared memory plus `smem`
+// exceeds the device's opt-in maximum; past the 48 KiB default it raises the kernel's limit on this
+// device, which is never lowered.  With `per_sm` it also returns the CTAs of `block` threads that
+// are resident per SM at `smem`.  `max_carveout` asks for the largest shared-memory carveout (it
+// shrinks the L1).  The state is per (kernel, device), under one lock: forward and backward
+// launch from different host threads.  0 or a YAMB_* code with the message set.
+int smem_optin(const char* fn, const void* kern, size_t smem, int* per_sm = nullptr,
+               int block = 256, bool max_carveout = false);
+
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                     const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,

@@ -201,18 +201,12 @@ int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t st) {
   p.rows_per_cta = R;
   const size_t smem = (size_t)R * (I2 + a->J) * 2;
   if (smem > 200 * 1024) return set_error(YAMB_EINVAL, "nl_gram: rows too wide for shared memory");
-  cudaError_t e;
-  static size_t attr = 0;   // process-wide: only ever raise the limit
-  if (smem > attr) {
-    e = cudaFuncSetAttribute(nl_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "nl_gram attr: %s", cudaGetErrorString(e));
-    attr = smem;
-  }
+  if ((rc = smem_optin("nl_gram", (const void*)nl_gram_kernel, smem))) return rc;
   dim3 grid((rows + R - 1) / R, a->N);
   p.part = a->G;
   if (grid.x > 1 && (rc = det_alloc((size_t)grid.x * n_out * sizeof(float), st, &p.part))) return rc;
   nl_gram_kernel<<<grid, 256, smem, st>>>(p);
-  e = cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     if (p.part != a->G) det_free(p.part, st);
     return set_error(YAMB_ECUDA, "nl_gram: %s", cudaGetErrorString(e));
@@ -247,16 +241,10 @@ int nl_rowmat_launch(const yamb_nl_rowmat* a, cudaStream_t st) {
   p.rows_per_cta = R;
   const size_t smem = (size_t)a->K * a->O * 4 + (size_t)R * K2 * 2;
   if (smem > 220 * 1024) return set_error(YAMB_EINVAL, "nl_rowmat: %d x %d matrix exceeds shared memory", a->K, a->O);
-  static size_t attr = 0;   // process-wide: only ever raise the limit
-  cudaError_t e;
-  if (smem > attr) {
-    e = cudaFuncSetAttribute(nl_rowmat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "nl_rowmat attr: %s", cudaGetErrorString(e));
-    attr = smem;
-  }
+  if ((rc = smem_optin("nl_rowmat", (const void*)nl_rowmat_kernel, smem))) return rc;
   dim3 grid((rows + R - 1) / R, a->N);
   nl_rowmat_kernel<<<grid, 256, smem, st>>>(p);
-  e = cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "nl_rowmat: %s", cudaGetErrorString(e));
   return 0;
 }

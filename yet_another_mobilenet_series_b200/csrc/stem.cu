@@ -304,20 +304,12 @@ template <bool EVAL>
 static int stem_fwd_run(const StemDev& p, int Cout, cudaStream_t st) {
   const size_t smem = 27 * 64 * 4 + (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
                       (size_t)8 * 64 * (Cout / 8) * 16;
-  static size_t attr_f = 0;   // process-wide: only ever raise the limit
-  cudaError_t e;
-  if (smem > attr_f) {
-    e = cudaFuncSetAttribute(stem_fwd_kernel<EVAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem fwd attr: %s", cudaGetErrorString(e));
-    attr_f = smem;
-  }
-  static int per_sm_f = 0;
-  if (per_sm_f == 0 &&
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_f, stem_fwd_kernel<EVAL>, 256, smem) != cudaSuccess)
-    per_sm_f = 2;
-  const int res_f = max_ctas() * (per_sm_f > 0 ? per_sm_f : 1);   // one resident wave: no tail
+  int per_sm = 0;
+  const int rc = smem_optin("stem conv fwd", (const void*)stem_fwd_kernel<EVAL>, smem, &per_sm);
+  if (rc) return rc;
+  const int res_f = max_ctas() * (per_sm > 0 ? per_sm : 1);   // one resident wave: no tail
   stem_fwd_kernel<EVAL><<<p.num_tiles < res_f ? p.num_tiles : res_f, 256, smem, st>>>(p);
-  e = cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv fwd: %s", cudaGetErrorString(e));
   return 0;
 }
@@ -358,19 +350,11 @@ int stem_conv_wgrad_launch(const yamb_stem_conv* a, cudaStream_t st) {
   if (256 % (a->Cout / 8 * 8)) return set_error(YAMB_EINVAL, "stem conv wgrad: Cout must be 8, 16, 32 or 64");
   const size_t smem = (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
                       (size_t)kStemTH * kStemTW * a->Cout * 2;
-  static size_t attr = 0;   // process-wide: only ever raise the limit
-  cudaError_t e;
-  if (smem > attr) {
-    e = cudaFuncSetAttribute(stem_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem wgrad attr: %s", cudaGetErrorString(e));
-    attr = smem;
-  }
-  const int cap = 4 * max_ctas();
-  static int per_sm_w = 0;
-  if (per_sm_w == 0 &&
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_w, stem_wgrad_kernel, 256, smem) != cudaSuccess)
-    per_sm_w = 2;
-  const int res_w = max_ctas() * (per_sm_w > 0 ? per_sm_w : 1);
+  // the grid sets the number of partial slabs and so the order of their sum: it comes from the
+  // occupancy at this Cout's shared memory
+  int per_sm = 0;
+  if ((rc = smem_optin("stem conv wgrad", (const void*)stem_wgrad_kernel, smem, &per_sm))) return rc;
+  const int res_w = max_ctas() * (per_sm > 0 ? per_sm : 1);
   const int grid = p.num_tiles < res_w ? p.num_tiles : res_w;
   const int slots = grid * (256 / p.Cout);
   rc = det_alloc((size_t)slots * p.Cout * 27 * sizeof(float), st, &p.part);
@@ -378,7 +362,7 @@ int stem_conv_wgrad_launch(const yamb_stem_conv* a, cudaStream_t st) {
   stem_wgrad_kernel<<<grid, 256, smem, st>>>(p);
   if (cudaPeekAtLastError() != cudaSuccess) det_free(p.part, st);
   else if ((rc = det_reduce_launch(p.part, slots, (long long)p.Cout * 27, p.dw, st)) != 0) return rc;
-  e = cudaGetLastError();
+  const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv wgrad: %s", cudaGetErrorString(e));
   return 0;
 }
