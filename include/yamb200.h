@@ -130,6 +130,23 @@ typedef struct yamb_gemm {
 
 int yamb_pointwise_gemm(const yamb_gemm* args, yamb_stream_t stream);
 
+/* The launch plan yamb_pointwise_gemm makes for `args`, computed on the host without a launch:
+ * the same argument checks (codes and messages) up to the shared-memory layout; pointers and their
+ * alignment are not checked.  num_sms > 0 plans for that many SMs and needs no device; <= 0 uses
+ * the current device (YAMB_ENODEV without one). */
+typedef struct yamb_gemm_plan_info {
+  int32_t xf, epi, block_n, a_mn, b_mn;  /* the gemm_tc_kernel instantiation */
+  int32_t m_blocks, n_blocks, num_k_blocks, ksplit, kb_per_split, num_work, grid;
+  int32_t a_tma, b_tma;                  /* transformed operand loaded by TMA (else registers) */
+  int32_t wg2x;                          /* warps 8-11 load instead of running epilogues */
+  int32_t lgroup;                        /* loader warps per pipeline stage */
+  int32_t num_stages, out_bufs, smem_bytes;
+  int32_t reg_stats;                     /* BatchNorm column sums held in registers to the end */
+  int32_t simple_work;                   /* one work item = one m-block (ksplit 1, one n-block) */
+} yamb_gemm_plan_info;
+
+int yamb_gemm_plan(const yamb_gemm* args, int32_t num_sms, yamb_gemm_plan_info* out);
+
 /* ---- depthwise k x k convolution (k in {3,5,7}, stride 1/2, pad (k-1)/2) -------------------------
  * Replaces nn.Conv2d(groups=C)+BatchNorm2d+activation of ConvBNReLU
  * (reference: models/mobilenet_base.py:405-411 unfused, :275-281 fused, :181-203 ConvBNReLU).
@@ -525,7 +542,7 @@ int yamb_max_ctas(void);
  * 6 bn_reduce, 7 se_pool, 8 rmsprop, 9 se_bwd_reduce, 10 se_bwd_apply, 11 bn_stats,
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
  * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
- * 25 stem_conv_eval, 26 head_pool_eval) so bindings can self-check */
+ * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

@@ -47,7 +47,7 @@ from dw_cases import CASES, WALK_CASES
 
 pytestmark = pytest.mark.gpu
 
-from gpu_probe_gemm import _act, _act_grad  # noqa: E402
+from ref64 import _act, _act_grad  # noqa: E402
 
 SENTINEL = -1536.0       # a bf16 value no output of these tests takes
 BAND = 2.0 ** -16        # relative distance of an intrinsic activation from the exact one

@@ -138,12 +138,16 @@ int yamb_struct_size(int which) {
     case 24: return (int)sizeof(yamb_sgd);
     case 25: return (int)sizeof(yamb_stem_conv_eval);
     case 26: return (int)sizeof(yamb_head_pool_eval);
+    case 27: return (int)sizeof(yamb_gemm_plan_info);
     default: return -1;
   }
 }
 
 int yamb_pointwise_gemm(const yamb_gemm* args, yamb_stream_t stream) {
   return yamb::gemm_launch(args, reinterpret_cast<cudaStream_t>(stream));
+}
+int yamb_gemm_plan(const yamb_gemm* args, int32_t num_sms, yamb_gemm_plan_info* out) {
+  return yamb::gemm_plan_query(args, num_sms, out);
 }
 
 

@@ -1002,16 +1002,28 @@ static LaunchFn pick_tc(bool xf) {
   return xf ? &launch_tc<true, EP, BN, AMN, BMN> : &launch_tc<false, EP, BN, AMN, BMN>;
 }
 
-int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
+// What a launch decides before it looks at a pointer: the argument checks, the tile grid and
+// split-K, the warp roles, the shared-memory layout and the kernel instantiation.
+struct GemmPlan {
+  GemmDev p;
+  LaunchFn fn;
+  int xf;          // XF of the instantiation fn launches
+  int sms;         // SM count planned for
+  int grid;
+  int smem_total;
+};
+
+// 0 or a YAMB_* code with the message set.  num_sms <= 0: the current device's SM count.
+static int gemm_plan(const yamb_gemm* a, int num_sms, GemmPlan& pl) {
   if (!a || a->M <= 0 || a->N <= 0 || a->K <= 0) return set_error(YAMB_EINVAL, "bad GEMM shape");
   if ((a->N % 8) || (a->a_mn_major ? (a->M % 8) : (a->K % 8)) || (a->b_mn_major ? 0 : (a->K % 8)))
     return set_error(YAMB_EINVAL, "GEMM channel dims must be multiples of 8 (M=%d N=%d K=%d)",
                      a->M, a->N, a->K);
   if (a->epi < 0 || a->epi > 2) return set_error(YAMB_EINVAL, "bad epilogue");
-  int dev_ctas = max_ctas();
+  const int dev_ctas = num_sms > 0 ? num_sms : max_ctas();
   if (dev_ctas <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
 
-  GemmDev p;
+  GemmDev& p = pl.p;
   memset(&p, 0, sizeof(p));
   p.M = a->M; p.N = a->N; p.K = a->K;
   p.a_mn = a->a_mn_major ? 1 : 0;
@@ -1033,12 +1045,6 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   static const int env_dbg = [] { const char* d = getenv("YAMB_GEMM_DEBUG"); return d ? atoi(d) : 0; }();
   p.dbg = env_dbg;
   p.dbg_buf = nullptr;
-  if (p.dbg & 512) {
-    static unsigned long long* dbuf = nullptr;
-    if (!dbuf) cudaMalloc(&dbuf, 16 * sizeof(unsigned long long));
-    cudaMemsetAsync(dbuf, 0, 16 * sizeof(unsigned long long), stream);
-    p.dbg_buf = dbuf;
-  }
   // transform-heavy / epilogue-light launches give warps 8-11 to the transform
   // warps 8-11 load/transform instead of running a second epilogue warpgroup when the epilogue
   // is light relative to the operand work: split-K wgrad (no store at all) or a forward/dgrad
@@ -1142,14 +1148,65 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   p.off_coef = off; off += (coef_bytes + 15) & ~15;
   p.off_stats = off; off += (stats_bytes + 15) & ~15;
   p.off_bars = (off + 15) & ~15; off = p.off_bars + (int)sizeof(Bars);
-  const int smem_total = off;  // the extern array is declared 1024-aligned: no slack needed
+  pl.smem_total = off;  // the extern array is declared 1024-aligned: no slack needed
+
+  // the operand layouts the layers produce (an MN-major B always has block_n 64)
+  LaunchFn fn = nullptr;
+  if (a->epi == 0 && !p.a_mn && !p.b_mn)   // forward
+    fn = p.block_n == 64 ? pick_tc<0, 64, 0, 0>(xf) : p.block_n == 32 ? pick_tc<0, 32, 0, 0>(xf)
+                                                                      : pick_tc<0, 16, 0, 0>(xf);
+  else if (a->epi == 0 && !p.a_mn)         // dgrad (+ residual)
+    fn = pick_tc<0, 64, 0, 1>(xf);
+  else if (a->epi == 1 && !p.a_mn && p.b_mn)   // dgrad + dz: plain A (dh3) or two-source A, one
+    fn = &launch_tc<true, 1, 64, 0, 1>;        // variant (XF = false spills 68 B at 128 registers)
+  else if (a->epi == 2 && p.a_mn && p.b_mn)    // wgrad
+    fn = pick_tc<2, 64, 1, 1>(xf);
+  if (!fn)
+    return set_error(YAMB_EINVAL, "GEMM operand layout not supported (epi %d, A %s, B %s)", a->epi,
+                     p.a_mn ? "MN-major" : "K-major", p.b_mn ? "MN-major" : "K-major");
+  pl.fn = fn;
+  pl.xf = (a->epi == 1 || xf) ? 1 : 0;
+  pl.sms = dev_ctas;
+  pl.grid = p.num_work < ctas ? p.num_work : ctas;
+  return 0;
+}
+
+int gemm_plan_query(const yamb_gemm* a, int num_sms, yamb_gemm_plan_info* out) {
+  if (!out) return set_error(YAMB_EINVAL, "no plan output");
+  GemmPlan pl;
+  const int rc = gemm_plan(a, num_sms, pl);
+  if (rc) return rc;
+  const GemmDev& p = pl.p;
+  memset(out, 0, sizeof(*out));
+  out->xf = pl.xf; out->epi = p.epi; out->block_n = p.block_n; out->a_mn = p.a_mn; out->b_mn = p.b_mn;
+  out->m_blocks = p.m_blocks; out->n_blocks = p.n_blocks; out->num_k_blocks = p.num_k_blocks;
+  out->ksplit = p.ksplit; out->kb_per_split = p.kb_per_split; out->num_work = p.num_work;
+  out->grid = pl.grid;
+  out->a_tma = p.a_tma; out->b_tma = p.b_tma; out->wg2x = p.wg2x; out->lgroup = p.lgroup;
+  out->num_stages = p.num_stages; out->out_bufs = p.out_bufs; out->smem_bytes = pl.smem_total;
+  // the kernel's own rules (consumer warps, loader warps)
+  out->reg_stats = (p.has_bnf || p.has_bnb) && p.n_blocks == 1;
+  out->simple_work = p.ksplit == 1 && p.n_blocks == 1;
+  return 0;
+}
+
+int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
+  GemmPlan pl;
+  int rc = gemm_plan(a, 0, pl);
+  if (rc) return rc;
+  GemmDev& p = pl.p;
+  if (p.dbg & 512) {
+    static unsigned long long* dbuf = nullptr;
+    if (!dbuf) cudaMalloc(&dbuf, 16 * sizeof(unsigned long long));
+    cudaMemsetAsync(dbuf, 0, 16 * sizeof(unsigned long long), stream);
+    p.dbg_buf = dbuf;
+  }
 
   // ---- tensor maps ----
   CUtensorMap tmA, tmB, tmA2, tmB2, tmD;
   memset(&tmA, 0, sizeof(tmA)); memset(&tmB, 0, sizeof(tmB));
   memset(&tmA2, 0, sizeof(tmA2)); memset(&tmB2, 0, sizeof(tmB2));
   memset(&tmD, 0, sizeof(tmD));
-  int rc;
   if (p.a_tma) {
     if (!p.a_mn) rc = make_map_2d(&tmA, a->A, a->K, a->M, a->lda, 64, 128);
     else rc = make_map_2d(&tmA, a->A, a->M, a->K, a->lda, 64, 64);
@@ -1192,21 +1249,6 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   if (p.side && ((reinterpret_cast<uintptr_t>(p.side) & 15) || (p.lds % 8)))
     return set_error(YAMB_EINVAL, "side operand must be 16-byte aligned with lds % 8 == 0");
 
-  // the operand layouts the layers produce (an MN-major B always has block_n 64)
-  LaunchFn fn = nullptr;
-  if (a->epi == 0 && !p.a_mn && !p.b_mn)   // forward
-    fn = p.block_n == 64 ? pick_tc<0, 64, 0, 0>(xf) : p.block_n == 32 ? pick_tc<0, 32, 0, 0>(xf)
-                                                                      : pick_tc<0, 16, 0, 0>(xf);
-  else if (a->epi == 0 && !p.a_mn)         // dgrad (+ residual)
-    fn = pick_tc<0, 64, 0, 1>(xf);
-  else if (a->epi == 1 && !p.a_mn && p.b_mn)   // dgrad + dz: plain A (dh3) or two-source A, one
-    fn = &launch_tc<true, 1, 64, 0, 1>;        // variant (XF = false spills 68 B at 128 registers)
-  else if (a->epi == 2 && p.a_mn && p.b_mn)    // wgrad
-    fn = pick_tc<2, 64, 1, 1>(xf);
-  if (!fn)
-    return set_error(YAMB_EINVAL, "GEMM operand layout not supported (epi %d, A %s, B %s)", a->epi,
-                     p.a_mn ? "MN-major" : "K-major", p.b_mn ? "MN-major" : "K-major");
-  const int grid = p.num_work < ctas ? p.num_work : ctas;
   cudaError_t e;
   if (a->epi == 2) {   // split-K partial tiles: released by the reduction below, on this stream
     rc = det_alloc((size_t)p.num_work * kBlockM * kMaxBlockN * sizeof(float), stream, &p.part);
@@ -1216,13 +1258,13 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
     if (p.part) det_free(p.part, stream);
     return set_error(YAMB_ECUDA, "%s: %s", what, cudaGetErrorString(err));
   };
-  if ((rc = fn(grid, smem_total, stream, tmA, tmB, tmA2, tmB2, tmD, p))) {
+  if ((rc = pl.fn(pl.grid, pl.smem_total, stream, tmA, tmB, tmA2, tmB2, tmD, p))) {
     if (p.part) det_free(p.part, stream);
     return rc;
   }
   if (a->epi == 2) {
     const long long total = (long long)a->M * a->N;
-    const long long cap = 4LL * dev_ctas, blocks = (total + 255) / 256;
+    const long long cap = 4LL * pl.sms, blocks = (total + 255) / 256;
     splitk_reduce_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, stream>>>(
         p.part, reinterpret_cast<float*>(a->D), a->ldd, a->M, a->N, p.block_n, p.n_blocks, p.ksplit);
     e = cudaGetLastError();
