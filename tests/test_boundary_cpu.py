@@ -200,6 +200,39 @@ def test_padded_shadow_flat_transfers_cpu():
         assert torch.equal(g.reshape(-1), sh.maps[n].float()), n
 
 
+def test_grad_targets_split_concatenated_weight_gradients_cpu():
+    """engine.GradTargets: a multi-branch project weight gradient is one [Cout, Chid] buffer whose
+    column slices become the branch weights' gradients; in direct mode they are added into the
+    `.grad` views and the buffer is kept by its owner, in autograd mode they are returned."""
+    from yet_another_mobilenet_series_b200 import engine
+    ws = [nn.Parameter(torch.zeros(8, c, 1, 1)) for c in (3, 5)]
+    full = torch.arange(64, dtype=torch.float32).view(8, 8)
+    owner = {}
+    for direct in (False, True):
+        for w in ws:
+            w.grad = torch.ones_like(w) if direct else None
+            w._yamb_direct = direct
+        gt = engine.GradTargets(ws)
+        assert gt.direct == direct and gt.host_reads != direct
+        buf = gt.concat(ws, 1, owner, "proj")
+        assert gt.host_reads                       # the split reads the buffer after the kernels
+        assert buf.shape == (8, 8) and bool((buf == 0).all())
+        assert ("proj" in owner) == direct
+        buf.copy_(full)
+        got = gt.result()
+        want = [full[:, :3].reshape(8, 3, 1, 1), full[:, 3:].reshape(8, 5, 1, 1)]
+        if direct:
+            assert got == (None, None)
+            got = [w.grad - 1 for w in ws]
+        for g, t in zip(got, want):
+            assert torch.equal(g, t)
+    single = engine.GradTargets(ws[:1])            # direct, one branch: the `.grad` itself
+    assert single.concat(ws[:1], 1, owner, "x").data_ptr() == ws[0].grad.data_ptr()
+    assert not single.host_reads and "x" not in owner
+    ws[1]._yamb_direct = False                     # mixed ownership: autograd mode
+    assert not engine.GradTargets(ws).direct
+
+
 def test_kernel_scratch_does_not_travel_with_a_deepcopy():
     """The EMA model is a deepcopy of the wrapper (reference common.py:164), possibly taken AFTER a
     forward has cached per-module kernel scratch (device buffers, ctypes argument structs) in the

@@ -183,10 +183,83 @@ def _at(t, c0):
     return None if t is None else t.data_ptr() + 4 * c0
 
 
-def direct_grads(params):
-    """True when every parameter carries a pre-allocated `.grad` that the flat-arena optimizer marked
-    `_yamb_direct`: the kernels then accumulate into those gradients and autograd gets None."""
-    return all(getattr(p, "_yamb_direct", False) and p.grad is not None for p in params)
+class GradTargets:
+    """Where the kernels of one backward accumulate the gradients of `params`, the parameters an
+    autograd Function received, and what that Function returns for them.
+
+    Direct mode: every parameter carries a pre-allocated `.grad` that the flat-arena optimizer
+    marked `_yamb_direct`.  The kernels `+=` into those gradients and autograd gets None.
+    Otherwise (autograd mode) the kernels accumulate into zeroed buffers made for this backward,
+    which are returned to autograd as they are: nothing outlives the backward, so nothing needs a
+    copy."""
+
+    def __init__(self, params):
+        self.params = list(params)
+        self.direct = all(getattr(p, "_yamb_direct", False) and p.grad is not None
+                          for p in self.params)
+        self.grads = {}
+        self.split = []      # (concatenated gradient, its parameters, dim): handed over by result()
+
+    def of(self, p):
+        """Accumulation target of `p`: its `.grad`, or a zeroed fp32 buffer of this backward."""
+        if self.direct:
+            return p.grad
+        g = self.grads.get(id(p))
+        if g is None:
+            g = self.grads[id(p)] = torch.zeros(p.shape, device=p.device, dtype=torch.float32)
+        return g
+
+    def concat(self, params, dim, owner, key):
+        """Accumulation target of 1x1 convolution weights concatenated along `dim` of their
+        [out, in] matrices; one weight gets its own target.  In direct mode several weights share
+        `owner[key]`, kept because a captured CUDA graph addresses it; in autograd mode a buffer
+        of this backward.  Each weight gets its slice from `result()`."""
+        if len(params) == 1:
+            return self.of(params[0]).view(params[0].shape[:2])
+        shape = list(params[0].shape[:2])
+        shape[dim] = sum(p.shape[dim] for p in params)
+        buf = owner.get(key) if self.direct else None
+        if buf is None:
+            buf = torch.zeros(shape, device=params[0].device, dtype=torch.float32)
+            if self.direct:
+                owner[key] = buf
+        else:
+            buf.zero_()
+        self.split.append((buf, params, dim))
+        return buf
+
+    def put(self, p, g):
+        """`g` is the finished gradient of `p` (added into `.grad` in direct mode)."""
+        if self.direct:
+            p.grad.add_(g)
+        else:
+            self.grads[id(p)] = g
+
+    def put_all(self, params, grads):
+        """`put` of a whole list: one multi-tensor add in direct mode."""
+        if self.direct:
+            torch._foreach_add_([p.grad for p in params], list(grads))
+        else:
+            self.grads.update((id(p), g) for p, g in zip(params, grads))
+
+    @property
+    def host_reads(self):
+        """Whether anything on the current stream still reads what the kernels accumulated:
+        autograd does in autograd mode, `result()` does to split a concatenated gradient."""
+        return not self.direct or bool(self.split)
+
+    def result(self):
+        """The gradients autograd gets, in parameter order (None in direct mode and for the
+        parameters without one)."""
+        for buf, params, dim in self.split:
+            c0 = 0
+            for p in params:
+                n = p.shape[dim]
+                self.put(p, buf.narrow(dim, c0, n).reshape(p.shape))
+                c0 += n
+        if self.direct:
+            return (None,) * len(self.params)
+        return tuple(self.grads.get(id(p)) for p in self.params)
 
 
 class _Bn:
@@ -551,7 +624,6 @@ class BlockPlan:
                     % nl.bn)
             self.nl_tail = _NlTail(nl, _Bn([nl.bn], dev), N, self.Ho, self.Wo, Cout, dev)
             self.bn4 = self.nl_tail.bn4
-            self.g_nl = torch.zeros_like(nl.depthwise_conv.weight, dtype=torch.float32)
         if self.se is not None:
             self.se_act = act_code_of(self.se.active_fn)
             self.se_r = self.se.se_reduce.weight.shape[0]
@@ -559,9 +631,6 @@ class BlockPlan:
             self.se_v = _f32(N * self.se_r, dev).view(N, self.se_r)
             self.se_du = _f32(N * self.se_r, dev).view(N, self.se_r)
             self.se_dt = _f32(N * Chid, dev).view(N, Chid)
-            self.g_se = {k: torch.zeros_like(t, dtype=torch.float32) for k, t in (
-                ("wr", self.se.se_reduce.weight), ("br", self.se.se_reduce.bias),
-                ("we", self.se.se_expand.weight), ("be", self.se.se_expand.bias))}
             self.pooled = _f32(N * Chid, dev).view(N, Chid)
             self.gate = _f32(N * Chid, dev).view(N, Chid)
             self.dgate = _f32(N * Chid, dev).view(N, Chid)
@@ -570,13 +639,12 @@ class BlockPlan:
         self.bn1 = _Bn(parts.bn1s, dev) if self.expand else None
         self.bn2 = _Bn([bn for _, bn in parts.dws], dev)
         self.bn3 = _Bn([parts.bn3], dev)
-        # ---- bf16 tensor-core operands + fp32 gradient accumulators ----
+        # ---- bf16 tensor-core operands ----
         self.w_exp_bf = torch.empty(Chid, Cin, device=dev, dtype=bf) if self.expand else None
         self.w_proj_bf = torch.empty(Cout, Chid, device=dev, dtype=bf)
         self.w_exp_own, self.w_proj_own = self.w_exp_bf, self.w_proj_bf
-        self.g_exp = _f32(Chid * Cin, dev).view(Chid, Cin) if self.expand else None
-        self.g_proj = _f32(Cout * Chid, dev).view(Cout, Chid)
-        self.g_dw = [torch.zeros_like(c.weight, dtype=torch.float32) for c in self.conv_dw]
+        # multi-branch expand / project weight gradients of direct mode (GradTargets.concat)
+        self.concat_grads = {}
         self.generation = 0
         self.pinned = False
 
@@ -976,9 +1044,8 @@ def _plan_for(block, x):
 class _BlockFn(torch.autograd.Function):
     """autograd boundary of the fused block: forward/backward run the sm_90a kernel sequences.
 
-    Parameter gradients: when a parameter carries a pre-allocated fp32 `.grad` that the flat-arena
-    optimizer marked with `_yamb_direct` the kernels accumulate straight into it and autograd gets
-    None; otherwise gradients are produced into plan-owned buffers and returned to autograd."""
+    Parameter gradients go where `GradTargets` puts them: straight into the flat-arena optimizer's
+    `.grad` views (autograd gets None), or into buffers of this backward returned to autograd."""
 
     @staticmethod
     def forward(ctx, x, block, *params):
@@ -999,116 +1066,38 @@ class _BlockFn(torch.autograd.Function):
                 "yamb: this block ran another forward before backward of the previous one; the "
                 "saved intermediates were overwritten (one forward/backward in flight per block)")
         (x,) = ctx.saved_tensors
-        dx, gmap = run_backward(block, plan, x, dy)
-        params = list(block.parameters())
-        pgrads = []
-        for p in params:
-            t = gmap.get(id(p))
-            pgrads.append(t.clone() if t is not None else None)
-        return (dx, None) + tuple(pgrads)
+        dx, grads = run_backward(block, plan, x, dy)
+        return (dx, None) + grads
 
 
 def run_backward(block, plan, x, dy):
-    """Backward kernel sequence of one block; returns dx and {id(param): grad} for the parameters
-    whose gradient was NOT accumulated straight into `.grad` (flat-arena direct mode)."""
+    """Backward kernel sequence of one block; returns dx and what autograd gets for
+    `block.parameters()` (`GradTargets.result`)."""
     dy = to_nhwc_bf16(dy)
-    direct = direct_grads(block.parameters())
+    gt = GradTargets(block.parameters())
 
-    def target(p, zero_buf):
-        if direct:
-            return p.grad
-        zero_buf.zero_()
-        return zero_buf
+    def bn_targets(bn):
+        return [] if bn is None else [(gt.of(m.weight), gt.of(m.bias)) for m in bn.mods]
 
-    def bn_targets(bn, key):
-        res = []
-        if bn is None:
-            return res
-        for i, m in enumerate(bn.mods):
-            if direct:
-                res.append((m.weight.grad, m.bias.grad))
-            else:
-                bufs = plan.__dict__.setdefault("_bn_gbuf", {})
-                k2 = (key, i)
-                if k2 not in bufs:
-                    bufs[k2] = (torch.zeros_like(m.weight), torch.zeros_like(m.bias))
-                bufs[k2][0].zero_()
-                bufs[k2][1].zero_()
-                res.append(bufs[k2])
-        return res
-
-    single_exp = plan.expand and len(plan.conv_exp) == 1
-    single_proj = len(plan.conv_proj) == 1
     g = {}
     if plan.expand:
-        if single_exp and direct:
-            g["exp"] = plan.conv_exp[0].weight.grad.view(plan.Chid, plan.Cin)
-        else:
-            plan.g_exp.zero_()
-            g["exp"] = plan.g_exp
-    if single_proj and direct:
-        g["proj"] = plan.conv_proj[0].weight.grad.view(plan.Cout, plan.Chid)
-    else:
-        plan.g_proj.zero_()
-        g["proj"] = plan.g_proj
-    g["dw"] = [target(c.weight, plan.g_dw[i]) for i, c in enumerate(plan.conv_dw)]
-    g["bn1"] = bn_targets(plan.bn1, "bn1")
-    g["bn2"] = bn_targets(plan.bn2, "bn2")
-    g["bn3"] = bn_targets(plan.bn3, "bn3")
+        g["exp"] = gt.concat([c.weight for c in plan.conv_exp], 0, plan.concat_grads, "exp")
+    g["proj"] = gt.concat([c.weight for c in plan.conv_proj], 1, plan.concat_grads, "proj")
+    g["dw"] = [gt.of(c.weight) for c in plan.conv_dw]
+    g["bn1"] = bn_targets(plan.bn1)
+    g["bn2"] = bn_targets(plan.bn2)
+    g["bn3"] = bn_targets(plan.bn3)
     if plan.se is not None:
         se = plan.se
-        g["se"] = {"wr": target(se.se_reduce.weight, plan.g_se["wr"]),
-                   "br": target(se.se_reduce.bias, plan.g_se["br"]),
-                   "we": target(se.se_expand.weight, plan.g_se["we"]),
-                   "be": target(se.se_expand.bias, plan.g_se["be"])}
+        g["se"] = {"wr": gt.of(se.se_reduce.weight), "br": gt.of(se.se_reduce.bias),
+                   "we": gt.of(se.se_expand.weight), "be": gt.of(se.se_expand.bias)}
     if plan.nl is not None:
-        g["bn4"] = bn_targets(plan.bn4, "bn4")
-        g["nl_dw"] = target(plan.nl.depthwise_conv.weight, plan.g_nl)
+        g["bn4"] = bn_targets(plan.bn4)
+        g["nl_dw"] = gt.of(plan.nl.depthwise_conv.weight)
     dx = plan.backward(x, dy, g)
-    if not (DEFER_JOIN and direct and single_proj and (single_exp or not plan.expand)):
-        join_side(plan.dev)   # the gradient hand-over below reads what the wgrads wrote
-    # ---- hand gradients to autograd ----
-    gmap = {}
-    if plan.expand:
-        if not (single_exp and direct):
-            c0 = 0
-            for conv in plan.conv_exp:
-                n = conv.weight.shape[0]
-                piece = plan.g_exp[c0:c0 + n].reshape(conv.weight.shape)
-                if direct:
-                    conv.weight.grad.add_(piece)
-                else:
-                    gmap[id(conv.weight)] = piece
-                c0 += n
-    if not (single_proj and direct):
-        c0 = 0
-        for conv in plan.conv_proj:
-            n = conv.weight.shape[1]
-            piece = plan.g_proj[:, c0:c0 + n].reshape(conv.weight.shape)
-            if direct:
-                conv.weight.grad.add_(piece)
-            else:
-                gmap[id(conv.weight)] = piece
-            c0 += n
-    if not direct:
-        for i, c in enumerate(plan.conv_dw):
-            gmap[id(c.weight)] = plan.g_dw[i]
-        if plan.nl is not None:
-            gmap[id(plan.nl.depthwise_conv.weight)] = plan.g_nl
-        for key, bn in (("bn1", plan.bn1), ("bn2", plan.bn2), ("bn3", plan.bn3),
-                        ("bn4", getattr(plan, "bn4", None))):
-            if bn is None:
-                continue
-            for i, m in enumerate(bn.mods):
-                dg, db = g[key][i]
-                gmap[id(m.weight)] = dg
-                gmap[id(m.bias)] = db
-    if plan.se is not None and not direct:
-        se = plan.se
-        for k, prm in (("wr", se.se_reduce.weight), ("br", se.se_reduce.bias),
-                       ("we", se.se_expand.weight), ("be", se.se_expand.bias)):
-            gmap[id(prm)] = plan.g_se[k]
-    return dx, gmap
+    if not DEFER_JOIN or gt.host_reads:
+        join_side(plan.dev)
+    return dx, gt.result()
 
 
 # ---- channel padding ---------------------------------------------------------------------------
@@ -1301,13 +1290,11 @@ class _PadFn(torch.autograd.Function):
         if plan.generation != ctx.generation:
             raise RuntimeError("yamb: block re-entered before its backward (see _BlockFn)")
         (x,) = ctx.saved_tensors
-        dx, gmap = run_backward(sh.shadow, plan, x, dy)
-        grads = sh.gather_grads(gmap, block)
-        params = list(block.parameters())
-        if direct_grads(params):
-            torch._foreach_add_([p.grad for p in params], grads)   # straight into the flat arena
-            return (dx, None) + (None,) * len(params)
-        return (dx, None) + tuple(grads)
+        dx, shadow_grads = run_backward(sh.shadow, plan, x, dy)
+        gmap = {id(p): g for p, g in zip(sh.shadow.parameters(), shadow_grads)}
+        gt = GradTargets(block.parameters())
+        gt.put_all(gt.params, sh.gather_grads(gmap, block))
+        return (dx, None) + gt.result()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1320,7 +1307,6 @@ class _PadFn(torch.autograd.Function):
 class _BnActState(Scratch):
     def __init__(self, bn, dev):
         self.bn = _Bn([bn], dev)
-        self.gbuf = None
 
 
 def _bn_act_state(bn, dev):
@@ -1374,16 +1360,8 @@ class _BnActFn(torch.autograd.Function):
         M = N * H * W
         hm = h.permute(0, 2, 3, 1).reshape(M, Cc)
         dym = dy.permute(0, 2, 3, 1).reshape(M, Cc)
-        direct = direct_grads((bn.weight, bn.bias))
-        if direct:
-            dg, db = bn.weight.grad, bn.bias.grad
-        else:
-            if st.gbuf is None:
-                st.gbuf = (torch.zeros_like(bn.weight), torch.zeros_like(bn.bias))
-            st.gbuf[0].zero_()
-            st.gbuf[1].zero_()
-            dg, db = st.gbuf
-        g = b.bwd_struct(M, [(dg, db)])
+        gt = GradTargets((bn.weight, bn.bias))
+        g = b.bwd_struct(M, [(gt.of(bn.weight), gt.of(bn.bias))])
         g.mean, g.invstd = c_mean, c_invstd      # this call's statistics, not the live buffers
         r = nat.BnReduce()
         r.M, r.C, r.lddy, r.ldh = M, Cc, Cc, Cc
@@ -1398,9 +1376,7 @@ class _BnActFn(torch.autograd.Function):
         a.ca, a.cb, a.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
         a.dh = dh.data_ptr()
         launch(lib.yamb_bn_bwd_apply_bwd, a, "bn_bwd_apply", 6 * M * Cc)
-        if direct:
-            return dh, None, None, None, None, None
-        return dh, None, None, dg.clone(), db.clone(), None
+        return (dh, None, None) + gt.result() + (None,)
 
 
 def bn_act_apply(bn, active_fn, h, stats_taken=False):

@@ -8,8 +8,8 @@ Every parameter, gradient and optimizer-state tensor is a VIEW into one flat fp3
     (utils/optim.py:53-64, train.py:109-114) are folded into the same pass (`fold_l2`,
     `attach_ema`),
   * a bf16 mirror of the weights is refreshed in the same pass and used directly as the
-    tensor-core operand of the block kernels (`_yamb_bf16`), and the block kernels accumulate
-    weight gradients straight into the arena (`_yamb_direct`).
+    tensor-core operand of the block kernels (`_yamb_bf16`), and the kernels accumulate
+    parameter gradients straight into the arena (`_yamb_direct`, read by `engine.GradTargets`).
 
 A subclass names its state arenas and per-parameter state (`_alloc_state`, `_link_state`), launches
 its kernel (`_launch`) and updates its host-side state after the launch (`_after_step`).

@@ -25,12 +25,11 @@ def _mat(t):
 
 
 class _PwState(engine.Scratch):
-    """Per-module device state of a 1x1 convolution: bf16 weight copy, fp32 weight gradient."""
+    """Per-module device state of a 1x1 convolution: bf16 weight copy."""
 
     def __init__(self, conv, dev):
         self.w_own = torch.empty(conv.out_channels, conv.in_channels, device=dev,
                                  dtype=torch.bfloat16)
-        self.g_own = None
         self.dev = dev
 
 
@@ -71,7 +70,7 @@ class _PwConvFn(torch.autograd.Function):
             g.bn_fwd = C.pointer(b.fwd_struct(M))
         engine.launch(nat.lib().yamb_pointwise_gemm, g, "head_conv_fwd", 2 * M * (Cin + Cout),
                       2 * M * Cin * Cout)
-        ctx.conv, ctx.st = conv, st
+        ctx.conv = conv
         ctx.save_for_backward(x, wbf)
         return h
 
@@ -79,19 +78,13 @@ class _PwConvFn(torch.autograd.Function):
     def backward(ctx, dh):
         lib = nat.lib()
         x, wbf = ctx.saved_tensors
-        conv, st = ctx.conv, ctx.st
+        conv = ctx.conv
         dh = engine.to_nhwc_bf16(dh)
         N, Cin, H, W = x.shape
         Cout = conv.out_channels
         M = N * H * W
-        direct = engine.direct_grads((conv.weight,))
-        if direct:
-            gw = conv.weight.grad
-        else:
-            if st.g_own is None:
-                st.g_own = torch.zeros(Cout, Cin, device=x.device, dtype=torch.float32)
-            st.g_own.zero_()
-            gw = st.g_own
+        gt = engine.GradTargets((conv.weight,))
+        gw = gt.of(conv.weight)
         # dgrad: dx[M, Cin] = dh[M, Cout] * W[Cout, Cin]   (weight read MN-major)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -106,7 +99,7 @@ class _PwConvFn(torch.autograd.Function):
                    a_mn_major=1, b_mn_major=1, epi=2)
         engine.launch(lib.yamb_pointwise_gemm, g2, "head_conv_wgrad", 2 * M * (Cin + Cout),
                       2 * M * Cin * Cout)
-        return dx, None, None, (None if direct else gw.view_as(conv.weight).clone())
+        return (dx, None, None) + gt.result()
 
 
 def pw_conv_bn_act(mod, x):
@@ -165,7 +158,6 @@ class _LinearState(engine.Scratch):
         self.w_own = torch.empty(lin.out_features, lin.in_features, device=dev,
                                  dtype=torch.bfloat16)
         self.bias_bf = torch.empty(lin.out_features, device=dev, dtype=torch.bfloat16)
-        self.g_own = None
         self.dev = dev
 
 
@@ -190,7 +182,7 @@ class _LinearFn(torch.autograd.Function):
                   residual=st.bias_bf.data_ptr(), ldr=0)
         engine.launch(lib.yamb_pointwise_gemm, g, "fc_fwd", 2 * (M * I + O * I + M * O),
                       2 * M * I * O)
-        ctx.lin, ctx.st = lin, st
+        ctx.lin = lin
         ctx.save_for_backward(x, wbf)
         return y
 
@@ -198,20 +190,14 @@ class _LinearFn(torch.autograd.Function):
     def backward(ctx, dy):
         lib = nat.lib()
         x, wbf = ctx.saved_tensors
-        lin, st = ctx.lin, ctx.st
+        lin = ctx.lin
         M, I = x.shape
         O = lin.out_features
         dy = dy.contiguous()
         if dy.dtype != torch.bfloat16:
             dy = dy.to(torch.bfloat16)
-        direct = engine.direct_grads((lin.weight, lin.bias))
-        if direct:
-            gw = lin.weight.grad
-        else:
-            if st.g_own is None:
-                st.g_own = torch.zeros(O, I, device=x.device, dtype=torch.float32)
-            st.g_own.zero_()
-            gw = st.g_own
+        gt = engine.GradTargets((lin.weight, lin.bias))
+        gw = gt.of(lin.weight)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(M, I, device=x.device, dtype=torch.bfloat16)
@@ -223,15 +209,10 @@ class _LinearFn(torch.autograd.Function):
         engine.launch(lib.yamb_pointwise_gemm, g2, "fc_wgrad", 2 * (M * I + M * O) + 4 * O * I,
                       2 * M * I * O)
         # bias gradient: column sums of dlogits
-        if direct:
-            gb_t = lin.bias.grad
-        else:
-            gb_t = torch.zeros(O, device=x.device, dtype=torch.float32)
-        nat.check(lib.yamb_colsum_bf16(dy.data_ptr(), M, O, O, gb_t.data_ptr(), nat.stream_handle()))
+        nat.check(lib.yamb_colsum_bf16(dy.data_ptr(), M, O, O, gt.of(lin.bias).data_ptr(),
+                                       nat.stream_handle()))
         engine.LAUNCHES += 1
-        if direct:
-            return dx, None, None, None
-        return dx, None, gw.clone(), gb_t
+        return (dx, None) + gt.result()
 
 
 def linear_apply(lin, x):
@@ -330,16 +311,14 @@ class _StemConvFn(torch.autograd.Function):
         dh = engine.to_nhwc_bf16(dh)
         N, _, H, W = x.shape
         Cout = conv.out_channels
-        w = conv.weight
-        direct = engine.direct_grads((w,))
-        gw = w.grad if direct else torch.zeros_like(w, dtype=torch.float32)
+        gt = engine.GradTargets((conv.weight,))
         a = nat.StemConv()
         a.N, a.H, a.W, a.Cout = N, H, W, Cout
-        a.x, a.dh, a.dw = x.data_ptr(), dh.data_ptr(), gw.data_ptr()
+        a.x, a.dh, a.dw = x.data_ptr(), dh.data_ptr(), gt.of(conv.weight).data_ptr()
         engine.launch(lib.yamb_stem_conv_wgrad, a, "stem_conv_wgrad",
                       2 * N * (H * W * 3 + dh.shape[2] * dh.shape[3] * Cout),
                       2 * N * dh.shape[2] * dh.shape[3] * Cout * 27)
-        return None, None, (None if direct else gw)
+        return (None, None) + gt.result()
 
 
 def stem_supported(mod, x):
