@@ -1,8 +1,8 @@
 """Host-side sequencing of the sm_90a kernels for one inverted-residual block.
 
 A `BlockPlan` owns the HBM-resident intermediates of one block for one input shape
-(NHWC bf16 [pixels, channels] matrices) and the pre-built C-ABI argument structs; `block_apply`
-is the autograd entry the modules in `mobilenet_base.py` call.  Kernel order (train mode):
+(NHWC bf16 [pixels, channels] matrices) and launches the kernels on them; `block_apply` is the
+autograd entry the modules in `mobilenet_base.py` call.  Kernel order (train mode):
 
   forward   expand GEMM (+BN1 stats) -> depthwise (BN1+act on load, +BN2 stats)
             -> project GEMM (BN2+act operand transform, +BN3 stats) -> BN3 apply (+x)
@@ -96,10 +96,6 @@ def join_side(dev=None):
                                                       else torch.cuda.current_device())):
             torch.cuda.current_stream().wait_stream(st["stream"])
             st["pending"] = False
-
-
-def lib_fn(name):
-    return getattr(nat.lib(), name)
 
 
 def act_code_of(active_fn):
@@ -396,6 +392,104 @@ def _nl_norm_supported(norm):
         norm.track_running_stats and norm.running_mean is not None
 
 
+# ---- kernel calls made from several places -------------------------------------------------------
+# Activations are bf16 [pixels, C] matrices, per-channel vectors fp32; one branch of a wider
+# activation is a column slice (a view), so C and the row pitch come from the tensor.  `stats` is
+# a yamb_bn_fwd / yamb_bn_bwd struct from `_Bn.fwd_struct` / `bwd_struct`, built by the caller
+# right before the call.
+
+def _bn_apply(bn, h, y, act, tag, residual=None, residual2=None):
+    """y = act(scale*h + shift) (+ residual) (+ residual2) with the coefficients of `bn` (a
+    `_Bn`); dense [M, C] operands."""
+    M, Cc = h.shape
+    a = nat.BnApply()
+    a.M, a.C, a.ldh, a.ldr, a.ldy = M, Cc, Cc, Cc, Cc
+    a.h, a.scale, a.shift, a.act = h.data_ptr(), bn.scale.data_ptr(), bn.shift.data_ptr(), act
+    a.residual, a.y = nat.ptr(residual), y.data_ptr()
+    if residual2 is not None:
+        a.residual2, a.ldr2 = residual2.data_ptr(), Cc
+    operands = 2 + (residual is not None) + (residual2 is not None)
+    launch(nat.lib().yamb_bn_apply_fwd, a, tag, 2 * M * Cc * operands)
+
+
+def _bn_reduce(stats, dy, h, tag, z=None):
+    """BatchNorm backward statistics of dy over dense [M, C] dy and h, finalised by `stats`;
+    z = (z_scale, z_shift, act): dy is first multiplied by act'(z_scale*h + z_shift)."""
+    M, Cc = h.shape
+    r = nat.BnReduce()
+    r.M, r.C, r.lddy, r.ldh = M, Cc, Cc, Cc
+    r.dy, r.h, r.bn = dy.data_ptr(), h.data_ptr(), C.pointer(stats)
+    if z is not None:
+        r.z_scale, r.z_shift, r.z_act = z
+    launch(nat.lib().yamb_bn_reduce_bwd, r, tag, 4 * M * Cc)
+
+
+def _bn_bwd_apply(bn, dy, h, dh, tag, z=None):
+    """dh = ca*dy + cb*h + cc with the backward coefficients of `bn` (a `_Bn`), dy taken as in
+    `_bn_reduce`; dense [M, C] operands."""
+    M, Cc = h.shape
+    a = nat.BnBwdApply()
+    a.M, a.C, a.lddy, a.ldh, a.lddh = M, Cc, Cc, Cc, Cc
+    a.dy, a.h, a.dh = dy.data_ptr(), h.data_ptr(), dh.data_ptr()
+    if z is not None:
+        a.z_scale, a.z_shift, a.z_act = z
+    a.ca, a.cb, a.cc = bn.ca.data_ptr(), bn.cb.data_ptr(), bn.cc.data_ptr()
+    launch(nat.lib().yamb_bn_bwd_apply_bwd, a, tag, 6 * M * Cc)
+
+
+def _dw_fwd(conv, nhw, x, y, tag, pre=None, stats=None):
+    """y = depthwise `conv` of x over N x H x W pixels (x read with y's pitch); pre = (scale,
+    shift, act) is applied to x on load; `stats` takes y's BatchNorm statistics."""
+    k, s = conv.kernel_size[0], conv.stride[0]
+    Cc = y.shape[1]
+    d = nat.DwFwd()
+    N, H, W = d.N, d.H, d.W = nhw
+    d.C, d.ldc, d.k, d.stride = Cc, y.stride(0), k, s
+    d.x, d.w, d.y = x.data_ptr(), conv.weight.data_ptr(), y.data_ptr()
+    if pre is not None:
+        d.in_scale, d.in_shift, d.in_act = pre[0].data_ptr(), pre[1].data_ptr(), pre[2]
+    if stats is not None:
+        d.bn = C.pointer(stats)
+    m_in, m_out = N * H * W, N * ((H - 1) // s + 1) * ((W - 1) // s + 1)
+    launch(nat.lib().yamb_depthwise_fwd, d, tag, 2 * Cc * (m_in + m_out), 2 * m_out * Cc * k * k)
+
+
+def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, stats=None):
+    """Backward of `_dw_fwd` from the output gradient ca*dz + cb*h + cc (coef = (ca, cb, cc)):
+    weight gradient += into dw, input gradient into dx, taken back through `pre` when given (its
+    BatchNorm backward statistics into `stats`), + residual.  Every matrix is read with dz's
+    pitch."""
+    k, s = conv.kernel_size[0], conv.stride[0]
+    Cc = dz.shape[1]
+    d = nat.DwBwd()
+    N, H, W = d.N, d.H, d.W = nhw
+    d.C, d.ldc, d.k, d.stride = Cc, dz.stride(0), k, s
+    d.dz, d.h = dz.data_ptr(), h.data_ptr()
+    d.ca, d.cb, d.cc = (t.data_ptr() for t in coef)
+    d.w, d.dw = conv.weight.data_ptr(), dw.data_ptr()
+    d.x, d.dx, d.residual = x.data_ptr(), dx.data_ptr(), nat.ptr(residual)
+    if pre is not None:
+        d.in_scale, d.in_shift, d.in_act = pre[0].data_ptr(), pre[1].data_ptr(), pre[2]
+    if stats is not None:
+        d.bn = C.pointer(stats)
+    m_in, m_out = N * H * W, N * ((H - 1) // s + 1) * ((W - 1) // s + 1)
+    launch(nat.lib().yamb_depthwise_bwd, d, tag, 4 * Cc * (m_in + m_out), 4 * m_out * Cc * k * k)
+
+
+def _se_fc(se, pooled, u, v, gate):
+    """gate = sigmoid(W_e act(W_r pooled + b_r) + b_e) of the Squeeze-and-Excitation module `se`
+    on pooled [N, C], keeping u = W_r pooled + b_r and v = act(u) [N, R] (fp32 throughout)."""
+    N, Cc = pooled.shape
+    R = se.se_reduce.weight.shape[0]
+    f = nat.SeFc()
+    f.N, f.C, f.R, f.act = N, Cc, R, act_code_of(se.active_fn)
+    f.pooled = pooled.data_ptr()
+    f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
+    f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
+    f.u, f.v, f.gate = u.data_ptr(), v.data_ptr(), gate.data_ptr()
+    launch(nat.lib().yamb_se_fc_fwd, f, "se_fc", 4 * N * Cc * 2, 4 * N * Cc * R)
+
+
 class _NlTail:
     """Non-local block (reference models/mobilenet_base.py:158-173) behind a BatchNorm output l,
     for one shape: y = norm(dw3x3(f)) + l (+ x), f = (W/H) theta (phi^T g).  Owns l, f, h (bf16
@@ -434,7 +528,7 @@ class _NlTail:
         g.X, g.ldx, g.I = X.data_ptr(), self.C, I
         g.Y, g.ldy, g.J = Y.data_ptr(), self.C, self.C
         g.alpha, g.G = alpha, G.data_ptr()
-        launch(lib_fn("yamb_nl_gram_fwd"), g, tag, 4 * self.M * self.C // (sub * sub))
+        launch(nat.lib().yamb_nl_gram_fwd, g, tag, 4 * self.M * self.C // (sub * sub))
 
     def rowmat(self, X, K, Mat, sk, so, O, sub, alpha, out, tag, base=None, accumulate=0):
         r = nat.NlRowmat()
@@ -446,11 +540,10 @@ class _NlTail:
             r.base, r.ldb, r.O_copy = base.data_ptr(), self.C, self.C
         r.accumulate = accumulate
         r.out, r.ldo = out.data_ptr(), self.C
-        launch(lib_fn("yamb_nl_rowmat_fwd"), r, tag, 4 * self.M * self.C // (sub * sub))
+        launch(nat.lib().yamb_nl_rowmat_fwd, r, tag, 4 * self.M * self.C // (sub * sub))
 
     def forward(self, xm, y, residual):
         """self.l -> y."""
-        lib = nat.lib()
         Cc, c = self.C, self.cr
         instance = self.instance and self.bn4.batch_stats
         if instance and self.H * self.W == 1:
@@ -460,34 +553,19 @@ class _NlTail:
         # F = phi^T g over the sub-sampled pixels; f = (W/H) theta F
         self.gram(self.l, c, self.l, self.sub, 1.0, self.F, "nl_gram")
         self.rowmat(self.l, c, self.F, Cc, 1, Cc, 1, self.scale, self.f, "nl_apply")
-        # depthwise 3x3 (no activation before it) + BN4 statistics
-        d = nat.DwFwd()
-        d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.H, self.W, Cc, Cc, 3, 1
-        d.x = self.f.data_ptr()
-        d.w = self.nl.depthwise_conv.weight.data_ptr()
-        d.y = self.h.data_ptr()
-        if instance:
-            pass                               # statistics per sample: yamb_instance_norm_fwd
-        elif self.bn4.batch_stats:
-            d.bn = C.pointer(self.bn4.fwd_struct(self.M))
-        else:
+        # depthwise 3x3 (no activation before it) + BN4 statistics (InstanceNorm: per sample, by
+        # yamb_instance_norm_fwd)
+        if not self.bn4.batch_stats:
             self.bn4.eval_coeffs()
-        launch(lib.yamb_depthwise_fwd, d, "nl_dw_fwd", 4 * Cc * self.M, 2 * self.M * Cc * 9)
+        _dw_fwd(self.nl.depthwise_conv, (self.N, self.H, self.W), self.f, self.h, "nl_dw_fwd",
+                stats=self.bn4.fwd_struct(self.M) if self.bn4.batch_stats and not instance
+                else None)
         if instance:
             self._instance_forward(xm, y, residual)
             return
         # y = BN4(h) + l (+ x)
-        a = nat.BnApply()
-        a.M, a.C = self.M, Cc
-        a.ldh = a.ldr = a.ldy = Cc
-        a.h, a.scale, a.shift = self.h.data_ptr(), self.bn4.scale.data_ptr(), \
-            self.bn4.shift.data_ptr()
-        a.act = 0
-        a.residual = self.l.data_ptr()
-        if residual:
-            a.residual2, a.ldr2 = xm.data_ptr(), Cc
-        a.y = y.data_ptr()
-        launch(lib.yamb_bn_apply_fwd, a, "nl_bn_apply", 2 * self.M * Cc * (4 if residual else 3))
+        _bn_apply(self.bn4, self.h, y, 0, "nl_bn_apply", residual=self.l,
+                  residual2=xm if residual else None)
 
     def _instance_forward(self, xm, y, residual):
         """y = InstanceNorm(h) + l (+ x) with per-sample statistics; mean / invstd [N][C] kept for
@@ -533,15 +611,11 @@ class _NlTail:
         """dy -> dl (gradient of the BN3 output): norm backward, depthwise 3x3 backward, the two
         products' backward, plus the `+ l` pass-through.  grads: the plan's accumulation targets
         ('bn4', 'nl_dw')."""
-        lib = nat.lib()
         Cc, c, bf, dev = self.C, self.cr, torch.bfloat16, self.l.device
         if self.df is None:
             self.df = torch.empty(self.M, Cc, device=dev, dtype=bf)
             self.dl = torch.empty(self.M, Cc, device=dev, dtype=bf)
             self.dF = _f32(self.N * c * Cc, dev)
-        d = nat.DwBwd()
-        d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.H, self.W, Cc, Cc, 3, 1
-        d.h = self.h.data_ptr()
         if self.used_instance_stats:
             # InstanceNorm with per-sample statistics: its backward writes dh (bf16), which the
             # depthwise backward takes with the identity coefficients ca = 1, cb = cc = 0
@@ -550,22 +624,12 @@ class _NlTail:
                 self.ones = torch.ones(Cc, device=dev, dtype=torch.float32)
                 self.zeros = _f32(Cc, dev)
             self.instance_backward(dym, self.in_dh, grads["bn4"])
-            d.dz = self.in_dh.data_ptr()
-            d.ca, d.cb, d.cc = self.ones.data_ptr(), self.zeros.data_ptr(), self.zeros.data_ptr()
+            dz, coef = self.in_dh, (self.ones, self.zeros, self.zeros)
         else:
-            r = nat.BnReduce()
-            r.M, r.C, r.lddy, r.ldh = self.M, Cc, Cc, Cc
-            r.dy, r.h = dym.data_ptr(), self.h.data_ptr()
-            r.bn = C.pointer(self.bn4.bwd_struct(self.M, grads["bn4"]))
-            launch(lib.yamb_bn_reduce_bwd, r, "nl_bn_reduce", 4 * self.M * Cc)
-            d.dz = dym.data_ptr()
-            d.ca, d.cb, d.cc = self.bn4.ca.data_ptr(), self.bn4.cb.data_ptr(), \
-                self.bn4.cc.data_ptr()
-        d.w = self.nl.depthwise_conv.weight.data_ptr()
-        d.dw = grads["nl_dw"].data_ptr()
-        d.x = self.f.data_ptr()
-        d.dx = self.df.data_ptr()
-        launch(lib.yamb_depthwise_bwd, d, "nl_dw_bwd", 8 * Cc * self.M, 4 * self.M * Cc * 9)
+            _bn_reduce(self.bn4.bwd_struct(self.M, grads["bn4"]), dym, self.h, "nl_bn_reduce")
+            dz, coef = dym, (self.bn4.ca, self.bn4.cb, self.bn4.cc)
+        _dw_bwd(self.nl.depthwise_conv, (self.N, self.H, self.W), dz, self.h, coef,
+                grads["nl_dw"], self.f, self.df, "nl_dw_bwd")
         # dF = (W/H) theta^T df (all pixels);  dl = dy + [dtheta | 0];  sub-sampled rows += dphi, dg
         self.gram(self.l, c, self.df, 1, self.scale, self.dF, "nl_gram_bwd")
         self.rowmat(self.df, Cc, self.F, 1, Cc, c, 1, self.scale, self.dl, "nl_dtheta", base=dym)
@@ -575,10 +639,14 @@ class _NlTail:
 
 
 class BlockPlan:
+    """The training-path kernel sequence of one block for one input shape, with the HBM-resident
+    intermediates it owns.  Every C-ABI argument struct is built per call, right before its
+    launch: a BatchNorm struct carries the statistics workspace of the stream it is launched on
+    (`Workspace.get`), and the same plan may run on another stream next time."""
+
     def __init__(self, block, x):
         dev = x.device
         self.dev = dev
-        self.lib = nat.lib()
         N, Cin, H, W = x.shape
         self.N, self.H, self.W, self.Cin = N, H, W, Cin
         self.stride = block.stride
@@ -587,7 +655,6 @@ class BlockPlan:
         self.Wo = (W - 1) // self.stride + 1
         self.Cout = block.output_dim
         self.channels = list(block.channels)
-        self.ks = list(block.kernel_sizes)
         self.expand = bool(block.expand)
         self.residual = bool(block.use_res_connect)
         self.act = act_code_of(block.active_fn)
@@ -692,57 +759,40 @@ class BlockPlan:
     # -- forward ---------------------------------------------------------------------------------
     def forward(self, x):
         """x: channels_last bf16 [N,Cin,H,W]; returns channels_last bf16 [N,Cout,Ho,Wo]."""
-        lib = self.lib
+        lib = nat.lib()
         self.generation += 1
         self._refresh_weights()
         xm = x.permute(0, 2, 3, 1).reshape(self.M_in, self.Cin)  # view, NHWC matrix
         y = torch.empty((self.N, self.Cout, self.Ho, self.Wo), device=self.dev,
                         dtype=torch.bfloat16, memory_format=torch.channels_last)
-        # 1. expand 1x1 + BN1 statistics
+        # 1. expand 1x1 + BN1 statistics: the GEMM finalises the statistics of one BatchNorm
+        #    module, so with one module per branch it runs once per branch slice
         if self.expand:
-            g = nat.Gemm()
-            g.M, g.N, g.K = self.M_in, self.Chid, self.Cin
-            g.A, g.lda = xm.data_ptr(), self.Cin
-            g.B, g.ldb = self.w_exp_bf.data_ptr(), self.Cin
-            g.D, g.ldd = self.h1.data_ptr(), self.Chid
-            if self.bn1.batch_stats:
-                if self.bn1.single:
-                    g.bn_fwd = C.pointer(self.bn1.fwd_struct(self.M_in))
-                    launch(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
-                           2 * self.M_in * (self.Cin + self.Chid),
-                           2 * self.M_in * self.Cin * self.Chid)
-                else:
-                    # per-branch BN modules: one finalize per branch slice is done by the GEMM only
-                    # for a single module; otherwise run the statistics per slice via N-slices
-                    self._gemm_sliced_stats(g, self.bn1, self.M_in)
-            else:
+            stats = self.bn1.batch_stats
+            if not stats:
                 self.bn1.eval_coeffs()
+            for c0, cb in self.bn1.slices if stats else [(0, self.Chid)]:
+                s = slice(c0, c0 + cb)
+                g = nat.Gemm()
+                g.M, g.N, g.K = self.M_in, cb, self.Cin
+                g.A, g.lda = xm.data_ptr(), self.Cin
+                g.B, g.ldb = self.w_exp_bf[s].data_ptr(), self.Cin
+                g.D, g.ldd = self.h1[:, s].data_ptr(), self.Chid
+                if stats:
+                    g.bn_fwd = C.pointer(self.bn1.fwd_struct(self.M_in, c0, cb))
                 launch(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
-                       2 * self.M_in * (self.Cin + self.Chid),
-                       2 * self.M_in * self.Cin * self.Chid)
-        # 2. depthwise per branch (BN1+act applied on load) + BN2 statistics
+                       2 * self.M_in * (self.Cin + cb), 2 * self.M_in * self.Cin * cb)
+        # 2. depthwise per branch (BN1+act applied on load) + BN2 statistics; without the
+        #    expansion hidden == inp, so x has the hidden pitch
         if not self.bn2.batch_stats:
             self.bn2.eval_coeffs()
-        c0 = 0
-        for b, (cb, k) in enumerate(zip(self.channels, self.ks)):
-            d = nat.DwFwd()
-            # hidden pitch; when not expanding hidden == inp, so x has the same pitch
-            d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.H, self.W, cb, self.Chid, k, \
-                self.stride
-            if self.expand:
-                d.x = self.h1.data_ptr() + c0 * 2
-                d.in_scale = self.bn1.scale.data_ptr() + c0 * 4
-                d.in_shift = self.bn1.shift.data_ptr() + c0 * 4
-                d.in_act = self.act
-            else:
-                d.x = xm.data_ptr()
-            d.w = self.conv_dw[b].weight.data_ptr()
-            d.y = self.h2.data_ptr() + c0 * 2
-            if self.bn2.batch_stats:
-                d.bn = C.pointer(self.bn2.fwd_struct(self.M_out, c0, cb))
-            launch(lib.yamb_depthwise_fwd, d, "dw_fwd", 2 * cb * (self.M_in + self.M_out),
-                   2 * self.M_out * cb * k * k)
-            c0 += cb
+        for (c0, cb), conv in zip(self.bn2.slices, self.conv_dw):
+            s = slice(c0, c0 + cb)
+            _dw_fwd(conv, (self.N, self.H, self.W), self.h1[:, s] if self.expand else xm,
+                    self.h2[:, s], "dw_fwd",
+                    pre=(self.bn1.scale[s], self.bn1.shift[s], self.act) if self.expand else None,
+                    stats=self.bn2.fwd_struct(self.M_out, c0, cb) if self.bn2.batch_stats
+                    else None)
         # 2b. Squeeze-and-Excitation gate (reference mobilenet_base.py:110-113): spatial mean of
         #     a2 = act(bn2(h2)) by a kernel, the two fully connected layers + sigmoid by another,
         #     the gate applied inside the project GEMM's operand transform
@@ -753,17 +803,9 @@ class BlockPlan:
                 self.bn2.shift.data_ptr(), self.act
             sp.pooled = self.pooled.data_ptr()
             launch(lib.yamb_se_pool_fwd, sp, "se_pool", 2 * self.M_out * self.Chid)
-            se = self.se
             # the two fully connected layers on the pooled [N, C] vectors (fp32, like the reference
             # keeps them) + sigmoid: one launch (csrc/se_fc.cu)
-            f = nat.SeFc()
-            f.N, f.C, f.R, f.act = self.N, self.Chid, self.se_r, self.se_act
-            f.pooled = self.pooled.data_ptr()
-            f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
-            f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
-            f.u, f.v, f.gate = self.se_u.data_ptr(), self.se_v.data_ptr(), self.gate.data_ptr()
-            launch(lib.yamb_se_fc_fwd, f, "se_fc", 4 * self.N * self.Chid * 2,
-                   4 * self.N * self.Chid * self.se_r)
+            _se_fc(self.se, self.pooled, self.se_u, self.se_v, self.gate)
         # 3. project 1x1 (BN2+act as operand transform) + BN3 statistics
         g = nat.Gemm()
         g.M, g.N, g.K = self.M_out, self.Cout, self.Chid
@@ -782,42 +824,18 @@ class BlockPlan:
                2 * self.M_out * (self.Chid + self.Cout),
                2 * self.M_out * self.Chid * self.Cout)
         # 4. BN3 apply (+ skip connection)
-        a = nat.BnApply()
-        a.M, a.C = self.M_out, self.Cout
-        a.ldh = a.ldr = a.ldy = self.Cout
-        a.h, a.scale, a.shift = self.h3.data_ptr(), self.bn3.scale.data_ptr(), \
-            self.bn3.shift.data_ptr()
-        a.act = 0
         if self.nl is None:
-            a.residual = xm.data_ptr() if self.residual else None
-            a.y = y.data_ptr()
-            launch(lib.yamb_bn_apply_fwd, a, "bn_apply",
-                   2 * self.M_out * self.Cout * (3 if self.residual else 2))
+            _bn_apply(self.bn3, self.h3, y, 0, "bn_apply", residual=xm if self.residual else None)
             return y
-        a.y = self.nl_tail.l.data_ptr()         # l = BN3(h3): the non-local block's input
-        launch(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * self.M_out * self.Cout)
+        _bn_apply(self.bn3, self.h3, self.nl_tail.l, 0, "bn_apply")   # l: the non-local input
         self.nl_tail.forward(xm, y, self.residual)
         return y
-
-    def _gemm_sliced_stats(self, g, bn, count):
-        """Expand GEMM whose output channels belong to several BN modules: one GEMM per module
-        slice (N-slices of the weight), each finalising its own BatchNorm."""
-        lib = self.lib
-        for (c0, cb) in bn.slices:
-            gs = nat.Gemm()
-            C.memmove(C.byref(gs), C.byref(g), C.sizeof(nat.Gemm))
-            gs.N = cb
-            gs.B = g.B + c0 * g.ldb * 2
-            gs.D = g.D + c0 * 2
-            gs.bn_fwd = C.pointer(bn.fwd_struct(count, c0, cb))
-            launch(lib.yamb_pointwise_gemm, gs, "pw_expand_fwd", 2 * gs.M * (gs.K + cb),
-                   2 * gs.M * gs.K * cb)
 
     def _se_backward(self, grads):
         """SE backward: dgate by a reduction kernel, the backward of the two fully connected layers
         (+ their parameter gradients) by yamb_se_fc_bwd, then
         dz2 = (d(a2*gate)*gate + dpool) * act'(z2) with the BN2-backward statistics."""
-        lib = self.lib
+        lib = nat.lib()
         se = self.se
         HW = self.Ho * self.Wo
         r = nat.SeBwdReduce()
@@ -836,19 +854,17 @@ class BlockPlan:
         b.g_wr, b.g_br, b.g_we, b.g_be = (tg[k].data_ptr() for k in ("wr", "br", "we", "be"))
         launch(lib.yamb_se_fc_bwd, b, "se_fc_bwd", 4 * self.N * self.Chid * 4,
                8 * self.N * self.Chid * self.se_r)
-        for (c0, cb) in self.bn2.slices:
+        for c0, cb in self.bn2.slices:
+            s = slice(c0, c0 + cb)
             a = nat.SeBwdApply()
             a.M, a.C, a.ldd, a.ldh, a.ldz = self.M_out, cb, self.Chid, self.Chid, self.Chid
             a.rows_per_sample = HW
-            a.dy = self.dz2.data_ptr() + c0 * 2
-            a.h = self.h2.data_ptr() + c0 * 2
-            a.scale = self.bn2.scale.data_ptr() + c0 * 4
-            a.shift = self.bn2.shift.data_ptr() + c0 * 4
+            a.dy = a.dz = self.dz2[:, s].data_ptr()
+            a.h = self.h2[:, s].data_ptr()
+            a.scale, a.shift = _at(self.bn2.scale, c0), _at(self.bn2.shift, c0)
             a.act = self.act
-            a.gate = self.gate.data_ptr() + c0 * 4
-            a.dpool = self.dpool.data_ptr() + c0 * 4
+            a.gate, a.dpool = self.gate[:, s].data_ptr(), self.dpool[:, s].data_ptr()
             a.ldg = self.Chid
-            a.dz = self.dz2.data_ptr() + c0 * 2
             a.bn = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
             launch(lib.yamb_se_bwd_apply_bwd, a, "se_bwd_apply", 6 * self.M_out * cb)
 
@@ -857,7 +873,7 @@ class BlockPlan:
         """grads: dict with fp32 accumulation targets:
            'exp' [Chid,Cin], 'proj' [Cout,Chid], 'dw' list[[C,1,k,k]], 'bn1'/'bn2'/'bn3' lists of
            (dgamma, dbeta) per reference BN module.  Returns dx (channels_last bf16)."""
-        lib = self.lib
+        lib = nat.lib()
         bf = torch.bfloat16
         if self.dz2 is None:
             self.dh3 = torch.empty(self.M_out, self.Cout, device=self.dev, dtype=bf)
@@ -872,57 +888,34 @@ class BlockPlan:
         if self.nl is not None:
             dym = self.nl_tail.backward(dym, grads)
         # 1. BN3 backward reduction -> ca3, cb3, cc3, dgamma3, dbeta3
-        r = nat.BnReduce()
-        r.M, r.C, r.lddy, r.ldh = self.M_out, self.Cout, self.Cout, self.Cout
-        r.dy, r.h = dym.data_ptr(), self.h3.data_ptr()
-        r.bn = C.pointer(self.bn3.bwd_struct(self.M_out, grads["bn3"]))
-        launch(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * self.M_out * self.Cout)
+        _bn_reduce(self.bn3.bwd_struct(self.M_out, grads["bn3"]), dym, self.h3, "bn_reduce")
         # 1b. dh3 = ca3*dy + cb3*h3 + cc3, formed once: both project GEMMs read it as a plain
         #     operand (as a loader transform it was re-read and re-formed for every n-block)
-        a = nat.BnBwdApply()
-        a.M, a.C, a.lddy, a.ldh, a.lddh = self.M_out, self.Cout, self.Cout, self.Cout, self.Cout
-        a.dy, a.h = dym.data_ptr(), self.h3.data_ptr()
-        a.ca, a.cb, a.cc = self.bn3.ca.data_ptr(), self.bn3.cb.data_ptr(), self.bn3.cc.data_ptr()
-        a.dh = self.dh3.data_ptr()
-        launch(lib.yamb_bn_bwd_apply_bwd, a, "bn3_bwd_apply", 6 * self.M_out * self.Cout)
+        _bn_bwd_apply(self.bn3, dym, self.h3, self.dh3, "bn3_bwd_apply")
         fork_ev = self._fork_event()
-        # 2. project dgrad: da2 = dh3 * W3, dz2 = da2 * act'(z2), BN2-backward statistics
-        g = nat.Gemm()
-        g.M, g.N, g.K = self.M_out, self.Chid, self.Cout
-        g.A, g.lda = self.dh3.data_ptr(), self.Cout
-        g.B, g.ldb, g.b_mn_major = self.w_proj_bf.data_ptr(), self.Chid, 1
-        g.D, g.ldd = self.dz2.data_ptr(), self.Chid
-        if self.se is not None:
-            # SE: the GEMM writes d(a2*gate); the gate / pooling gradients need a reduction over
-            # HW first, so act'/BN2-backward happen in se_bwd_apply afterwards
+        # 2. project dgrad: da2 = dh3 * W3, dz2 = da2 * act'(z2), BN2-backward statistics, which
+        #    the GEMM finalises for one BatchNorm module: one launch per branch slice.  With SE the
+        #    GEMM writes d(a2*gate) over all channels; the gate / pooling gradients need a
+        #    reduction over HW first, so act'/BN2-backward happen in se_bwd_apply afterwards
+        se = self.se is not None
+        for c0, cb in [(0, self.Chid)] if se else self.bn2.slices:
+            s = slice(c0, c0 + cb)
+            g = nat.Gemm()
+            g.M, g.N, g.K = self.M_out, cb, self.Cout
+            g.A, g.lda = self.dh3.data_ptr(), self.Cout
+            g.B, g.ldb, g.b_mn_major = self.w_proj_bf[:, s].data_ptr(), self.Chid, 1
+            g.D, g.ldd = self.dz2[:, s].data_ptr(), self.Chid
+            if not se:
+                g.epi = 1
+                g.H, g.ldh = self.h2[:, s].data_ptr(), self.Chid
+                g.h_scale, g.h_shift, g.h_act = _at(self.bn2.scale, c0), _at(self.bn2.shift, c0), \
+                    self.act
+                g.bn_bwd = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
             launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
-                   2 * self.M_out * (self.Cout + self.Chid),
-                   2 * self.M_out * self.Chid * self.Cout)
+                   2 * self.M_out * (self.Cout + (1 if se else 2) * cb),
+                   2 * self.M_out * cb * self.Cout)
+        if se:
             self._se_backward(grads)
-        else:
-            g.epi = 1
-            g.H, g.ldh = self.h2.data_ptr(), self.Chid
-            g.h_scale, g.h_shift, g.h_act = self.bn2.scale.data_ptr(), \
-                self.bn2.shift.data_ptr(), self.act
-            if len(self.bn2.mods) == 1:
-                g.bn_bwd = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"]))
-                launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
-                       2 * self.M_out * (self.Cout + 2 * self.Chid),
-                       2 * self.M_out * self.Chid * self.Cout)
-            else:
-                for (c0, cb) in self.bn2.slices:
-                    gs = nat.Gemm()
-                    C.memmove(C.byref(gs), C.byref(g), C.sizeof(nat.Gemm))
-                    gs.N = cb
-                    gs.B = g.B + c0 * 2
-                    gs.D = g.D + c0 * 2
-                    gs.H = g.H + c0 * 2
-                    gs.h_scale = g.h_scale + c0 * 4
-                    gs.h_shift = g.h_shift + c0 * 4
-                    gs.bn_bwd = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
-                    launch(lib.yamb_pointwise_gemm, gs, "pw_project_dgrad",
-                           2 * self.M_out * (self.Cout + 2 * cb),
-                           2 * self.M_out * cb * self.Cout)
         # 3. project wgrad: dW3[Cout,Chid] += dh3^T * a2
         g = nat.Gemm()
         g.M, g.N, g.K = self.Cout, self.Chid, self.M_out
@@ -940,32 +933,17 @@ class BlockPlan:
                         2 * self.M_out * (self.Cout + self.Chid),
                         2 * self.M_out * self.Chid * self.Cout, fork_ev, (self.dh3,))
         # 4. depthwise backward per branch
-        c0 = 0
-        for b, (cb, k) in enumerate(zip(self.channels, self.ks)):
-            d = nat.DwBwd()
-            d.N, d.H, d.W, d.C, d.ldc, d.k, d.stride = self.N, self.H, self.W, cb, self.Chid, k, \
-                self.stride
-            d.dz = self.dz2.data_ptr() + c0 * 2
-            d.h = self.h2.data_ptr() + c0 * 2
-            d.ca = self.bn2.ca.data_ptr() + c0 * 4
-            d.cb = self.bn2.cb.data_ptr() + c0 * 4
-            d.cc = self.bn2.cc.data_ptr() + c0 * 4
-            d.w = self.conv_dw[b].weight.data_ptr()
-            d.dw = grads["dw"][b].data_ptr()
+        for (c0, cb), conv, dw in zip(self.bn2.slices, self.conv_dw, grads["dw"]):
+            s = slice(c0, c0 + cb)
+            coef = (self.bn2.ca[s], self.bn2.cb[s], self.bn2.cc[s])
             if self.expand:
-                d.x = self.h1.data_ptr() + c0 * 2
-                d.in_scale = self.bn1.scale.data_ptr() + c0 * 4
-                d.in_shift = self.bn1.shift.data_ptr() + c0 * 4
-                d.in_act = self.act
-                d.dx = self.dz1.data_ptr() + c0 * 2
-                d.bn = C.pointer(self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb))
+                _dw_bwd(conv, (self.N, self.H, self.W), self.dz2[:, s], self.h2[:, s], coef, dw,
+                        self.h1[:, s], self.dz1[:, s], "dw_bwd",
+                        pre=(self.bn1.scale[s], self.bn1.shift[s], self.act),
+                        stats=self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb))
             else:
-                d.x = xm.data_ptr()
-                d.dx = dx.data_ptr()
-                d.residual = dym_skip.data_ptr() if self.residual else None
-            launch(lib.yamb_depthwise_bwd, d, "dw_bwd", 4 * cb * (self.M_in + self.M_out),
-                   4 * self.M_out * cb * k * k)
-            c0 += cb
+                _dw_bwd(conv, (self.N, self.H, self.W), self.dz2[:, s], self.h2[:, s], coef, dw,
+                        xm, dx, "dw_bwd", residual=dym_skip if self.residual else None)
         if not self.expand:
             return dx
         fork2_ev = self._fork_event()   # dz1 and the BN1-backward coefficients exist from here on
@@ -1019,7 +997,7 @@ MAX_PLANS_PER_BLOCK = 2   # e.g. the training batch and the validation / calibra
 
 
 def _plan_for(block, x):
-    """BlockPlan (intermediates + argument structs) of `block` for this input shape.  At most
+    """BlockPlan (kernel sequence + intermediates) of `block` for this input shape.  At most
     MAX_PLANS_PER_BLOCK shapes are kept per block, least recently used first out: a partial last
     batch or another evaluation resolution no longer pins a whole extra activation set for ever
     (ADVICE r1)."""
@@ -1334,11 +1312,7 @@ class _BnActFn(torch.autograd.Function):
             s.M, s.C, s.ldh, s.h, s.bn = M, Cc, Cc, hm.data_ptr(), C.pointer(b.fwd_struct(M))
             launch(lib.yamb_bn_stats_fwd, s, "bn_stats", 2 * M * Cc)
         y = torch.empty_like(h, memory_format=torch.channels_last)
-        a = nat.BnApply()
-        a.M, a.C, a.ldh, a.ldr, a.ldy = M, Cc, Cc, Cc, Cc
-        a.h, a.scale, a.shift, a.act = hm.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), act
-        a.y = y.data_ptr()
-        launch(lib.yamb_bn_apply_fwd, a, "bn_apply", 4 * M * Cc)
+        _bn_apply(b, hm, y, act, "bn_apply")
         ctx.bn, ctx.act, ctx.st = bn, act, st
         # per-call copy of [scale, shift, mean, invstd]: another forward through this module before
         # the backward (eval / calibration pass, gradient accumulation) must not change what the
@@ -1350,7 +1324,6 @@ class _BnActFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
-        lib = nat.lib()
         h, coef = ctx.saved_tensors
         bn, act, st = ctx.bn, ctx.act, ctx.st
         b = st.bn
@@ -1363,19 +1336,9 @@ class _BnActFn(torch.autograd.Function):
         gt = GradTargets((bn.weight, bn.bias))
         g = b.bwd_struct(M, [(gt.of(bn.weight), gt.of(bn.bias))])
         g.mean, g.invstd = c_mean, c_invstd      # this call's statistics, not the live buffers
-        r = nat.BnReduce()
-        r.M, r.C, r.lddy, r.ldh = M, Cc, Cc, Cc
-        r.dy, r.h, r.bn = dym.data_ptr(), hm.data_ptr(), C.pointer(g)
-        r.z_scale, r.z_shift, r.z_act = c_scale, c_shift, act
-        launch(lib.yamb_bn_reduce_bwd, r, "bn_reduce", 4 * M * Cc)
+        _bn_reduce(g, dym, hm, "bn_reduce", z=(c_scale, c_shift, act))
         dh = torch.empty_like(h, memory_format=torch.channels_last)
-        a = nat.BnBwdApply()
-        a.M, a.C, a.lddy, a.ldh, a.lddh = M, Cc, Cc, Cc, Cc
-        a.dy, a.h = dym.data_ptr(), hm.data_ptr()
-        a.z_scale, a.z_shift, a.z_act = c_scale, c_shift, act
-        a.ca, a.cb, a.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
-        a.dh = dh.data_ptr()
-        launch(lib.yamb_bn_bwd_apply_bwd, a, "bn_bwd_apply", 6 * M * Cc)
+        _bn_bwd_apply(b, dym, hm, dh, "bn_bwd_apply", z=(c_scale, c_shift, act))
         return (dh, None, None) + gt.result() + (None,)
 
 
@@ -1561,18 +1524,12 @@ def eval_forward(block, x):
         gate = torch.empty(N, Chid, device=dev, dtype=torch.float32)
         uv = torch.empty(2, N, R, device=dev, dtype=torch.float32)
         a.pooled = pooled.data_ptr()
-        launch(lib_fn("yamb_block_eval_pool_fwd"), a, "block_eval_pool",
+        launch(nat.lib().yamb_block_eval_pool_fwd, a, "block_eval_pool",
                *_block_eval_cost(block, x, Ho, Wo, False, project=False))
-        f = nat.SeFc()
-        f.N, f.C, f.R, f.act = N, Chid, R, act_code_of(se.active_fn)
-        f.pooled = pooled.data_ptr()
-        f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
-        f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
-        f.u, f.v, f.gate = uv[0].data_ptr(), uv[1].data_ptr(), gate.data_ptr()
-        launch(lib_fn("yamb_se_fc_fwd"), f, "se_fc", 4 * N * Chid * 2, 4 * N * Chid * R)
+        _se_fc(se, pooled, uv[0], uv[1], gate)
         a.pooled = None
         a.gate = gate.data_ptr()
-    launch(lib_fn("yamb_block_eval_fwd"), a, "block_eval",
+    launch(nat.lib().yamb_block_eval_fwd, a, "block_eval",
            *_block_eval_cost(block, x, Ho, Wo, residual))
     if tail is not None:
         xm = x.permute(0, 2, 3, 1).reshape(N * H * W, Cin)    # view, NHWC matrix
