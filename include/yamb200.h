@@ -362,10 +362,12 @@ int yamb_instance_norm_fwd(const yamb_in_fwd* args, yamb_stream_t stream);
 int yamb_instance_norm_bwd(const yamb_in_bwd* args, yamb_stream_t stream);
 
 /* ---- stem convolution -----------------------------------------------------------------------------
- * 3x3, stride 2, pad 1, 3 input channels -> Cout (multiple of 8, <= 64) on NHWC bf16: the first
- * layer of the network (reference models/mobilenet_supernet.py:124-130; its BatchNorm + activation
- * follow through yamb_bn_stats_fwd / yamb_bn_apply_fwd).  Weights fp32 in the parameter's own
- * [Cout][3][3][3] layout.  fwd writes y; wgrad ACCUMULATES dw += sum dh * x (no input gradient). */
+ * 3x3, stride 2, pad 1, 3 input channels -> Cout on NHWC bf16: the first layer of the network
+ * (reference models/mobilenet_supernet.py:124-130; its BatchNorm + activation follow through
+ * yamb_bn_stats_fwd / yamb_bn_apply_fwd).  Weights fp32 in the parameter's own [Cout][3][3][3]
+ * layout.  fwd writes y (16-byte aligned), Cout a multiple of 8, <= 64; wgrad ACCUMULATES
+ * dw += sum dh * x (dh 16-byte aligned; no input gradient), Cout in {8, 16, 32, 64}.  Other
+ * arguments return YAMB_EINVAL, with or without a device. */
 typedef struct yamb_stem_conv {
   int32_t N, H, W, Cout;
   const void* x;        /* bf16 [N][H][W][3] */
@@ -420,7 +422,9 @@ int yamb_head_pool_eval_fwd(const yamb_head_pool_eval* args, yamb_stream_t strea
  *             correct1/5[n] in {0,1} (ties like torch.topk: lower index wins);
  *             G[n][c] = softmax - t (bf16), what the backward needs
  *   backward: dlogits[n][c] = G[n][c] * dloss[n];  dbias[c] += sum_n dlogits[n][c] (classifier
- *             bias gradient, optional) */
+ *             bias gradient, optional)
+ * forward: C <= 4096, ld >= C, ldg >= C; backward: C, ldg, ldd even and >= C, G / dlogits 4-byte
+ * aligned.  Other arguments return YAMB_EINVAL, with or without a device. */
 typedef struct yamb_softmax_ce {
   int32_t N, C; int64_t ld;
   const void* logits;          /* bf16 [N][ld] */
@@ -442,7 +446,7 @@ typedef struct yamb_softmax_ce_grad {
 int yamb_softmax_ce_fwd(const yamb_softmax_ce* args, yamb_stream_t stream);
 int yamb_softmax_ce_bwd(const yamb_softmax_ce_grad* args, yamb_stream_t stream);
 /* out[c] += sum_rows X[row][c] over a bf16 [M][ld] matrix (bias gradient of the classifier,
- * reference models/mobilenet_supernet.py:163-167) */
+ * reference models/mobilenet_supernet.py:163-167); C and ld >= C even, X 4-byte aligned */
 int yamb_colsum_bf16(const void* X, int64_t M, int32_t C, int64_t ld, float* out,
                      yamb_stream_t stream);
 

@@ -113,8 +113,10 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* X
 }
 
 int colsum_bf16_launch(const void* X, long long M, int C, long long ld, float* out, cudaStream_t st) {
-  if (!X || !out || M <= 0 || C <= 0 || (C % 2) || (ld % 2))
-    return set_error(YAMB_EINVAL, "colsum args (C and ld must be even)");
+  // column pairs are read as 32-bit words
+  if (!X || !out || M <= 0 || C <= 0 || (C % 2) || (ld % 2) || ld < C ||
+      (reinterpret_cast<uintptr_t>(X) & 3))
+    return set_error(YAMB_EINVAL, "colsum args (C and ld >= C must be even, X 4-byte aligned)");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   dim3 grid((C / 2 + 255) / 256, (unsigned)(M < 32 ? M : 32));
   float* part = nullptr;
@@ -141,9 +143,12 @@ int softmax_ce_fwd_launch(const yamb_softmax_ce* a, cudaStream_t st) {
 }
 
 int softmax_ce_bwd_launch(const yamb_softmax_ce_grad* a, cudaStream_t st) {
+  // G and dlogits are read and written as 32-bit column pairs
   if (!a || a->N <= 0 || a->C <= 0 || (a->C % 2) || (a->ldg % 2) || (a->ldd % 2) || !a->G ||
-      !a->dloss || !a->dlogits)
-    return set_error(YAMB_EINVAL, "softmax_ce bwd args (C and pitches must be even)");
+      !a->dloss || !a->dlogits || a->ldg < a->C || a->ldd < a->C ||
+      ((reinterpret_cast<uintptr_t>(a->G) | reinterpret_cast<uintptr_t>(a->dlogits)) & 3))
+    return set_error(YAMB_EINVAL,
+                     "softmax_ce bwd args (C and pitches >= C must be even, G / dlogits 4-byte aligned)");
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   int grid = a->N < 2 * max_ctas() ? a->N : 2 * max_ctas();
   float* part = nullptr;

@@ -282,12 +282,13 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__
   }
 }
 
+// Shape checks and the tile plan; touches no device.  Every launcher finishes its own argument
+// checks before it looks for a device, so a malformed call is YAMB_EINVAL with or without one.
 static int stem_fill(const yamb_stem_conv* a, StemDev& p) {
   if (!a || a->N <= 0 || a->H <= 0 || a->W <= 0 || !a->x)
     return set_error(YAMB_EINVAL, "stem conv: bad arguments");
   if (a->Cout <= 0 || a->Cout > 64 || (a->Cout % 8))
     return set_error(YAMB_EINVAL, "stem conv: Cout=%d must be a multiple of 8, <= 64", a->Cout);
-  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   p.N = a->N; p.H = a->H; p.W = a->W; p.Cout = a->Cout;
   p.Ho = (a->H - 1) / 2 + 1; p.Wo = (a->W - 1) / 2 + 1;
   p.x = (const __nv_bfloat16*)a->x; p.w = a->w; p.y = (__nv_bfloat16*)a->y;
@@ -320,6 +321,7 @@ int stem_conv_fwd_launch(const yamb_stem_conv* a, cudaStream_t st) {
   if (rc) return rc;
   if (!a->w || !a->y || (reinterpret_cast<uintptr_t>(a->y) & 15))
     return set_error(YAMB_EINVAL, "stem conv fwd: w / y (16-byte aligned) required");
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   p.scale = p.shift = nullptr;
   p.act = 0;
   return stem_fwd_run<false>(p, a->Cout, st);
@@ -335,6 +337,7 @@ int stem_conv_eval_fwd_launch(const yamb_stem_conv_eval* a, cudaStream_t st) {
     return set_error(YAMB_EINVAL, "stem conv eval: w / y (16-byte aligned) / scale / shift required");
   if (a->act < YAMB_ACT_NONE || a->act > YAMB_ACT_HSWISH)
     return set_error(YAMB_EINVAL, "stem conv eval: act=%d", a->act);
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   p.scale = a->scale;
   p.shift = a->shift;
   p.act = a->act;
@@ -347,7 +350,8 @@ int stem_conv_wgrad_launch(const yamb_stem_conv* a, cudaStream_t st) {
   if (rc) return rc;
   if (!a->dh || !a->dw || (reinterpret_cast<uintptr_t>(a->dh) & 15))
     return set_error(YAMB_EINVAL, "stem conv wgrad: dh (16-byte aligned) / dw required");
-  if (256 % (a->Cout / 8 * 8)) return set_error(YAMB_EINVAL, "stem conv wgrad: Cout must be 8, 16, 32 or 64");
+  if (256 % a->Cout) return set_error(YAMB_EINVAL, "stem conv wgrad: Cout must be 8, 16, 32 or 64");
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   const size_t smem = (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
                       (size_t)kStemTH * kStemTW * a->Cout * 2;
   // the grid sets the number of partial slabs and so the order of their sum: it comes from the
