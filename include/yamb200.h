@@ -395,6 +395,22 @@ typedef struct yamb_stem_conv_eval {
 
 int yamb_stem_conv_eval_fwd(const yamb_stem_conv_eval* args, yamb_stream_t stream);
 
+/* The three stem entry points on uint8 images: x is uint8 [N][H][W][3] (HWC bytes, as a decoded
+ * RGB image), normalised while the kernel stages it, with the fp32 operations and rounding of
+ * torchvision's ToTensor() + Normalize(mean, std) followed by the bf16 rounding:
+ *   x_staged = bf16(((float)u / 255 - mean[c]) / std[c])   inside the image, 0 in the padding.
+ * Each entry computes the bits its bf16 twin computes on that normalised image.  Shapes, y, dh, dw
+ * and ev.scale / ev.shift / ev.act (eval entry only) as the bf16 entries; a non-finite mean, or a
+ * std that is zero or not finite, returns YAMB_EINVAL. */
+typedef struct yamb_stem_conv_u8 {
+  yamb_stem_conv_eval ev;    /* ev.conv.x: uint8 [N][H][W][3]; ev.scale/shift/act: eval entry only */
+  float mean[3], std[3];     /* staged x = bf16(((float)u / 255 - mean[c]) / std[c]), 0 outside */
+} yamb_stem_conv_u8;
+
+int yamb_stem_conv_u8_fwd(const yamb_stem_conv_u8* args, yamb_stream_t stream);
+int yamb_stem_conv_u8_wgrad(const yamb_stem_conv_u8* args, yamb_stream_t stream);
+int yamb_stem_conv_u8_eval_fwd(const yamb_stem_conv_u8* args, yamb_stream_t stream);
+
 /* ---- eval-mode head: 1x1 ConvBNReLU + full-extent average pool, ONE launch ------------------------
  * Replaces, in eval mode, the head ConvBNReLU (reference models/mobilenet_supernet.py:152-158) and
  * the AvgPool2d over the whole final feature map (:159):
@@ -546,7 +562,8 @@ int yamb_max_ctas(void);
  * 6 bn_reduce, 7 se_pool, 8 rmsprop, 9 se_bwd_reduce, 10 se_bwd_apply, 11 bn_stats,
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
  * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
- * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info) so bindings can self-check */
+ * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8) so bindings can
+ * self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

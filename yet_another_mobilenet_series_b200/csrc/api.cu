@@ -139,6 +139,7 @@ int yamb_struct_size(int which) {
     case 25: return (int)sizeof(yamb_stem_conv_eval);
     case 26: return (int)sizeof(yamb_head_pool_eval);
     case 27: return (int)sizeof(yamb_gemm_plan_info);
+    case 28: return (int)sizeof(yamb_stem_conv_u8);
     default: return -1;
   }
 }
@@ -171,6 +172,9 @@ int yamb_colsum_bf16(const void* X, int64_t M, int32_t C, int64_t ld, float* out
 int yamb_stem_conv_fwd(const yamb_stem_conv* a, yamb_stream_t s) { return yamb::stem_conv_fwd_launch(a, YAMB_ST(s)); }
 int yamb_stem_conv_wgrad(const yamb_stem_conv* a, yamb_stream_t s) { return yamb::stem_conv_wgrad_launch(a, YAMB_ST(s)); }
 int yamb_stem_conv_eval_fwd(const yamb_stem_conv_eval* a, yamb_stream_t s) { return yamb::stem_conv_eval_fwd_launch(a, YAMB_ST(s)); }
+int yamb_stem_conv_u8_fwd(const yamb_stem_conv_u8* a, yamb_stream_t s) { return yamb::stem_conv_u8_fwd_launch(a, YAMB_ST(s)); }
+int yamb_stem_conv_u8_wgrad(const yamb_stem_conv_u8* a, yamb_stream_t s) { return yamb::stem_conv_u8_wgrad_launch(a, YAMB_ST(s)); }
+int yamb_stem_conv_u8_eval_fwd(const yamb_stem_conv_u8* a, yamb_stream_t s) { return yamb::stem_conv_u8_eval_fwd_launch(a, YAMB_ST(s)); }
 int yamb_head_pool_eval_fwd(const yamb_head_pool_eval* a, yamb_stream_t s) { return yamb::head_pool_eval_launch(a, YAMB_ST(s)); }
 int yamb_nl_gram_fwd(const yamb_nl_gram* a, yamb_stream_t s) { return yamb::nl_gram_launch(a, YAMB_ST(s)); }
 int yamb_nl_rowmat_fwd(const yamb_nl_rowmat* a, yamb_stream_t s) { return yamb::nl_rowmat_launch(a, YAMB_ST(s)); }

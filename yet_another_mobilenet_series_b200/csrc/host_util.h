@@ -46,6 +46,9 @@ int colsum_bf16_launch(const void* X, long long M, int C, long long ld, float* o
 int stem_conv_fwd_launch(const yamb_stem_conv* a, cudaStream_t stream);
 int stem_conv_wgrad_launch(const yamb_stem_conv* a, cudaStream_t stream);
 int stem_conv_eval_fwd_launch(const yamb_stem_conv_eval* a, cudaStream_t stream);
+int stem_conv_u8_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
+int stem_conv_u8_wgrad_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
+int stem_conv_u8_eval_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
 int head_pool_eval_launch(const yamb_head_pool_eval* a, cudaStream_t stream);
 int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t stream);
 int nl_rowmat_launch(const yamb_nl_rowmat* a, cudaStream_t stream);

@@ -11,8 +11,61 @@ Differences from the reference, all on the device side:
   * two device buffers are recycled instead of allocating a new tensor per batch, and an event
     (not a whole-stream wait) guards their reuse.
 `TrainStep.load` is the same mechanism for a single static buffer (CUDA-graph replay).
+
+uint8 input (the batches of NVIDIA apex's ImageNet example, the origin of the reference's
+prefetcher): `fast_collate` packs decoded images as uint8 NCHW batches with channels_last storage,
+`DataPrefetcher(loader, dtype=torch.uint8)` uploads them byte for byte (a quarter of the fp32
+bytes), and a model given `set_input_norm(model, mean, std)` normalises them inside its stem
+convolution kernels, to the bits `ToTensor()` + `Normalize(mean, std)` give on the host.
 """
+import math
+
+import numpy as np
 import torch
+
+
+def set_input_norm(model, mean, std):
+    """Attach the `Normalize(mean, std)` of the input pipeline to `model` (the module whose forward
+    runs the network, not a DDP wrapper): a uint8 image batch passed to it is then normalised by
+    its stem kernels.  A plain attribute, not a buffer: state_dict() keys stay those of the
+    reference, and copy.deepcopy (TrainStep.ema_model) carries it."""
+    mean = tuple(float(v) for v in mean)
+    std = tuple(float(v) for v in std)
+    if len(mean) != 3 or len(std) != 3:
+        raise ValueError("set_input_norm: mean and std need 3 values (RGB), got %r, %r" % (mean, std))
+    if not all(math.isfinite(v) for v in mean + std) or any(v == 0.0 for v in std):
+        raise ValueError("set_input_norm: mean and std must be finite and std non-zero: %r, %r"
+                         % (mean, std))
+    model.input_norm = (mean, std)
+    return model
+
+
+def input_norm_of(model):
+    """The (mean, std) set_input_norm attached to `model`, or None."""
+    return getattr(model, "input_norm", None)
+
+
+def fast_collate(batch):
+    """collate_fn for a DataLoader whose transforms end before `ToTensor()`: a list of
+    (PIL RGB image or uint8 HWC array, target) -> (uint8 [N, 3, H, W] with channels_last storage,
+    int64 [N]).  Each image is copied once, into one buffer, pinned when CUDA is available and
+    the call runs in the main process (in DataLoader workers, use `pin_memory=True`: pinning
+    there would initialise CUDA in a forked process)."""
+    imgs = [np.asarray(img, dtype=np.uint8) for img, _ in batch]
+    if not imgs:
+        raise ValueError("fast_collate: empty batch")
+    H, W = imgs[0].shape[:2]
+    for a in imgs:
+        if a.shape != (H, W, 3):
+            raise ValueError("fast_collate: images must be RGB of one size, %r vs %r"
+                             % (a.shape, (H, W, 3)))
+    pin = torch.cuda.is_available() and torch.utils.data.get_worker_info() is None
+    out = torch.empty((len(imgs), H, W, 3), dtype=torch.uint8, pin_memory=pin)
+    dst = out.numpy()
+    for i, a in enumerate(imgs):
+        dst[i] = a
+    target = torch.tensor([int(t) for _, t in batch], dtype=torch.int64)
+    return out.permute(0, 3, 1, 2), target
 
 
 class DataPrefetcher:

@@ -11,6 +11,7 @@ from torch import nn
 
 from .mobilenet_base import ConvBNReLU, _make_divisible, get_active_fn, get_block
 from . import engine
+from .dataflow import input_norm_of
 
 __all__ = ["MobileNetV2"]
 
@@ -51,16 +52,25 @@ def _full_extent(pool, x):
 
 
 def run_features(model, x):
-    """Shared forward of both builders: bf16 channels_last through stem, blocks, head, pool."""
+    """Shared forward of both builders: bf16 channels_last through stem, blocks, head, pool.  A
+    uint8 image on a model with an input normalisation (dataflow.set_input_norm) goes to the stem
+    as it is; the stem normalises it."""
     if x.is_cuda:
         from . import tail_ops
-        x = engine.to_nhwc_bf16(x)
+        norm = input_norm_of(model) if x.dtype == torch.uint8 else None
+        if norm is None:
+            x = engine.to_nhwc_bf16(x)
+        else:
+            x = x.contiguous(memory_format=torch.channels_last)
         layers = list(model.features)
         with torch.autocast("cuda", dtype=torch.bfloat16):
             skip = False
             for i, layer in enumerate(layers):
                 if skip:
                     skip = False
+                    continue
+                if i == 0 and norm is not None:
+                    x = tail_ops.stem_u8(layer, x, norm)
                     continue
                 nxt = layers[i + 1] if i + 1 < len(layers) else None
                 if (engine.EVAL_TAIL_FUSED and isinstance(layer, ConvBNReLU)

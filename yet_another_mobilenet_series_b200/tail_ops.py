@@ -281,25 +281,53 @@ def softmax_ce(logits, target, smoothing):
 
 
 # ---- stem ----------------------------------------------------------------------------------------
+# `norm` = ((mean x 3), (std x 3)) marks a uint8 image: x is uint8 [N, 3, H, W] channels_last, and
+# the yamb_stem_conv_u8_* entries normalise it inside the kernels, with the bits of torchvision's
+# ToTensor() + Normalize() on the host followed by the bf16 cast (no normalised tensor in HBM).
+def _stem_args(norm, eval_args=False):
+    """(argument struct, its yamb_stem_conv part, its yamb_stem_conv_eval part or None) of a call
+    on a bf16 x (`norm` None) or a uint8 x."""
+    if norm is None:
+        if eval_args:
+            a = nat.StemConvEval()
+            return a, a.conv, a
+        a = nat.StemConv()
+        return a, a, None
+    a = nat.StemConvU8()
+    a.mean[:] = norm[0]
+    a.std[:] = norm[1]
+    return a, a.ev.conv, a.ev
+
+
+def _stem_bytes(x, Ho, Wo, Cout):
+    N, _, H, W = x.shape
+    return N * (H * W * 3 * x.element_size() + 2 * Ho * Wo * Cout)
+
+
 class _StemConvFn(torch.autograd.Function):
     """Raw output of the 3x3 / stride-2 / 3-channel first convolution (reference
     models/mobilenet_supernet.py:124-130) by the direct kernels of csrc/stem.cu; weight gradient
     in backward, no input gradient."""
 
     @staticmethod
-    def forward(ctx, x, conv, weight):
+    def forward(ctx, x, conv, norm, weight):
         lib = nat.lib()
         N, _, H, W = x.shape
         Cout = conv.out_channels
         Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
         y = torch.empty((N, Cout, Ho, Wo), device=x.device, dtype=torch.bfloat16,
                         memory_format=torch.channels_last)
-        a = nat.StemConv()
-        a.N, a.H, a.W, a.Cout = N, H, W, Cout
-        a.x, a.w, a.y = x.data_ptr(), conv.weight.data_ptr(), y.data_ptr()
-        engine.launch(lib.yamb_stem_conv_fwd, a, "stem_conv_fwd",
-                      2 * N * (H * W * 3 + Ho * Wo * Cout), 2 * N * Ho * Wo * Cout * 27)
+        a, c, _ = _stem_args(norm)
+        c.N, c.H, c.W, c.Cout = N, H, W, Cout
+        c.x, c.w, c.y = x.data_ptr(), conv.weight.data_ptr(), y.data_ptr()
+        if norm is None:
+            engine.launch(lib.yamb_stem_conv_fwd, a, "stem_conv_fwd",
+                          _stem_bytes(x, Ho, Wo, Cout), 2 * N * Ho * Wo * Cout * 27)
+        else:
+            engine.launch(lib.yamb_stem_conv_u8_fwd, a, "stem_conv_u8_fwd",
+                          _stem_bytes(x, Ho, Wo, Cout), 2 * N * Ho * Wo * Cout * 27)
         ctx.conv = conv
+        ctx.norm = norm
         ctx.save_for_backward(x)
         return y
 
@@ -312,13 +340,17 @@ class _StemConvFn(torch.autograd.Function):
         N, _, H, W = x.shape
         Cout = conv.out_channels
         gt = engine.GradTargets((conv.weight,))
-        a = nat.StemConv()
-        a.N, a.H, a.W, a.Cout = N, H, W, Cout
-        a.x, a.dh, a.dw = x.data_ptr(), dh.data_ptr(), gt.of(conv.weight).data_ptr()
-        engine.launch(lib.yamb_stem_conv_wgrad, a, "stem_conv_wgrad",
-                      2 * N * (H * W * 3 + dh.shape[2] * dh.shape[3] * Cout),
-                      2 * N * dh.shape[2] * dh.shape[3] * Cout * 27)
-        return (None, None) + gt.result()
+        a, c, _ = _stem_args(ctx.norm)
+        c.N, c.H, c.W, c.Cout = N, H, W, Cout
+        c.x, c.dh, c.dw = x.data_ptr(), dh.data_ptr(), gt.of(conv.weight).data_ptr()
+        Ho, Wo = dh.shape[2], dh.shape[3]
+        if ctx.norm is None:
+            engine.launch(lib.yamb_stem_conv_wgrad, a, "stem_conv_wgrad",
+                          _stem_bytes(x, Ho, Wo, Cout), 2 * N * Ho * Wo * Cout * 27)
+        else:
+            engine.launch(lib.yamb_stem_conv_u8_wgrad, a, "stem_conv_u8_wgrad",
+                          _stem_bytes(x, Ho, Wo, Cout), 2 * N * Ho * Wo * Cout * 27)
+        return (None, None, None) + gt.result()
 
 
 def stem_supported(mod, x):
@@ -331,22 +363,25 @@ def stem_supported(mod, x):
             and type(act).__name__ in ("ReLU", "ReLU6", "Swish", "HSwish", "Identity"))
 
 
-def stem_conv_bn_act(mod, x):
+def stem_conv_bn_act(mod, x, norm=None):
     """ConvBNReLU(3, C, stride=2) on CUDA: direct convolution kernel -> BatchNorm statistics ->
-    BatchNorm apply + activation (engine.bn_act_apply)."""
-    x = engine.to_nhwc_bf16(x)
+    BatchNorm apply + activation (engine.bn_act_apply).  With `norm`, x is a uint8 image the
+    kernels normalise."""
+    if norm is None:
+        x = engine.to_nhwc_bf16(x)
     conv, bn, act = mod[0], mod[1], mod[2]
     if _tail_eval_wanted(bn):
-        y = _stem_eval(conv, bn, act, x)
+        y = _stem_eval(conv, bn, act, x, norm)
         if y is not None:
             return y
-    h = _StemConvFn.apply(x, conv, conv.weight)
+    h = _StemConvFn.apply(x, conv, norm, conv.weight)
     return engine.bn_act_apply(bn, act, h)
 
 
-def _stem_eval(conv, bn, act, x):
-    """Eval-mode stem in one launch (yamb_stem_conv_eval_fwd), bitwise equal to the stem kernel
-    followed by bn_act_apply; None when the kernel declines the shape."""
+def _stem_eval(conv, bn, act, x, norm=None):
+    """Eval-mode stem in one launch (yamb_stem_conv_eval_fwd, or yamb_stem_conv_u8_eval_fwd on a
+    uint8 x), bitwise equal to the stem kernel followed by bn_act_apply; None when the kernel
+    declines the shape."""
     N, _, H, W = x.shape
     Cout = conv.out_channels
     Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
@@ -355,12 +390,39 @@ def _stem_eval(conv, bn, act, x):
         b.eval_coeffs()
     y = torch.empty((N, Cout, Ho, Wo), device=x.device, dtype=torch.bfloat16,
                     memory_format=torch.channels_last)
-    a = nat.StemConvEval()
-    a.conv.N, a.conv.H, a.conv.W, a.conv.Cout = N, H, W, Cout
-    a.conv.x, a.conv.w, a.conv.y = x.data_ptr(), conv.weight.data_ptr(), y.data_ptr()
-    a.scale, a.shift, a.act = b.scale.data_ptr(), b.shift.data_ptr(), engine.act_code_of(act)
-    if not engine.try_launch(nat.lib().yamb_stem_conv_eval_fwd, a, "stem_conv_eval",
-                             2 * N * (H * W * 3 + Ho * Wo * Cout), 2 * N * Ho * Wo * Cout * 27):
+    a, c, e = _stem_args(norm, eval_args=True)
+    c.N, c.H, c.W, c.Cout = N, H, W, Cout
+    c.x, c.w, c.y = x.data_ptr(), conv.weight.data_ptr(), y.data_ptr()
+    e.scale, e.shift, e.act = b.scale.data_ptr(), b.shift.data_ptr(), engine.act_code_of(act)
+    fn = nat.lib().yamb_stem_conv_eval_fwd if norm is None else nat.lib().yamb_stem_conv_u8_eval_fwd
+    if not engine.try_launch(fn, a, "stem_conv_eval", _stem_bytes(x, Ho, Wo, Cout),
+                             2 * N * Ho * Wo * Cout * 27):
         return None
     engine.EVAL_TAIL_CALLS += 1
     return y
+
+
+_NORM_TENSORS = {}
+
+
+def normalize_u8(x, norm):
+    """uint8 [N, 3, H, W] -> bf16 channels_last ((x / 255 - mean) / std), with the fp32 operations
+    and rounding of torchvision's ToTensor() + Normalize() on the host, then the bf16 cast: the
+    input of a stem the direct kernels do not cover.  Every divisor is a device tensor: CUDA torch
+    may turn a division by a Python scalar into a multiply by its reciprocal, other bits."""
+    key = (norm, x.device)
+    t = _NORM_TENSORS.get(key)
+    if t is None:       # built on the first (eager) call, so a graph capture later copies nothing
+        mk = lambda v: torch.tensor(v, dtype=torch.float32, device=x.device).view(1, 3, 1, 1)
+        t = _NORM_TENSORS[key] = (mk((255.0,) * 3), mk(norm[0]), mk(norm[1]))
+    y = x.float().div_(t[0]).sub_(t[1]).div_(t[2])
+    return y.to(dtype=torch.bfloat16, memory_format=torch.channels_last)
+
+
+def stem_u8(mod, x, norm):
+    """The first layer of a network fed a uint8 image `x` (channels_last) with normalisation
+    `norm`: the uint8 stem kernels when they cover the layer, else the layer on the image
+    normalised on the device (normalize_u8)."""
+    if isinstance(mod, torch.nn.Sequential) and len(mod) == 3 and stem_supported(mod, x):
+        return stem_conv_bn_act(mod, x, norm)
+    return mod(normalize_u8(x, norm))

@@ -18,12 +18,17 @@ The other half of an epoch, the reference's `validate()` (train.py:273-309), is
 `TrainStep.validate`: `ema_model()` (get_ema_model, common.py:155-172) -> `EvalStep.calibrate`
 (bn_calibration, utils/common.py:175-187) -> `EvalStep.evaluate` (forward_loss, common.py:67-80,
 with the metrics summed on the device).
+
+Both steps take uint8 image batches (`input_dtype=torch.uint8, input_norm=(mean, std)`, e.g. from
+`dataflow.fast_collate`): the static buffers are then uint8 channels_last, `load` is a plain H2D
+copy of a quarter of the fp32 bytes, and the stem kernels apply ToTensor() + Normalize(mean, std).
 """
 import copy
 
 import torch
 import torch.distributed as dist
 
+from . import dataflow
 from . import distributed as udist
 from . import engine
 from . import tail_ops
@@ -42,9 +47,13 @@ class TrainStep:
     def __init__(self, model, per_gpu_batch, image_size=224, base_lr=0.016, base_total_batch=256,
                  alpha=0.9, momentum=0.9, eps=1e-3, weight_decay=1e-5, label_smoothing=0.1,
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
-                 optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas"):
+                 optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
+                 input_norm=None):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
-        `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both."""
+        `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
+        `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
+        there); it is attached to the model (dataflow.set_input_norm)."""
+        _attach_input_norm(model, input_dtype, input_norm)
         self.model = model
         dev = next(model.parameters()).device
         if dev.type != "cuda":
@@ -199,11 +208,20 @@ class TrainStep:
         if self._eval_step is None:
             self._eval_step = EvalStep(model, self.batch, image_size=self.x.shape[-1],
                                        calib_batch=calib_batch, use_graph=self.use_graph,
-                                       input_dtype=self.x.dtype)
+                                       input_dtype=self.x.dtype,
+                                       input_norm=dataflow.input_norm_of(self.model))
         es = self._eval_step
         if calib_batches is not None:
             es.calibrate(calib_batches, calib_steps)
         return es.evaluate(val_batches)
+
+
+def _attach_input_norm(model, input_dtype, input_norm):
+    if input_dtype == torch.uint8 and input_norm is None:
+        raise ValueError("uint8 input needs input_norm=(mean, std): the Normalize() of the "
+                         "input pipeline, applied by the stem kernels")
+    if input_norm is not None:
+        dataflow.set_input_norm(model, *input_norm)
 
 
 def metrics_from_sums(loss_sum, correct1, correct5, count):
@@ -247,7 +265,8 @@ class EvalStep:
     SUM at the end when the world is larger than one."""
 
     def __init__(self, model, per_gpu_batch, image_size=224, calib_batch=None, use_graph=True,
-                 input_dtype=torch.bfloat16, optimizer=None):
+                 input_dtype=torch.bfloat16, optimizer=None, input_norm=None):
+        _attach_input_norm(model, input_dtype, input_norm)
         dev = next(model.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("EvalStep needs the model on a CUDA device (no CPU path)")
@@ -305,7 +324,12 @@ class EvalStep:
         """One batch: a graph replay when it has the phase's full shape, else eagerly."""
         ph = self.phases[phase]
         if tuple(x.shape) != tuple(ph.x.shape):
-            body(engine.to_nhwc_bf16(x.to(self.dev, non_blocking=True)), t)
+            x = x.to(self.dev, non_blocking=True)
+            if ph.x.dtype == torch.uint8:       # the stem normalises it
+                x = x.contiguous(memory_format=torch.channels_last)
+            else:
+                x = engine.to_nhwc_bf16(x)
+            body(x, t)
             return
         self.load(x, t, phase)
         self._publish(ph)
