@@ -59,6 +59,14 @@ def l2_mask(named_params, method):
     raise ValueError("Unknown weight_decay method: {}".format(method))
 
 
+def ema_momentum(decay, num_updates):
+    """EMA momentum of update `num_updates`: min(decay, (1+t)/(10+t)) (reference
+    utils/optim.py:56-64); `decay` itself when `num_updates` is None."""
+    if num_updates is None:
+        return decay
+    return min(decay, (1.0 + num_updates) / (10.0 + num_updates))
+
+
 class FlatArenaOptimizer(Optimizer):
     """`torch.optim.Optimizer` whose parameters, gradients and state live in flat fp32 arenas."""
 
@@ -180,6 +188,47 @@ class FlatArenaOptimizer(Optimizer):
         o = A["offs"][i]
         return A["ema"][o:o + p.numel()].view(p.shape)
 
+    def load_in_place(self, state_dict, ema=None):
+        """`load_state_dict` into the CURRENT arenas: hyper-parameters and per-parameter state are
+        copied into the existing views, and `ema` (tensors in parameter order, e.g. the shadows of
+        a checkpoint) into the EMA arena.  No arena is rebuilt, so the addresses a captured CUDA
+        graph holds stay valid.  State a parameter has no entry for in `state_dict` is zeroed, as
+        in a fresh arena."""
+        A = self.arenas()
+        saved = state_dict["param_groups"]
+        if len(saved) != len(self.param_groups) or \
+                any(len(g["params"]) != len(s["params"]) for g, s in zip(self.param_groups, saved)):
+            raise ValueError("loaded state dict has a different parameter layout than the optimizer")
+        index = {id(p): i for g, s in zip(self.param_groups, saved)
+                 for p, i in zip(g["params"], s["params"])}
+        for g, s in zip(self.param_groups, saved):
+            g.update({k: v for k, v in s.items() if k != "params"})
+        with torch.no_grad():
+            for p, o in zip(A["plist"], A["offs"]):
+                old = state_dict["state"].get(index[id(p)], {})
+                st = self._link_state(A, p, old, o)
+                for k, v in st.items():
+                    if torch.is_tensor(v) and k not in old:
+                        v.zero_()
+                if st:
+                    self.state[p] = st
+                else:
+                    self.state.pop(p, None)
+            if ema is not None:
+                if A["ema"] is None:
+                    raise ValueError("load_in_place: this optimizer keeps no EMA (attach_ema)")
+                shadows = list(ema)
+                if len(shadows) != len(A["plist"]):
+                    raise ValueError("load_in_place: %d EMA shadows for %d parameters"
+                                     % (len(shadows), len(A["plist"])))
+                for p, o, s in zip(A["plist"], A["offs"], shadows):
+                    A["ema"][o:o + p.numel()].view(p.shape).copy_(s)
+        self._state_loaded(A)
+
+    def _state_loaded(self, A):
+        """Hook: host-side bookkeeping derived from `self.state` is stale (load_in_place)."""
+        A["frozen"] = None
+
     def zero_grad(self, set_to_none=True):
         """Zero the flat gradient arena; the `.grad` views are kept (setting them to None would
         detach the parameters from the arena the kernels accumulate into)."""
@@ -233,9 +282,15 @@ class FlatArenaOptimizer(Optimizer):
         return A["frozen"][1], set(inactive)
 
     def load_state_dict(self, state_dict):
+        """torch's load_state_dict, then the loaded state is linked into fresh arenas.  The EMA of
+        the weights is not part of an optimizer state_dict: the shadows are carried over (use
+        `load_in_place` to load them too and keep the arenas)."""
+        old = self._arenas
         super().load_state_dict(state_dict)
         self._arenas = None  # re-link loaded state tensors into fresh arenas on next use
-        self.arenas()
+        A = self.arenas()
+        if old is not None and old["ema"] is not None and A["ema"] is not None:
+            A["ema"].copy_(old["ema"])
 
     # ---- the step ------------------------------------------------------------------------------
     def set_hyper_device(self, lr, ema_m):
@@ -243,8 +298,7 @@ class FlatArenaOptimizer(Optimizer):
         self._hyper.copy_(torch.tensor([lr, ema_m], dtype=torch.float32), non_blocking=True)
 
     def ema_momentum(self, num_updates):
-        d = self._ema_decay
-        return d if num_updates is None else min(d, (1.0 + num_updates) / (10.0 + num_updates))
+        return ema_momentum(self._ema_decay, num_updates)
 
     @torch.no_grad()
     def step(self, closure=None, num_updates=None, use_device_hyper=False):

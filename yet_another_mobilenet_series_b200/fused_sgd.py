@@ -83,6 +83,10 @@ class SGD(FlatArenaOptimizer):
         # torch creates the buffer as a copy of the gradient on the parameter's first step
         return [(i, MASK_FIRST_MOMENTUM) for i in A["fresh"] if i not in inactive]
 
+    def _state_loaded(self, A):
+        super()._state_loaded(A)
+        A["fresh"] = None   # which parameters have a momentum buffer may have changed
+
     # ---- the step ------------------------------------------------------------------------------
     def _launch(self, A, mask, num_updates, use_device_hyper):
         """One fused update of every parameter (torch.optim.SGD.step, _single_tensor_sgd)."""

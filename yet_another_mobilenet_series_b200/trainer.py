@@ -12,7 +12,14 @@ or 'slimmable' (utils/optim.py:161-200); EMA: utils/optim.py:53-64.
 Forward+backward are captured once into a CUDA graph (static input buffers) and replayed; inputs
 arrive through `load(x, target)` which accepts HOST (ideally pinned) or device tensors and copies
 them on a side stream so the H2D copy of step i+1 overlaps the compute of step i (the role of the
-reference's DataPrefetcher, utils/dataflow.py:13-58).
+reference's DataPrefetcher, utils/dataflow.py:13-58).  A batch of another shape (the partial last
+batch of a `drop_last=False` loader, utils/dataflow.py:217-225) runs the same kernels eagerly and
+leaves the graph in place.  The graph is captured again when the optimizer rebuilt the arenas it
+holds pointers into.
+
+Checkpoints have the layout of the reference's save_status (utils/common.py:122-133):
+`state_dict` / `save_status` write it, `load_state_dict` continues from it (or from one the
+reference wrote) by copying into the existing tensors; resuming is bit-exact.
 
 The other half of an epoch, the reference's `validate()` (train.py:273-309), is
 `TrainStep.validate`: `ema_model()` (get_ema_model, common.py:155-172) -> `EvalStep.calibrate`
@@ -24,6 +31,8 @@ Both steps take uint8 image batches (`input_dtype=torch.uint8, input_norm=(mean,
 copy of a quarter of the fp32 bytes, and the stem kernels apply ToTensor() + Normalize(mean, std).
 """
 import copy
+import os
+from collections import OrderedDict
 
 import torch
 import torch.distributed as dist
@@ -32,6 +41,7 @@ from . import dataflow
 from . import distributed as udist
 from . import engine
 from . import tail_ops
+from .flat_arena import ema_momentum
 from .fused_rmsprop import RMSprop
 from .fused_sgd import SGD
 
@@ -92,6 +102,7 @@ class TrainStep:
         self.x_stage = torch.zeros_like(self.x)
         self.t_stage = torch.zeros_like(self.t)
         self.staged = False
+        self.partial = None       # (x, target) of a batch of another shape, run eagerly
         self.loss = torch.zeros((), device=dev)
         self.top1 = torch.zeros((), device=dev)   # fraction correct@1 / @5 of the last batch
         self.top5 = torch.zeros((), device=dev)
@@ -101,6 +112,7 @@ class TrainStep:
         self.consumed.record()
         self.use_graph = use_graph
         self.graph = None
+        self._graph_arenas = None  # the optimizer arenas the graph holds raw pointers into
         self.global_step = 0
         self.launches_per_step = None
         self._warm = 0
@@ -109,7 +121,12 @@ class TrainStep:
 
     # ---- input path ----------------------------------------------------------------------------
     def load(self, x, target):
-        """Stage the next batch into the static device buffers (async on the copy stream)."""
+        """Stage the next batch into the static device buffers (async on the copy stream).  A batch
+        of another shape (the partial last batch of a `drop_last=False` loader) is kept as given:
+        `run` moves it to the device and runs that step eagerly."""
+        if tuple(x.shape) != tuple(self.x.shape):
+            self.partial = (x, target)
+            return
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(self.consumed)  # staging buffers were drained
             self.x_stage.copy_(x, non_blocking=True)
@@ -118,11 +135,14 @@ class TrainStep:
         self.staged = True
 
     # ---- one iteration -------------------------------------------------------------------------
-    def _fwd_bwd(self):
+    def _fwd_bwd(self, x=None, t=None):
+        """Forward + loss + backward on (x, t), by default the static buffers."""
+        x = self.x if x is None else x
+        t = self.t if t is None else t
         self.opt.zero_grad()
-        logits = self.model(self.x)
+        logits = self.model(x)
         # label-smoothed CE + top-1 / top-5 in one kernel, no host sync (common.py:67-80)
-        per_sample, c1, c5 = tail_ops.softmax_ce(logits, self.t, self.smoothing)
+        per_sample, c1, c5 = tail_ops.softmax_ce(logits, t, self.smoothing)
         loss = per_sample.mean()
         engine.DEFER_JOIN = True      # wgrad side stream: one join after the whole backward
         try:
@@ -141,28 +161,43 @@ class TrainStep:
             self._fwd_bwd()
         self.launches_per_step = engine.LAUNCHES - before + 1  # + fused optimizer kernel
         self.graph = g
+        self._graph_arenas = self.opt.arenas()
 
     def run(self):
         """Run one iteration on the staged batch; returns the (device) loss tensor."""
         cur = torch.cuda.current_stream()
-        if self.staged:
+        partial, self.partial = self.partial, None
+        if partial is not None:
+            x = torch.empty(partial[0].shape, device=self.dev, dtype=self.x.dtype,
+                            memory_format=torch.channels_last)
+            x.copy_(partial[0], non_blocking=True)
+            t = partial[1].to(self.dev, dtype=self.t.dtype, non_blocking=True)
+        elif self.staged:
             cur.wait_event(self.copied)
             self.x.copy_(self.x_stage)
             self.t.copy_(self.t_stage)
             self.consumed.record(cur)
             self.staged = False
         self.model.train()
+        if self.graph is not None and self._graph_arenas is not self.opt.arenas():
+            # the optimizer rebuilt its arenas (its load_state_dict, fold_l2, attach_ema): the
+            # graph would accumulate into the freed gradient arena and read the old bf16 mirror
+            self.graph = self._graph_arenas = None
+            self._warm = 0
         self.opt.sync_mirror()   # masters written in place since the last step (load_state_dict ...)
-        if self.use_graph and self.graph is None and self._warm >= 2:
-            torch.cuda.synchronize()
-            self._capture()
-        if self.graph is not None:
-            self.graph.replay()
+        if partial is not None:
+            self._fwd_bwd(x, t)   # eager; the graph and its pinned plans stay for full batches
         else:
-            before = engine.LAUNCHES
-            self._fwd_bwd()
-            self.launches_per_step = engine.LAUNCHES - before + 1
-            self._warm += 1
+            if self.use_graph and self.graph is None and self._warm >= 2:
+                torch.cuda.synchronize()
+                self._capture()
+            if self.graph is not None:
+                self.graph.replay()
+            else:
+                before = engine.LAUNCHES
+                self._fwd_bwd()
+                self.launches_per_step = engine.LAUNCHES - before + 1
+                self._warm += 1
         if self.world > 1:
             dist.all_reduce(self.opt.arenas()["g"])   # in place on the flat arena; mean is folded
         self.global_step += 1
@@ -176,6 +211,74 @@ class TrainStep:
     def __call__(self, x, target):
         self.load(x, target)
         return self.run()
+
+    # ---- checkpoints ---------------------------------------------------------------------------
+    def state_dict(self, epoch=None, best_val=None, meters=None):
+        """The checkpoint of the reference's save_status (utils/common.py:122-133): 'model' (keys
+        prefixed 'module.', as its DataParallel wrapper writes them), 'optimizer', 'ema' (the
+        layout of its ExponentialMovingAverage.state_dict(), None without EMA), 'last_epoch',
+        'best_val', 'meters'; plus 'global_step' and 'cuda_rng_state' (the model device's
+        generator, for Dropout), which the reference ignores.  Tensors are the live ones, not
+        copies."""
+        ema = None
+        if self.ema_decay is not None:
+            pnames, snames = ema_names(self.model)
+            shadow = OrderedDict((n, self.opt.ema_shadow(p))
+                                 for n, p in zip(pnames, self.model.parameters()))
+            shadow.update(zip(snames, self.stat_shadow))
+            ema = ema_state_dict(shadow, self.global_step, self.ema_decay)
+        return {"model": OrderedDict(("module." + k, v) for k, v in self.model.state_dict().items()),
+                "optimizer": self.opt.state_dict(), "ema": ema, "last_epoch": epoch,
+                "best_val": best_val, "meters": meters, "global_step": self.global_step,
+                "cuda_rng_state": torch.cuda.get_rng_state(self.dev)}
+
+    def save_status(self, path, epoch, best_val, meters):
+        """`torch.save(self.state_dict(...), path)` on the master rank only (the reference's
+        save_status).  The file is written next to `path` and renamed over it, so a run stopped
+        while writing leaves the previous checkpoint intact."""
+        sd = self.state_dict(epoch, best_val, meters)
+        if udist.is_master():
+            tmp = path + ".tmp"
+            torch.save(sd, tmp)
+            os.replace(tmp, path)
+
+    def load_state_dict(self, ckpt):
+        """Continue from a checkpoint of `state_dict` / `save_status`, or one the reference's
+        save_status wrote: model (keys with or without 'module.'), optimizer state and
+        hyper-parameters, EMA shadows of the weights and of the running statistics, `global_step`
+        ('global_step', else the EMA's num_updates) and the CUDA generator state.  'optimizer' and
+        'ema' may be absent or None; without 'ema' the EMA restarts from the loaded model.
+
+        Everything is copied into the tensors that exist (the model's parameters are views of the
+        optimizer's arenas), so a captured step graph stays valid and is replayed next."""
+        model = OrderedDict((k[len("module."):] if k.startswith("module.") else k, v)
+                            for k, v in ckpt["model"].items())
+        self.model.load_state_dict(model)
+        ema = ckpt.get("ema")
+        shadows = None
+        if self.ema_decay is not None:
+            pnames, snames = ema_names(self.model)
+            if ema is not None:
+                shadows = [ema["shadow"][n] for n in pnames]
+                stats = [ema["shadow"][n] for n in snames]
+            else:
+                shadows = list(self.model.parameters())
+                stats = self.stat_bufs
+            with torch.no_grad():
+                for s, v in zip(self.stat_shadow, stats):
+                    s.copy_(v)
+        if ckpt.get("optimizer") is not None:
+            self.opt.load_in_place(ckpt["optimizer"], ema=shadows)
+        elif shadows is not None:
+            with torch.no_grad():
+                for p, s in zip(self.model.parameters(), shadows):
+                    self.opt.ema_shadow(p).copy_(s)
+        if ckpt.get("global_step") is not None:
+            self.global_step = int(ckpt["global_step"])
+        elif ema is not None and ema["info"]:
+            self.global_step = int(next(iter(ema["info"].values()))["num_updates"])
+        if ckpt.get("cuda_rng_state") is not None:
+            torch.cuda.set_rng_state(ckpt["cuda_rng_state"].cpu(), self.dev)
 
     # ---- validation ----------------------------------------------------------------------------
     def ema_model(self):
@@ -222,6 +325,25 @@ def _attach_input_norm(model, input_dtype, input_norm):
                          "input pipeline, applied by the stem kernels")
     if input_norm is not None:
         dataflow.set_input_norm(model, *input_norm)
+
+
+def ema_names(model):
+    """(parameter names, running-statistics names) of `model`: together, the variables and the
+    registration order of the reference's setup_ema (common.py:58-63); the second list is also
+    the order of `TrainStep.stat_bufs`."""
+    return ([n for n, _ in model.named_parameters()],
+            [n for n, _ in model.named_buffers() if "running_mean" in n or "running_var" in n])
+
+
+def ema_state_dict(shadow, num_updates, momentum):
+    """The layout of the reference's ExponentialMovingAverage.state_dict() (utils/optim.py:87-95)
+    for `shadow` ({name: fp32 tensor}, in registration order), every variable updated
+    `num_updates` times with the momentum rule of `flat_arena.ema_momentum`."""
+    last = ema_momentum(momentum, num_updates) if num_updates > 0 else None
+    return {"info": OrderedDict((n, {"num_updates": num_updates, "last_momemtum": last,
+                                     "zero_init": False}) for n in shadow),
+            "shadow": OrderedDict(shadow),
+            "param": {"momentum": momentum, "zero_debias": False}}
 
 
 def metrics_from_sums(loss_sum, correct1, correct5, count):
