@@ -510,6 +510,19 @@ typedef struct yamb_block_eval {
 int yamb_block_eval_fwd(const yamb_block_eval* args, yamb_stream_t stream);
 int yamb_block_eval_pool_fwd(const yamb_block_eval* args, yamb_stream_t stream);
 
+/* The same two calls with the 64-channel slices of the hidden dimension of every output tile split
+ * over the `cluster` CTAs (2, 4 or 8) of a thread-block cluster: rank r runs the slices
+ * [r*NC/cluster, (r+1)*NC/cluster) of NC = ceil(Chid/64) and the ranks add their fp32 project
+ * partials in rank order over distributed shared memory before BN3 (+x).  For small batches, whose
+ * tiles leave most SMs idle.  The same function as yamb_block_eval_fwd, with the fp32 sum over the
+ * slices associated differently (a fixed order: the same bits on every run); the pool pass writes
+ * the same values as yamb_block_eval_pool_fwd.  YAMB_EINVAL for another cluster size, for a shape
+ * yamb_block_eval_fwd does not cover, and when the tile plan with the partials does not fit a CTA's
+ * shared memory (nothing enqueued). */
+int yamb_block_eval_cluster_fwd(const yamb_block_eval* args, int32_t cluster, yamb_stream_t stream);
+int yamb_block_eval_cluster_pool_fwd(const yamb_block_eval* args, int32_t cluster,
+                                     yamb_stream_t stream);
+
 /* ---- fused flat-arena RMSprop (+L2 decay, +DDP mean, +EMA, +bf16 repack) -------------------------
  * Replaces RMSprop.step (reference utils/rmsprop.py:67-129), the gradient of cal_l2_loss
  * (utils/optim.py:177-200; l2 * p added where bit 0 of wd_mask is set; bit 1 marks a parameter

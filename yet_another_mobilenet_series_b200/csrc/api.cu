@@ -107,7 +107,7 @@ PFN_encodeTiled get_encode_tiled() {
 extern "C" {
 
 const char* yamb_last_error(void) { return yamb::g_err; }
-int yamb_version(void) { return 102; }
+int yamb_version(void) { return 103; }
 int yamb_max_ctas(void) { int n = yamb::max_ctas(); return n > 0 ? 4 * n : n; }
 int yamb_struct_size(int which) {
   switch (which) {
@@ -180,6 +180,12 @@ int yamb_nl_gram_fwd(const yamb_nl_gram* a, yamb_stream_t s) { return yamb::nl_g
 int yamb_nl_rowmat_fwd(const yamb_nl_rowmat* a, yamb_stream_t s) { return yamb::nl_rowmat_launch(a, YAMB_ST(s)); }
 int yamb_block_eval_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_launch(a, YAMB_ST(s)); }
 int yamb_block_eval_pool_fwd(const yamb_block_eval* a, yamb_stream_t s) { return yamb::block_eval_pool_launch(a, YAMB_ST(s)); }
+int yamb_block_eval_cluster_fwd(const yamb_block_eval* a, int32_t cluster, yamb_stream_t s) {
+  return yamb::block_eval_cluster_launch(a, cluster, YAMB_ST(s));
+}
+int yamb_block_eval_cluster_pool_fwd(const yamb_block_eval* a, int32_t cluster, yamb_stream_t s) {
+  return yamb::block_eval_cluster_pool_launch(a, cluster, YAMB_ST(s));
+}
 int yamb_instance_norm_fwd(const yamb_in_fwd* a, yamb_stream_t s) { return yamb::in_fwd_launch(a, YAMB_ST(s)); }
 int yamb_instance_norm_bwd(const yamb_in_bwd* a, yamb_stream_t s) { return yamb::in_bwd_launch(a, YAMB_ST(s)); }
 int yamb_rmsprop_step(const yamb_rmsprop* a, yamb_stream_t s) { return yamb::rmsprop_launch(a, YAMB_ST(s)); }

@@ -54,6 +54,8 @@ int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t stream);
 int nl_rowmat_launch(const yamb_nl_rowmat* a, cudaStream_t stream);
 int block_eval_launch(const yamb_block_eval* a, cudaStream_t stream);
 int block_eval_pool_launch(const yamb_block_eval* a, cudaStream_t stream);
+int block_eval_cluster_launch(const yamb_block_eval* a, int cluster, cudaStream_t stream);
+int block_eval_cluster_pool_launch(const yamb_block_eval* a, int cluster, cudaStream_t stream);
 int in_fwd_launch(const yamb_in_fwd* a, cudaStream_t stream);
 int in_bwd_launch(const yamb_in_bwd* a, cudaStream_t stream);
 int rmsprop_launch(const yamb_rmsprop* a, cudaStream_t stream);

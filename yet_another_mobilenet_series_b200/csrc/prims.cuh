@@ -14,6 +14,31 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 // ----------------------------------------------------------------------------------------------
+// thread-block clusters: rank, barrier, distributed shared memory
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders this CTA's shared-memory writes before the
+// peers' reads that follow their wait
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the address of this CTA's shared-memory word `addr` in the CTA of cluster rank `rank`
+__device__ __forceinline__ uint32_t dsmem_map(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ float2 dsmem_ld_f2(uint32_t cluster_addr) {
+  float2 v;
+  asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(cluster_addr) : "memory");
+  return v;
+}
+
+// ----------------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {

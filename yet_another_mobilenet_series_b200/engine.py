@@ -1433,6 +1433,50 @@ def _block_eval_cost(block, x, Ho, Wo, residual, project=True):
 # path (tests, tests/gpu_eval_bench_fused_class.py).
 FUSED_CLASS_SHAPE_RULE = True
 
+# ---- small batches: the hidden slices of every output tile split over a thread-block cluster -------
+# (yamb_block_eval_cluster_fwd).  None: eval_cluster_size decides; 1, 2, 4 or 8: every block kernel
+# launch of the eval path takes that cluster size (tests and tests/gpu_eval_latency_bench.py).
+EVAL_CLUSTER = None
+EVAL_CLUSTER_CALLS = 0   # block kernel launches that ran split over a cluster (tests)
+
+
+def eval_tiles(k, stride, N, Ho, Wo, Cout):
+    """Output tiles of one block_eval launch: the tile plan of csrc/block_eval.cuh
+    (block_eval_launch_impl), which takes the geometry with the fewest tiles."""
+    def tiles(toh, tow, ti):
+        return -(-Ho // toh) * -(-Wo // tow) * -(-N // ti)
+    if stride == 2:
+        return tiles({3: 7, 5: 6, 7: 4}[k], 7, 1)
+    if k == 7 or (Cout + 15) // 16 * 16 > 160:   # 7x7 depthwise, or a project wider than 160
+        return tiles(7, 7, 1)
+    return min(tiles(7, 16, 1), tiles(7, 14, 1), tiles(7, 7, 2))
+
+
+def eval_cluster_size(k, stride, N, Ho, Wo, Chid, Cout, sms):
+    """CTAs per cluster of one block_eval launch on a device with `sms` SMs: 1 (one CTA per tile)
+    for a hidden dimension of fewer than 4 slices of 64 channels, else the largest S in {8, 4, 2}
+    with tiles * S <= sms and at least S slices, else 1.  tests/gpu_eval_latency_bench.py on an
+    H100 80GB HBM3 at 700 W (BASELINE.md, "Small-batch eval") measured the split slower than one
+    CTA per tile on blocks of 2 or 3 slices (MobileNetV2 blocks 2-7 at N = 1: 37-43 vs 36-38 us)
+    and faster on the wider ones (blocks 8-17: 42-46 vs 55-124 us)."""
+    tiles, nc = eval_tiles(k, stride, N, Ho, Wo, Cout), -(-Chid // 64)
+    if nc < 4:
+        return 1
+    for s in (8, 4, 2):
+        if tiles * s <= sms and nc >= s:
+            return s
+    return 1
+
+
+_SM_COUNT = {}
+
+
+def _sm_count(dev):
+    n = _SM_COUNT.get(dev.index)
+    if n is None:
+        n = _SM_COUNT[dev.index] = torch.cuda.get_device_properties(dev).multi_processor_count
+    return n
+
 
 def _bn_eval_ready(bn):
     return isinstance(bn, torch.nn.BatchNorm2d) and not bn.training and \
@@ -1490,6 +1534,17 @@ def eval_supported(block, x):
     return True
 
 
+def _block_eval_launch(fn, fn_cluster, a, cluster, tag, nbytes, flops):
+    """One block kernel launch, split over clusters of `cluster` CTAs when cluster > 1 and the
+    tile plan with the exchanged partials fits shared memory, else unsplit."""
+    global EVAL_CLUSTER_CALLS
+    if cluster > 1 and try_launch(lambda st, s: fn_cluster(st, cluster, s), a, tag + "_cluster",
+                                  nbytes, flops):
+        EVAL_CLUSTER_CALLS += 1
+        return
+    launch(fn, a, tag, nbytes, flops)
+
+
 def eval_forward(block, x):
     """y = block(x) in eval mode; x channels_last bf16 on CUDA.  C-ABI calls: the block kernel
     (1); with SE the pool pass and the gate FCs first (3); with a non-local block the kernel writes
@@ -1517,6 +1572,9 @@ def eval_forward(block, x):
         tail = _NlTail(nl, bn4, N, Ho, Wo, Cout, dev)
     out = y if tail is None else tail.l
     a = _block_eval_args(block, x, out, w1, w3, conv_d, (bn1, bn2, bn3), residual)
+    cluster = EVAL_CLUSTER if EVAL_CLUSTER is not None else eval_cluster_size(
+        block.kernel_sizes[0], stride, N, Ho, Wo, Chid, Cout, _sm_count(dev))
+    lib = nat.lib()
     if se is not None:
         # gate = sigmoid(W_e act(W_r mean_HW(a2) + b_r) + b_e): pool pass, then the two FCs
         R = se.se_reduce.weight.shape[0]
@@ -1524,13 +1582,14 @@ def eval_forward(block, x):
         gate = torch.empty(N, Chid, device=dev, dtype=torch.float32)
         uv = torch.empty(2, N, R, device=dev, dtype=torch.float32)
         a.pooled = pooled.data_ptr()
-        launch(nat.lib().yamb_block_eval_pool_fwd, a, "block_eval_pool",
-               *_block_eval_cost(block, x, Ho, Wo, False, project=False))
+        _block_eval_launch(lib.yamb_block_eval_pool_fwd, lib.yamb_block_eval_cluster_pool_fwd, a,
+                           cluster, "block_eval_pool",
+                           *_block_eval_cost(block, x, Ho, Wo, False, project=False))
         _se_fc(se, pooled, uv[0], uv[1], gate)
         a.pooled = None
         a.gate = gate.data_ptr()
-    launch(nat.lib().yamb_block_eval_fwd, a, "block_eval",
-           *_block_eval_cost(block, x, Ho, Wo, residual))
+    _block_eval_launch(lib.yamb_block_eval_fwd, lib.yamb_block_eval_cluster_fwd, a, cluster,
+                       "block_eval", *_block_eval_cost(block, x, Ho, Wo, residual))
     if tail is not None:
         xm = x.permute(0, 2, 3, 1).reshape(N * H * W, Cin)    # view, NHWC matrix
         tail.forward(xm, y.permute(0, 2, 3, 1).reshape(N * Ho * Wo, Cout), block.use_res_connect)
