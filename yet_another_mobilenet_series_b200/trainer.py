@@ -29,6 +29,12 @@ with the metrics summed on the device).
 Both steps take uint8 image batches (`input_dtype=torch.uint8, input_norm=(mean, std)`, e.g. from
 `dataflow.fast_collate`): the static buffers are then uint8 channels_last, `load` is a plain H2D
 copy of a quarter of the fp32 bytes, and the stem kernels apply ToTensor() + Normalize(mean, std).
+
+Gradient accumulation (`micro_batch`): one step runs k = per_gpu_batch / micro_batch forward and
+backward passes over consecutive row slices of the batch into the one gradient arena, then one
+all-reduce, one optimizer step and one EMA update, so a recipe's global batch (the reference's
+`per_gpu_batch_size` x world) is reached with fewer GPUs: the global batch of a step is
+per_gpu_batch x world, and the learning rate and EMA decay follow it.
 """
 import copy
 import os
@@ -53,26 +59,58 @@ def label_smooth_ce(logits, target, smoothing):
     return (1.0 - smoothing) * nll - (smoothing / logits.size(1)) * logp.sum(1)
 
 
+def step_hyper(per_gpu_batch, micro_batch, world, base_lr=0.016, base_total_batch=256,
+               ema_decay=0.9999, ema_base_batch=4096):
+    """What a step of `per_gpu_batch` images per GPU, run in micro-batches of `micro_batch`
+    (None: the whole batch) on `world` GPUs, derives: (micro_batch, k micro-batches per step,
+    learning rate, EMA decay or None, optimizer grad_scale).  The learning rate and the EMA decay
+    follow the global batch per_gpu_batch x world (reference common.py:47-57, 204-205); every
+    micro-batch backpropagates its own mean loss, so grad_scale = 1 / (world x k) turns the sum
+    over ranks and micro-batches into the mean over the global batch."""
+    micro_batch = per_gpu_batch if micro_batch is None else micro_batch
+    if micro_batch <= 0 or per_gpu_batch % micro_batch:
+        raise ValueError("micro_batch must be a positive divisor of per_gpu_batch (got %r for %r)"
+                         % (micro_batch, per_gpu_batch))
+    k = per_gpu_batch // micro_batch
+    gbatch = per_gpu_batch * world
+    lr = base_lr * gbatch / base_total_batch                     # reference common.py:204-205
+    decay = None
+    if ema_decay and ema_decay > 0:
+        decay = ema_decay ** (gbatch / ema_base_batch)           # adjust_momentum, :118-128
+    return micro_batch, k, lr, decay, 1.0 / (world * k)
+
+
 class TrainStep:
     def __init__(self, model, per_gpu_batch, image_size=224, base_lr=0.016, base_total_batch=256,
                  alpha=0.9, momentum=0.9, eps=1e-3, weight_decay=1e-5, label_smoothing=0.1,
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
-                 input_norm=None):
+                 input_norm=None, micro_batch=None):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
-        there); it is attached to the model (dataflow.set_input_norm)."""
+        there); it is attached to the model (dataflow.set_input_norm).
+
+        `per_gpu_batch` is the number of images per GPU per optimizer step: the batch `load` and
+        `__call__` take, and the batch the learning rate and the EMA decay are derived from.
+        `micro_batch` (default `per_gpu_batch`, a divisor of it) is the number of images per
+        forward and backward pass: a step accumulates the gradients of k = per_gpu_batch /
+        micro_batch passes, captured together in one CUDA graph.  BatchNorm then behaves like the
+        reference's per-GPU local BatchNorm at per_gpu_batch_size = micro_batch: batch statistics
+        are those of each micro-batch, the running statistics are updated once per micro-batch (k
+        times per step), and their EMA shadow once per step.  `micro_batch` is not part of a
+        checkpoint: one written with any k loads into a TrainStep with any other."""
+        self.world = udist.get_world_size_fallback()
+        self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
+            per_gpu_batch, micro_batch, self.world, base_lr, base_total_batch, ema_decay,
+            ema_base_batch)
         _attach_input_norm(model, input_dtype, input_norm)
         self.model = model
         dev = next(model.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("TrainStep needs the model on a CUDA device (no CPU path)")
         self.dev = dev
-        self.world = udist.get_world_size_fallback()
         self.batch = per_gpu_batch
-        gbatch = per_gpu_batch * self.world
-        self.lr = base_lr * gbatch / base_total_batch            # reference common.py:204-205
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
                                eps=eps, eps_inside_sqrt=True, weight_decay=0)
@@ -82,11 +120,9 @@ class TrainStep:
         else:
             raise ValueError("Unknown optimizer: {}".format(optimizer))
         self.opt.fold_l2(weight_decay, list(model.named_parameters()), weight_decay_method)
-        self.ema_decay = None
-        if ema_decay and ema_decay > 0:
-            self.ema_decay = ema_decay ** (gbatch / ema_base_batch)  # adjust_momentum, :118-128
+        if self.ema_decay is not None:
             self.opt.attach_ema(self.ema_decay)
-        self.opt.grad_scale = 1.0 / self.world
+        self.opt.grad_scale = self.grad_scale
         self.opt.arenas()
         self.smoothing = label_smoothing
         # BN running statistics and their EMA shadows (flat, for one fused update)
@@ -136,23 +172,57 @@ class TrainStep:
 
     # ---- one iteration -------------------------------------------------------------------------
     def _fwd_bwd(self, x=None, t=None):
-        """Forward + loss + backward on (x, t), by default the static buffers."""
+        """Forward + loss + backward on (x, t), by default the static buffers, in passes of at
+        most `micro_batch` rows whose gradients accumulate in the flat arena.  A batch of
+        `per_gpu_batch` rows backpropagates the mean loss of every pass (grad_scale divides by
+        their number k); any other batch of n rows (a partial last batch) weights the mean of a
+        pass of n_i rows by n_i / n, a device scalar, so its gradient is that of the mean over the
+        n rows."""
         x = self.x if x is None else x
         t = self.t if t is None else t
+        n, b = x.shape[0], self.micro_batch
         self.opt.zero_grad()
+        if n <= b:
+            loss, _, c1, c5 = self._micro_step(x, t)
+            self.loss.copy_(loss.detach())
+            self.top1.copy_(c1.mean())
+            self.top5.copy_(c5.mean())
+            return
+        weights = None
+        if n != self.batch:
+            weights = torch.tensor([min(b, n - s) / n for s in range(0, n, b)], device=self.dev)
+        self.loss.zero_()
+        self.top1.zero_()
+        self.top5.zero_()
+        for i, s in enumerate(range(0, n, b)):
+            # a row slice of a channels_last batch is a channels_last view: no copy
+            _, per_sample, c1, c5 = self._micro_step(x[s:s + b], t[s:s + b],
+                                                     None if weights is None else weights[i])
+            self.loss.add_(per_sample.detach().sum())
+            self.top1.add_(c1.sum())
+            self.top5.add_(c5.sum())
+        self.loss.div_(n)
+        self.top1.div_(n)
+        self.top5.div_(n)
+
+    def _micro_step(self, x, t, weight=None):
+        """Forward, loss and backward of one pass; returns (the loss it backpropagated, the
+        per-sample loss, correct@1, correct@5)."""
         logits = self.model(x)
         # label-smoothed CE + top-1 / top-5 in one kernel, no host sync (common.py:67-80)
         per_sample, c1, c5 = tail_ops.softmax_ce(logits, t, self.smoothing)
         loss = per_sample.mean()
-        engine.DEFER_JOIN = True      # wgrad side stream: one join after the whole backward
+        if weight is not None:
+            loss = loss * weight
+        engine.DEFER_JOIN = True      # wgrad side stream: one join after this pass's backward
         try:
             loss.backward()
         finally:
             engine.DEFER_JOIN = False
+            # the side-stream weight-gradient GEMMs read block intermediates (h1, h2, dh3, the
+            # BatchNorm coefficients) that the next pass's forward rewrites: join before it
             engine.join_side(self.dev)
-        self.loss.copy_(loss.detach())
-        self.top1.copy_(c1.mean())
-        self.top5.copy_(c5.mean())
+        return loss, per_sample, c1, c5
 
     def _capture(self):
         g = torch.cuda.CUDAGraph()
@@ -200,6 +270,8 @@ class TrainStep:
                 self._warm += 1
         if self.world > 1:
             dist.all_reduce(self.opt.arenas()["g"])   # in place on the flat arena; mean is folded
+        # a partial batch's passes are weighted to its mean already: only the ranks' sum is left
+        self.opt.grad_scale = self.grad_scale if partial is None else 1.0 / self.world
         self.global_step += 1
         self.opt.step(num_updates=self.global_step)
         if self.ema_decay is not None and self.stat_bufs:
