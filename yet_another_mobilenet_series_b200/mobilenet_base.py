@@ -11,8 +11,8 @@ module names and therefore the same `state_dict()` keys/shapes, the same helper 
   ConvBNReLU :181-203, SqueezeAndExcitation :91-118, Nonlocal :131-178, ZeroInitBN :121-128,
   Swish :70-78, HSwish :81-88, Narrow/Identity :50-67, init_weights_* :492-537
 
-so the reference's yml model descriptions, checkpoints, `bn_calibration`, `cal_l2_loss`,
-`setup_ema` and the profiler (which all reach into the children) work unchanged.  The children
+so the reference's yml model descriptions, checkpoints, `bn_calibration`, `cal_l2_loss` and
+`setup_ema` (which all reach into the children) work unchanged.  The children
 stay real `nn.Conv2d` / `nn.BatchNorm2d` parameter holders; only `forward` of the two block
 classes is replaced: on CUDA it runs the fused kernel sequence of `engine.py`
 (there is no CPU fallback for it).

@@ -51,12 +51,33 @@ def _full_extent(pool, x):
     return tuple(x.shape[2:]) == tuple(k) and tuple(st) == tuple(k) and tuple(pad) == (0, 0)
 
 
+# ---- instrumentation (model_profiling) -----------------------------------------------------------
+# When STEPS is a list, run_features on CUDA records a CUDA event on the current stream before its
+# first step and after each one, and appends (module, event): (None, e) first, then the stem (its
+# step includes the input's conversion to bf16 channels_last), each block, the head, the pool and
+# model.classifier (its step includes the cast of the logits to fp32).  The time between two
+# consecutive events is the device time of the step the second one ends.  A head run together with
+# the pool (engine.EVAL_TAIL_FUSED) is one step, recorded for the head.
+STEPS = None
+
+
+def _step_done(stream, module):
+    """Ends `module`'s step on `stream`, the current stream looked up once per forward (the lookup
+    costs the host more than the record); None when STEPS is off."""
+    if stream is not None:
+        e = torch.cuda.Event(enable_timing=True)
+        e.record(stream)
+        STEPS.append((module, e))
+
+
 def run_features(model, x):
     """Shared forward of both builders: bf16 channels_last through stem, blocks, head, pool.  A
     uint8 image on a model with an input normalisation (dataflow.set_input_norm) goes to the stem
     as it is; the stem normalises it."""
     if x.is_cuda:
         from . import tail_ops
+        stream = torch.cuda.current_stream() if STEPS is not None else None
+        _step_done(stream, None)
         norm = input_norm_of(model) if x.dtype == torch.uint8 else None
         if norm is None:
             x = engine.to_nhwc_bf16(x)
@@ -71,6 +92,7 @@ def run_features(model, x):
                     continue
                 if i == 0 and norm is not None:
                     x = tail_ops.stem_u8(layer, x, norm)
+                    _step_done(stream, layer)
                     continue
                 nxt = layers[i + 1] if i + 1 < len(layers) else None
                 if (engine.EVAL_TAIL_FUSED and isinstance(layer, ConvBNReLU)
@@ -79,6 +101,7 @@ def run_features(model, x):
                     y = tail_ops.head_pool_eval(layer, x)
                     if y is not None:
                         x, skip = y, True
+                        _step_done(stream, layer)
                         continue
                 if (isinstance(layer, nn.AvgPool2d) and _full_extent(layer, x)):
                     # global average pool: same numbers as nn.AvgPool2d(H), but torch's NHWC
@@ -86,9 +109,12 @@ def run_features(model, x):
                     x = x.mean((2, 3), keepdim=True)
                 else:
                     x = layer(x)
+                _step_done(stream, layer)
             x = x.flatten(1)
             x = run_classifier(model.classifier, x)
-        return x.float()
+        x = x.float()
+        _step_done(stream, model.classifier)
+        return x
     # CPU: stem/head/classifier are plain torch, but the blocks have no CPU path and will raise
     x = model.features(x)
     return model.classifier(x.squeeze(3).squeeze(2))
