@@ -147,6 +147,43 @@ typedef struct yamb_gemm_plan_info {
 
 int yamb_gemm_plan(const yamb_gemm* args, int32_t num_sms, yamb_gemm_plan_info* out);
 
+/* ---- expand-side backward in one pass (csrc/expand_bwd.cu) ------------------------------------
+ * The two gradients of the expand 1x1 convolution, from one read of dz1 and h1:
+ *   dh1 = ca[c]*dz1 + cb[c]*h1 + cc[c]      (BatchNorm-1 backward; the dgrad / wgrad GEMMs' xform 2)
+ *   dx  = dh1 * W1 (+ residual)             bf16 [M][Cin]
+ *   dW1 += dh1^T * x                        fp32 [Chid][Cin], one partial per slab of the split-K
+ *                                           wgrad GEMM's plan, added in slab order: bitwise the
+ *                                           values of the dgrad + wgrad GEMMs
+ * Every tensor is dense: dz1, h1 [M][Chid]; W1 [Chid][Cin]; x, residual, dx [M][Cin].
+ * Caps: 8 <= Cin <= 32, 64 <= Chid <= 192, both multiples of 8.  Other shapes, NULL or
+ * misaligned (16-byte) pointers return YAMB_EINVAL before any device work.  Enqueues on `stream`,
+ * never synchronises, CUDA-graph capturable. */
+typedef struct yamb_expand_bwd_args {
+  int32_t M, Cin, Chid;
+  const void* dz1; const void* h1;
+  const float* ca; const float* cb; const float* cc;
+  const void* W1;                      /* bf16 */
+  const void* x;                       /* bf16 */
+  const void* residual;                /* bf16, or NULL */
+  void* dx;                            /* bf16 */
+  float* dW1;                          /* fp32, += */
+} yamb_expand_bwd_args;
+
+int yamb_expand_bwd(const yamb_expand_bwd_args* args, yamb_stream_t stream);
+
+/* The launch plan of yamb_expand_bwd, computed on the host: the same shape checks (pointers are not
+ * checked).  num_sms > 0 plans for that many SMs and needs no device; <= 0 uses the current
+ * device (YAMB_ENODEV without one). */
+typedef struct yamb_expand_bwd_plan_info {
+  int32_t block_n;                     /* wgmma width: Cin padded to 16 or 32 */
+  int32_t panels;                      /* 64-channel panels of Chid */
+  int32_t slabs, slab_rows;            /* the split-K wgrad GEMM's slabs of pixels: one dW1 partial each */
+  int32_t grid, num_stages, smem_bytes;
+} yamb_expand_bwd_plan_info;
+
+int yamb_expand_bwd_plan(const yamb_expand_bwd_args* args, int32_t num_sms,
+                         yamb_expand_bwd_plan_info* out);
+
 /* ---- depthwise k x k convolution (k in {3,5,7}, stride 1/2, pad (k-1)/2) -------------------------
  * Replaces nn.Conv2d(groups=C)+BatchNorm2d+activation of ConvBNReLU
  * (reference: models/mobilenet_base.py:405-411 unfused, :275-281 fused, :181-203 ConvBNReLU).

@@ -140,6 +140,8 @@ int yamb_struct_size(int which) {
     case 26: return (int)sizeof(yamb_head_pool_eval);
     case 27: return (int)sizeof(yamb_gemm_plan_info);
     case 28: return (int)sizeof(yamb_stem_conv_u8);
+    case 29: return (int)sizeof(yamb_expand_bwd_args);
+    case 30: return (int)sizeof(yamb_expand_bwd_plan_info);
     default: return -1;
   }
 }
@@ -149,6 +151,12 @@ int yamb_pointwise_gemm(const yamb_gemm* args, yamb_stream_t stream) {
 }
 int yamb_gemm_plan(const yamb_gemm* args, int32_t num_sms, yamb_gemm_plan_info* out) {
   return yamb::gemm_plan_query(args, num_sms, out);
+}
+int yamb_expand_bwd(const yamb_expand_bwd_args* args, yamb_stream_t stream) {
+  return yamb::expand_bwd_launch(args, reinterpret_cast<cudaStream_t>(stream));
+}
+int yamb_expand_bwd_plan(const yamb_expand_bwd_args* args, int32_t num_sms, yamb_expand_bwd_plan_info* out) {
+  return yamb::expand_bwd_plan_query(args, num_sms, out);
 }
 
 

@@ -28,6 +28,8 @@ PFN_encodeTiled get_encode_tiled();
 
 int gemm_launch(const yamb_gemm* a, cudaStream_t stream);
 int gemm_plan_query(const yamb_gemm* a, int num_sms, yamb_gemm_plan_info* out);
+int expand_bwd_launch(const yamb_expand_bwd_args* a, cudaStream_t stream);
+int expand_bwd_plan_query(const yamb_expand_bwd_args* a, int num_sms, yamb_expand_bwd_plan_info* out);
 int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t stream);
 int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t stream);
 int bn_apply_launch(const yamb_bn_apply* a, cudaStream_t stream);

@@ -8,7 +8,8 @@ autograd entry the modules in `mobilenet_base.py` call.  Kernel order (train mod
             -> project GEMM (BN2+act operand transform, +BN3 stats) -> BN3 apply (+x)
   backward  BN3 reduce -> project dgrad GEMM (BN3-bwd operand transform, act'/BN2-bwd epilogue)
             + project wgrad GEMM -> depthwise bwd (BN2-bwd on load, fused wgrad, act'/BN1-bwd
-            epilogue) -> expand dgrad GEMM (+dy) + expand wgrad GEMM
+            epilogue) -> expand dgrad GEMM (+dy) + expand wgrad GEMM, or both in one
+            expand_bwd launch (expand_bwd_fused)
 
 Reference semantics: models/mobilenet_base.py:446-451 (unfused), :330-342 (fused) and their
 torch.autograd backward.  No tensor between the 1x1 convs is ever normalised in HBM: BatchNorm +
@@ -710,6 +711,8 @@ class BlockPlan:
         self.w_exp_bf = torch.empty(Chid, Cin, device=dev, dtype=bf) if self.expand else None
         self.w_proj_bf = torch.empty(Cout, Chid, device=dev, dtype=bf)
         self.w_exp_own, self.w_proj_own = self.w_exp_bf, self.w_proj_bf
+        # backward: the expand-side gradients in one yamb_expand_bwd launch, or two GEMMs
+        self.expand_fused = self.expand and expand_bwd_fused(self.M_in, Cin, Chid)
         # multi-branch expand / project weight gradients of direct mode (GradTargets.concat)
         self.concat_grads = {}
         self.generation = 0
@@ -946,6 +949,20 @@ class BlockPlan:
                         xm, dx, "dw_bwd", residual=dym_skip if self.residual else None)
         if not self.expand:
             return dx
+        # 5+6. dh1 = ca1*dz1 + cb1*h1 + cc1 formed once, dx = dh1 * W1 (+ dy) and
+        #      dW1 += dh1^T * x from the same staged tile: one read of dz1 and h1
+        if self.expand_fused:
+            a = nat.ExpandBwd()
+            a.M, a.Cin, a.Chid = self.M_in, self.Cin, self.Chid
+            a.dz1, a.h1 = self.dz1.data_ptr(), self.h1.data_ptr()
+            a.ca, a.cb, a.cc = (t.data_ptr() for t in (self.bn1.ca, self.bn1.cb, self.bn1.cc))
+            a.W1, a.x = self.w_exp_bf.data_ptr(), xm.data_ptr()
+            a.residual = dym_skip.data_ptr() if self.residual else None
+            a.dx, a.dW1 = dx.data_ptr(), grads["exp"].data_ptr()
+            launch(lib.yamb_expand_bwd, a, "expand_bwd",
+                   2 * self.M_in * (2 * self.Chid + self.Cin * (3 if self.residual else 2)),
+                   4 * self.M_in * self.Chid * self.Cin)
+            return dx
         fork2_ev = self._fork_event()   # dz1 and the BN1-backward coefficients exist from here on
         # 5. expand dgrad: dx = dh1 * W1 (+ dy)
         g = nat.Gemm()
@@ -978,6 +995,28 @@ class BlockPlan:
                         2 * self.M_in * (2 * self.Chid + self.Cin),
                         2 * self.M_in * self.Chid * self.Cin, fork2_ev, (x,))
         return dx
+
+
+# Expand-side backward: one yamb_expand_bwd launch where its plan covers the shape and the block
+# has at least this many input pixels, else the dgrad GEMM + split-K wgrad GEMM.  Both paths give
+# the same bits.  Measured on H100 (tests/gpu_expand_bwd_bench.py, BASELINE.md §5) the fused kernel
+# is about twice as fast down to the smallest covered MobileNetV2 block, 25088 pixels (28 x 28 at
+# N = 32: 98 slabs, fewer than the SMs); smaller maps are not measured and keep the two GEMMs.
+EXPAND_BWD_MIN_M = 25088
+
+
+def expand_bwd_fused(M_in, Cin, Chid):
+    """True when BlockPlan.backward runs the expand-side backward as one yamb_expand_bwd launch."""
+    if M_in < EXPAND_BWD_MIN_M or M_in >= 2 ** 31:
+        return False
+    a = nat.ExpandBwd()
+    a.M, a.Cin, a.Chid = M_in, Cin, Chid
+    info = nat.ExpandBwdPlanInfo()
+    rc = nat.lib().yamb_expand_bwd_plan(C.byref(a), 1, C.byref(info))   # shape checks, no device
+    if rc == nat.EINVAL:
+        return False
+    nat.check(rc)
+    return True
 
 
 def _bf16_operand(w, own, shape):

@@ -335,14 +335,30 @@ class InBwd(C.Structure):
     ]
 
 
+class ExpandBwd(C.Structure):
+    _fields_ = [
+        ("M", C.c_int32), ("Cin", C.c_int32), ("Chid", C.c_int32),
+        ("dz1", C.c_void_p), ("h1", C.c_void_p),
+        ("ca", C.c_void_p), ("cb", C.c_void_p), ("cc", C.c_void_p),
+        ("W1", C.c_void_p), ("x", C.c_void_p), ("residual", C.c_void_p),
+        ("dx", C.c_void_p), ("dW1", C.c_void_p),
+    ]
+
+
+class ExpandBwdPlanInfo(C.Structure):
+    _fields_ = [(name, C.c_int32) for name in (
+        "block_n", "panels", "slabs", "slab_rows", "grid", "num_stages", "smem_bytes")]
+
+
 _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnReduce, 7: SePool,
             8: Rmsprop, 9: SeBwdReduce, 10: SeBwdApply, 11: BnStats, 12: BnBwdApply, 13: NlGram,
             14: NlRowmat, 15: SeFc, 16: SeFcBwd, 17: SoftmaxCe, 18: SoftmaxCeGrad,
             19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd, 24: Sgd,
-            25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8}
+            25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
+            29: ExpandBwd, 30: ExpandBwdPlanInfo}
 
 # every symbol include/yamb200.h declares
-SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
+SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
            "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_head_pool_eval_fwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
@@ -373,6 +389,9 @@ def lib():
                                   (which, n, C.sizeof(st)))
         l.yamb_pointwise_gemm.argtypes = [C.POINTER(Gemm), C.c_void_p]
         l.yamb_gemm_plan.argtypes = [C.POINTER(Gemm), C.c_int32, C.POINTER(GemmPlanInfo)]
+        l.yamb_expand_bwd.argtypes = [C.POINTER(ExpandBwd), C.c_void_p]
+        l.yamb_expand_bwd_plan.argtypes = [C.POINTER(ExpandBwd), C.c_int32,
+                                           C.POINTER(ExpandBwdPlanInfo)]
         l.yamb_depthwise_fwd.argtypes = [C.POINTER(DwFwd), C.c_void_p]
         l.yamb_depthwise_bwd.argtypes = [C.POINTER(DwBwd), C.c_void_p]
         l.yamb_bn_apply_fwd.argtypes = [C.POINTER(BnApply), C.c_void_p]
