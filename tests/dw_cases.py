@@ -18,7 +18,7 @@ H100_MAX_CTAS = 4 * 132
 
 def pick_ct(C, rows):
     """Channels per tile; the forward passes Ho as `rows`, the backward H (pick_ct in
-    depthwise.cu, without the YAMB_DW_CT override)."""
+    depthwise.cu)."""
     if C <= 8 and rows >= 28:
         return 8
     if C <= 16 and rows >= 14:

@@ -57,8 +57,6 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <map>
@@ -206,7 +204,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     for (int tp = (tid & 3); tp < K * K; tp += 4)
       asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst + (uint32_t)(tp * 256)),
                    "l"(src + tp), "r"(ok ? 4 : 0) : "memory");
-    asm volatile("cp.async.commit_group;" ::: "memory");
+    cp_async_commit();
   };
   auto tab_store = [&](float* tb) {
     if (tid < 128) {
@@ -214,7 +212,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       tb[which * 128 + ch] = pre_s;          // s1 at 0, s2 at 128
       tb[which * 128 + 64 + ch] = pre_t;     // t1 at 64, t2 at 192
     }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");   // this thread's taps have landed
+    cp_async_wait<0>();   // this thread's taps have landed
   };
 
   // ---- TMA (control thread) ------------------------------------------------------------------------
@@ -701,10 +699,6 @@ static int launch_eval_act(BlockEvalDev& p, const yamb_block_eval* a, cudaStream
   long long cap = (long long)max_ctas();
   if (CLUSTER && (rc = max_active_clusters(kern, smem, p.cs, &cap))) return rc;
   const int grid = (int)(p.num_tiles < cap ? p.num_tiles : cap) * (CLUSTER ? p.cs : 1);
-  static const bool dbg = getenv("YAMB_EVAL_DEBUG") != nullptr;
-  if (dbg)
-    fprintf(stderr, "block_eval: mode %d tiles %d grid %d cluster %d smem %d Npad %d NC %d KB %d\n",
-            MODE, p.num_tiles, grid, CLUSTER ? p.cs : 1, smem, p.Npad, p.NC, p.KB);
   auto run = [&]() -> cudaError_t {
     if (!CLUSTER) {
       block_eval_kernel<G, EXPAND, LEAN, MODE, CLUSTER><<<grid, 256, smem, st>>>(tmX, tmW1, tmW3, p);

@@ -21,11 +21,7 @@ static int check_common(int N, int H, int W, int C, int ldc, int k, int stride) 
 // (searched networks: AtomNAS keeps branches of 1-23 channels at 56 x 56, padded to 8 / 16 / 24)
 // get 8- or 16-channel tiles — with 32-channel tiles three quarters / half of the lanes computed
 // padding — as long as the image is tall enough for the 64- / 32-row tiles that go with them.
-// YAMB_DW_CT overrides.
 static int pick_ct(int C, int H) {
-  static int forced = -1;
-  if (forced < 0) { const char* e = getenv("YAMB_DW_CT"); forced = e ? atoi(e) : 0; }
-  if (forced == 8 || forced == 16 || forced == 32 || forced == 64) return forced;
   if (C <= 8 && H >= 28) return 8;
   if (C <= 16 && H >= 14) return 16;
   if (C <= 32) return 32;

@@ -22,30 +22,20 @@
 // shared accesses are bank-conflict free.  CTAs are persistent over (channel chunk, image tile).
 #pragma once
 #include <cuda_bf16.h>
-#include <stdlib.h>
 #include <cuda_runtime.h>
 
 #include "bn_finalize.cuh"
 #include "host_util.h"
 #include "prims.cuh"
 
-// resident CTAs per SM the 3x3 kernels are compiled for (register cap 64 Ki / (256 * n)); the
-// profiling variant build overrides it (-DYAMB_DW_MINBLOCKS=3) to A/B occupancy against spills
-#ifndef YAMB_DW_MINBLOCKS
-#define YAMB_DW_MINBLOCKS 2
-#endif
-
 namespace yamb {
+
+// resident CTAs per SM the 3x3 kernels are compiled for (register cap 64 Ki / (256 * n))
+constexpr int kDw3MinBlocks = 2;
 
 __device__ __forceinline__ void ld4(const __nv_bfloat16* p, float (&v)[4]) {
   const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
   v[0] = bf16lo(u.x); v[1] = bf16hi(u.x); v[2] = bf16lo(u.y); v[3] = bf16hi(u.y);
-}
-// round to bf16, store, and leave the rounded values in v
-__device__ __forceinline__ void st4_round(__nv_bfloat16* p, float (&v)[4]) {
-  const uint32_t a = pack_bf16(v[0], v[1]), b = pack_bf16(v[2], v[3]);
-  v[0] = bf16lo(a); v[1] = bf16hi(a); v[2] = bf16lo(b); v[3] = bf16hi(b);
-  *reinterpret_cast<uint2*>(p) = make_uint2(a, b);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -79,22 +69,11 @@ struct FwdGeom {
   static constexpr int IW = (TOW - 1) * S + K;
 };
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, int src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)),
-               "l"(gsrc), "r"(src_bytes)
-               : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-
 // Forward, v4: the raw bf16 input tile (with halo) of tile t+1 streams into shared memory with
 // cp.async (zero-fill outside the image) while tile t is transformed IN PLACE (BN + activation,
 // rounded to bf16 like every other materialised activation) and convolved.
 template <int K, int S, int CT, int TW>
-__global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_fwd_kernel(
+__global__ void __launch_bounds__(256, (K == 3 ? kDw3MinBlocks : 1)) dw_fwd_kernel(
     const __grid_constant__ DwFwdDev p) {
   using G = FwdGeom<K, S, CT, TW>;
   constexpr int P = (K - 1) / 2;
@@ -166,9 +145,7 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_fwd_
       if ((k + 1) * PSTEP > NPIX) ok = ok && (pslot + k * PSTEP < NPIX);
       const __nv_bfloat16* src = img + (ok ? (unsigned)((iy * p.W + ix) * p.ldc) : 0u);
       if ((k + 1) * PSTEP <= NPIX || pslot + k * PSTEP < NPIX)
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + k * PSTEP * CT * 2),
-                     "l"(src), "r"(ok ? 16 : 0)
-                     : "memory");
+        cp_async_zfill16(dst + k * PSTEP * CT * 2, src, ok ? 16 : 0);
       mask |= ok ? (1u << k) : 0u;
       cc += DC; r += DR;
       if (cc >= IW) { cc -= IW; ++r; }
@@ -403,7 +380,7 @@ __device__ __forceinline__ constexpr bool tap_hits(int a, int k, int r) {
 // gathers a 2x2 pixel tile from registers: every staged gradient vector feeds up to 4 dgrad and
 // 4 wgrad FMAs, all shared-memory offsets are immediates, no bounds or parity branches.
 template <int K, int S, int CT, int TAP0, int TAP1, bool DGRAD>
-__global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_kernel(
+__global__ void __launch_bounds__(256, (K == 3 ? kDw3MinBlocks : 1)) dw_bwd_kernel(
     const __grid_constant__ DwBwdDev p) {
   using G = BwdGeom<K, S, CT>;
   constexpr int P = G::P, TIH = G::TIH, TIW = G::TIW, RH = G::RH, RW = G::RW, R = G::R;
@@ -552,10 +529,8 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_
       if ((k + 1) * PSTEP > NPR) ok = ok && (pslot + k * PSTEP < NPR);
       const unsigned o = ok ? (unsigned)((oy * p.Wo + ox) * p.ldc) : 0u;
       if ((k + 1) * PSTEP <= NPR || pslot + k * PSTEP < NPR) {
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d_dz + k * PSTEP * CT * 2),
-                     "l"(gdz + o), "r"(ok ? 16 : 0) : "memory");
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d_h + k * PSTEP * CT * 2),
-                     "l"(gh + o), "r"(ok ? 16 : 0) : "memory");
+        cp_async_zfill16(d_dz + k * PSTEP * CT * 2, gdz + o, ok ? 16 : 0);
+        cp_async_zfill16(d_h + k * PSTEP * CT * 2, gh + o, ok ? 16 : 0);
       }
       mask |= ok ? (1u << k) : 0u;
       cc += DC_R; r += DR_R;
@@ -570,8 +545,7 @@ __global__ void __launch_bounds__(256, (K == 3 ? YAMB_DW_MINBLOCKS : 1)) dw_bwd_
       if ((k + 1) * PSTEP > NPX) ok = ok && (pslot + k * PSTEP < NPX);
       const unsigned o = ok ? (unsigned)((y * p.W + x) * p.ldc) : 0u;
       if ((k + 1) * PSTEP <= NPX || pslot + k * PSTEP < NPX)
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d_x + k * PSTEP * CT * 2),
-                     "l"(gx + o), "r"(ok ? 16 : 0) : "memory");
+        cp_async_zfill16(d_x + k * PSTEP * CT * 2, gx + o, ok ? 16 : 0);
     }
     return mask;
   };

@@ -264,11 +264,9 @@ expand_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constan
         const __nv_bfloat16* src = ok ? p.x + (size_t)(u0 + r) * p.Cin : p.x;
         const uint32_t dst = s_x + xb * kXbPanel + r * 128;
         for (int c = 0; c < p.Cin / 8; ++c)
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(
-                           dst + (uint32_t)((c ^ (r & 7)) << 4)),
-                       "l"(ok ? src + 8 * c : src), "r"(ok ? 16 : 0)
-                       : "memory");
-        asm volatile("cp.async.commit_group;" ::: "memory");
+          cp_async_zfill16(dst + (uint32_t)((c ^ (r & 7)) << 4), ok ? src + 8 * c : src,
+                           ok ? 16 : 0);
+        cp_async_commit();
       }
       for (int pn = 0; pn < p.panels; ++pn) {
         const int c0 = pn * 64 + lc * 8;
@@ -298,11 +296,8 @@ expand_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constan
         for (int j = 0; j < 8; ++j) {
           const int r = 32 * tw + (lane >> 3) + 4 * j;
           const uint32_t off = (uint32_t)(r * 128) + (swz ^ (uint32_t)((r & 7) << 4));
-          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-                       : "=r"(v[j].x), "=r"(v[j].y), "=r"(v[j].z), "=r"(v[j].w) : "r"(sA + off));
-          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-                       : "=r"(u[j].x), "=r"(u[j].y), "=r"(u[j].z), "=r"(u[j].w)
-                       : "r"(sA + kXbPanel + off));
+          v[j] = lds128(sA + off);
+          u[j] = lds128(sA + kXbPanel + off);
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -320,12 +315,10 @@ expand_bwd_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constan
           }
           // rows past M and channels past Chid stay zero (the TMA's fill)
           const bool ok = cok && r < rlimit;
-          asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(sA + off),
-                       "r"(ok ? o[0] : 0u), "r"(ok ? o[1] : 0u), "r"(ok ? o[2] : 0u),
-                       "r"(ok ? o[3] : 0u)
-                       : "memory");
+          sts128(sA + off,
+                 make_uint4(ok ? o[0] : 0u, ok ? o[1] : 0u, ok ? o[2] : 0u, ok ? o[3] : 0u));
         }
-        if (pn == 0) asm volatile("cp.async.wait_group 0;" ::: "memory");   // x rows landed
+        if (pn == 0) cp_async_wait<0>();   // x rows landed
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars->full[stage]);

@@ -24,8 +24,6 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "bn_finalize.cuh"
@@ -33,15 +31,6 @@
 #include "prims.cuh"
 
 namespace yamb {
-// phase timers of the roles (YAMB_GEMM_DEBUG=512) are compiled in only with -DYAMB_GEMM_TIMERS
-// (YAMB_GEMM_TIMERS=1 python -c 'import __graft_entry__ as g; g.build(force=True)'): the clock
-// reads are scheduling barriers in the hot loops
-#ifdef YAMB_GEMM_TIMERS
-#define YCLK() clock64()
-#else
-#define YCLK() 0LL
-#endif
-
 // Why the last mbarrier wait of gemm_tc_kernel that gave up did so:
 //   bits 40..63 block, 24..39 thread, 0..23 shared-memory address of the barrier.
 // Zero while no wait has timed out; readable from a debugger or a GPU core dump after the trap.
@@ -98,8 +87,6 @@ struct GemmDev {
   const float *a_gate, *b_gate;  // optional per-(sample, channel) gates [n][C] (SE)
   long long gate_rps;            // pixels per sample
   int wg2x;                   // 1: warps 8-11 transform (light epilogue), 0: they are epilogue WG 1
-  int dbg;                    // YAMB_GEMM_DEBUG bits: 1 skip transform math, 2 skip proxy fence
-  unsigned long long* dbg_buf;  // bit 512: per-phase cycle sums of the loader warps
   // operand tensors in global memory ([pixels|rows][channels], bf16) for the cp.async loaders
   const __nv_bfloat16 *gA, *gA2, *gB, *gB2;
   long long lda, lda2, ldb, ldb2;
@@ -123,31 +110,8 @@ struct Bars {
   uint64_t turn[2];   // main-loop hand-over between the two consumer warpgroups
 };
 
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait_n() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// ---- explicit shared-space vector accesses (32-bit shared addresses, never generic) ----
-__device__ __forceinline__ uint4 lds128(uint32_t a) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ float4 lds128f(uint32_t a) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t a, const uint4& v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z),
-               "r"(v.w) : "memory");
 }
 
 // Register-staged load + transform of one operand panel by ONE warp: every lane owns the same
@@ -736,7 +700,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       named_bar_sync(2, nxt);
     }
-    long long dbg_l[4] = {0, 0, 0, 0};
     const ActParam apa = make_act((kXform && p.a_xform == 1) ? p.a_act : ACT_NONE);
     const ActParam apb = make_act((kXform && p.b_xform == 1) ? p.b_act : ACT_NONE);
     const int na = kAmn ? 2 : 1;                                         // panels of A
@@ -807,16 +770,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int r = i >> g.cshift, lc = i & ((1 << g.cshift) - 1);
         const bool ok = r < g.rlimit && g.col0 + lc * 8 < g.climit;
         const __nv_bfloat16* sp = ok ? base + (long long)r * ld + lc * 8 : src;
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(
-                         dst + (uint32_t)(r * 128 + ((lc ^ (r & 7)) << 4))),
-                     "l"(sp), "r"(ok ? 16 : 0)
-                     : "memory");
+        cp_async_zfill16(dst + (uint32_t)(r * 128 + ((lc ^ (r & 7)) << 4)), sp, ok ? 16 : 0);
       }
     };
     auto issue = [&](const Cur& c, int stage, int rnd) {
-      const long long tl0 = YCLK();
       gemm_wait(&bars->empty[stage], (rnd & 1) ^ 1);
-      dbg_l[0] += YCLK() - tl0;
       const uint32_t sA = smem_u32(smem + (size_t)stage * p.stage_bytes);
       for (int pi = 0; pi < na + nb; ++pi) {
         const Pan g = panel_of(c, pi);
@@ -825,7 +783,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     };
     auto consume = [&](const Cur& c, int stage, int rnd) {
-      const long long tl3 = YCLK();
       if (kXform && use_x) {
         const uint32_t sA = smem_u32(smem + (size_t)stage * p.stage_bytes);
         // narrow transformed operands: registers (few bytes per row, latency hidden by the batch)
@@ -853,44 +810,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         // wide transformed operands: the TMA producer loaded them; rewrite the tile in place
         if (p.a_tma || p.b_tma) {
-          const long long tl1 = YCLK();
           gemm_wait(&bars->xdone[stage], rnd & 1);
-          dbg_l[1] += YCLK() - tl1;
-          if (!(p.dbg & 1)) {
 #pragma unroll 1
-            for (int pi = 0; pi < na + nb; ++pi) {
-              const Pan g = panel_of(c, pi);
-              const int mode = g.isA ? p.a_xform : p.b_xform;
-              if (mode == 0 || !(g.isA ? p.a_tma : p.b_tma)) continue;
-              const ActParam& ap = g.isA ? apa : apb;
-              const float* tab = g.isA ? xa : xb;
-              const int Ct = g.isA ? Ca : Cb;
-              const uint32_t t_s = smem_u32(tab), t_b = smem_u32(tab + Ct), t_s2 = smem_u32(tab + 2 * Ct);
-              const float* gate = (mode == 1 && (g.mn || g.isA)) ? (g.isA ? p.a_gate : p.b_gate) : nullptr;
-              const uint32_t op2 = sA + (g.isA ? p.a2_off : p.b2_off) +
-                                   (g.off - (g.isA ? 0u : (uint32_t)p.a_bytes));
-              // rows the TMA zero-filled (outside the tensor) must stay zero: limit = rlimit
-              if (mode == 2)
-                gxform_panel<2, true>(sA + g.off, op2, nullptr, 0, nullptr, 0, ls * ((1 << g.logR) / G),
-                                      min(g.rlimit, (ls + 1) * ((1 << g.logR) / G)), g.rlimit, ln, 3, ap,
-                                      t_s, t_b, t_s2, g.col0, g.climit, gate, (unsigned)g.row0,
-                                      (unsigned)p.gate_rps);
-              else
-                gxform_panel<1, true>(sA + g.off, op2, nullptr, 0, nullptr, 0, ls * ((1 << g.logR) / G),
-                                      min(g.rlimit, (ls + 1) * ((1 << g.logR) / G)), g.rlimit, ln, 3, ap,
-                                      t_s, t_b, t_s2, g.col0, g.climit, gate, (unsigned)g.row0,
-                                      (unsigned)p.gate_rps);
-            }
+          for (int pi = 0; pi < na + nb; ++pi) {
+            const Pan g = panel_of(c, pi);
+            const int mode = g.isA ? p.a_xform : p.b_xform;
+            if (mode == 0 || !(g.isA ? p.a_tma : p.b_tma)) continue;
+            const ActParam& ap = g.isA ? apa : apb;
+            const float* tab = g.isA ? xa : xb;
+            const int Ct = g.isA ? Ca : Cb;
+            const uint32_t t_s = smem_u32(tab), t_b = smem_u32(tab + Ct), t_s2 = smem_u32(tab + 2 * Ct);
+            const float* gate = (mode == 1 && (g.mn || g.isA)) ? (g.isA ? p.a_gate : p.b_gate) : nullptr;
+            const uint32_t op2 = sA + (g.isA ? p.a2_off : p.b2_off) +
+                                 (g.off - (g.isA ? 0u : (uint32_t)p.a_bytes));
+            // rows the TMA zero-filled (outside the tensor) must stay zero: limit = rlimit
+            if (mode == 2)
+              gxform_panel<2, true>(sA + g.off, op2, nullptr, 0, nullptr, 0, ls * ((1 << g.logR) / G),
+                                    min(g.rlimit, (ls + 1) * ((1 << g.logR) / G)), g.rlimit, ln, 3, ap,
+                                    t_s, t_b, t_s2, g.col0, g.climit, gate, (unsigned)g.row0,
+                                    (unsigned)p.gate_rps);
+            else
+              gxform_panel<1, true>(sA + g.off, op2, nullptr, 0, nullptr, 0, ls * ((1 << g.logR) / G),
+                                    min(g.rlimit, (ls + 1) * ((1 << g.logR) / G)), g.rlimit, ln, 3, ap,
+                                    t_s, t_b, t_s2, g.col0, g.climit, gate, (unsigned)g.row0,
+                                    (unsigned)p.gate_rps);
           }
         }
       }
-      const long long tl2 = YCLK();
-      dbg_l[2] += tl2 - tl3;
-      cp_async_wait_n<0>();
+      cp_async_wait<0>();
       fence_proxy_async_smem();
       __syncwarp();
       if (ln == 0) mbar_arrive(&bars->full[stage]);
-      dbg_l[3] += YCLK() - tl2;
     };
 
     // One loader WARP fills a whole stage, and every stage has ONE owner warp (stage s belongs to
@@ -901,7 +851,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     Cur c;
     c.w = blockIdx.x;
     cur_set(c);
-    const long long dbg_l0 = YCLK();
     // n = running k-block index, st = n % S, rnd = n / S (no divisions in the loop)
     int st = 0, rnd = 0;
     for (; c.w < p.num_work; cur_next(c)) {
@@ -911,14 +860,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         consume(c, st, rnd);
       }
       if (++st == S) { st = 0; ++rnd; }
-    }
-    if ((p.dbg & 512) && ln == 0) {
-      atomicAdd(p.dbg_buf + 12, (unsigned long long)dbg_l[0]);
-      atomicAdd(p.dbg_buf + 13, (unsigned long long)dbg_l[1]);
-      atomicAdd(p.dbg_buf + 14, (unsigned long long)dbg_l[2]);
-      atomicAdd(p.dbg_buf + 15, (unsigned long long)dbg_l[3]);
-      atomicAdd(p.dbg_buf + 8, (unsigned long long)(YCLK() - dbg_l0));
-      atomicAdd(p.dbg_buf + 9, 1ull);
     }
   }
 
@@ -1042,17 +983,12 @@ static int gemm_plan(const yamb_gemm* a, int num_sms, GemmPlan& pl) {
   if ((p.a_xform == 2 && (!a->A2 || !a->a_scale2)) || (p.b_xform == 2 && (!a->B2 || !a->b_scale2)))
     return set_error(YAMB_EINVAL, "two-source transform without second tensor");
   p.has_residual = (a->epi == 0 && a->residual) ? 1 : 0;
-  static const int env_dbg = [] { const char* d = getenv("YAMB_GEMM_DEBUG"); return d ? atoi(d) : 0; }();
-  p.dbg = env_dbg;
-  p.dbg_buf = nullptr;
   // transform-heavy / epilogue-light launches give warps 8-11 to the transform
   // warps 8-11 load/transform instead of running a second epilogue warpgroup when the epilogue
   // is light relative to the operand work: split-K wgrad (no store at all) or a forward/dgrad
   // store of <= 192 columns fed by more than one k-block per tile
   p.wg2x = ((a->a_xform || a->b_xform) &&
             (a->epi == 2 || (a->epi == 0 && p.block_n <= 192 && p.num_k_blocks >= 2))) ? 1 : 0;
-  if (p.dbg & 16) p.wg2x = 0;
-  if (p.dbg & 32) p.wg2x = (a->a_xform || a->b_xform) ? 1 : 0;
   p.a_gate = a->a_xform == 1 ? a->a_gate : nullptr;
   p.b_gate = a->b_xform == 1 ? a->b_gate : nullptr;
   p.gate_rps = a->gate_rows_per_sample > 0 ? a->gate_rows_per_sample : 1;
@@ -1093,8 +1029,6 @@ static int gemm_plan(const yamb_gemm* a, int num_sms, GemmPlan& pl) {
   // second source needs its own region; narrow ones are combined in registers on their way in
   p.a_tma = (p.a_xform != 0 && (p.a_mn ? a->M : a->K) >= 64) ? 1 : 0;
   p.b_tma = (p.b_xform != 0 && (p.b_mn ? a->N : a->K) >= 64) ? 1 : 0;
-  const int dbg_env = env_dbg;
-  if (dbg_env & 1024) p.a_tma = p.b_tma = 0;
   // transformed operands: 4 (2) loader warps share a stage so that its transform latency is short;
   // plain GEMMs are bound by load latency: one warp per stage, as many stages in flight as warps
   p.a2_off = p.b2_off = 0;
@@ -1139,9 +1073,6 @@ static int gemm_plan(const yamb_gemm* a, int num_sms, GemmPlan& pl) {
     // fewer stages than loader warps: the surplus warps would idle — let them share stages
     while (p.lgroup < 4 && nlw / (p.lgroup * 2) >= stages) p.lgroup *= 2;
   }
-  if (dbg_env & 2048) p.lgroup = 4;
-  if (dbg_env & 4096) p.lgroup = 2;
-  if (dbg_env & 8192) p.lgroup = 1;
   int off = stages * p.stage_bytes;
   p.off_out = off; off += out_bytes;
   p.off_hside = off; off += side_bytes;
@@ -1195,12 +1126,6 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
   int rc = gemm_plan(a, 0, pl);
   if (rc) return rc;
   GemmDev& p = pl.p;
-  if (p.dbg & 512) {
-    static unsigned long long* dbuf = nullptr;
-    if (!dbuf) cudaMalloc(&dbuf, 16 * sizeof(unsigned long long));
-    cudaMemsetAsync(dbuf, 0, 16 * sizeof(unsigned long long), stream);
-    p.dbg_buf = dbuf;
-  }
 
   // ---- tensor maps ----
   CUtensorMap tmA, tmB, tmA2, tmB2, tmD;
@@ -1271,16 +1196,6 @@ int gemm_launch(const yamb_gemm* a, cudaStream_t stream) {
     if (e != cudaSuccess) return fail("split-K reduce launch", e);
     rc = det_free(p.part, stream);
     if (rc) return rc;
-  }
-  if (p.dbg & 512) {
-    unsigned long long h[16];
-    cudaStreamSynchronize(stream);
-    cudaMemcpy(h, p.dbg_buf, sizeof(h), cudaMemcpyDeviceToHost);
-    const double lw_n = h[9] ? (double)h[9] : 1.0;
-    fprintf(stderr, "gemm dbg (cycles per loader warp): wait_empty %.0f wait_tma %.0f xform(incl wait_tma) %.0f "
-            "publish %.0f total %.0f (warps %.0f); stages %d out_bufs %d block_n %d tma %d%d wg2x %d\n",
-            h[12] / lw_n, h[13] / lw_n, h[14] / lw_n, h[15] / lw_n, h[8] / lw_n, lw_n, p.num_stages,
-            p.out_bufs, p.block_n, p.a_tma, p.b_tma, p.wg2x);
   }
   return 0;
 }

@@ -44,12 +44,9 @@ __device__ __forceinline__ void head_stage(uint8_t* dst, const __nv_bfloat16* sr
     const int kb = q >> 3, c = q & 7;
     const bool ok = r < rows_valid && q * 8 < Cin;
     const void* s = ok ? (const void*)(src + (size_t)r * Cin + q * 8) : (const void*)src;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(
-                     smem_u32(dst + kb * 8192 + r * 128 + ((c ^ (r & 7)) << 4))),
-                 "l"(s), "r"(ok ? 16 : 0)
-                 : "memory");
+    cp_async_zfill16(smem_u32(dst + kb * 8192 + r * 128 + ((c ^ (r & 7)) << 4)), s, ok ? 16 : 0);
   }
-  asm volatile("cp.async.commit_group;" ::: "memory");
+  cp_async_commit();
 }
 
 __global__ void __launch_bounds__(128) head_pool_eval_kernel(const __grid_constant__ HeadDev p) {
@@ -80,7 +77,7 @@ __global__ void __launch_bounds__(128) head_pool_eval_kernel(const __grid_consta
   for (int p0 = 0; p0 < p.HW; p0 += 64) {
     const int rows = min(64, p.HW - p0);
     head_stage(sA, img + (size_t)p0 * p.Cin, rows, p.Cin, p.kpanels);
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    cp_async_wait<0>();
     fence_proxy_async_smem();
     __syncthreads();
     float acc[32];

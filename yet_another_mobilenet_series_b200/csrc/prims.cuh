@@ -1,4 +1,5 @@
-// sm_90a device primitives: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
+// sm_90a device primitives: mbarrier, cp.async, shared-memory vectors, TMA (cp.async.bulk.tensor),
+// wgmma.
 // Everything here is inline PTX; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -94,49 +95,37 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// Wait where a few hundred ns of wake-up latency do not matter (epilogue waiting for an
-// accumulator): back off between polls so that the poller does not eat the issue slots of the
-// warps that do the work (ncu: the suspended try_wait loop was 19 % of all issued instructions).
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  uint64_t t0 = global_timer_ns();
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(256);
-    if (((++spins) & 0xfff) == 0) {
-      if (global_timer_ns() - t0 > 4000000000ull) {
-        printf("yamb: mbarrier timeout block %d thread %d bar %u parity %u\n", (int)blockIdx.x,
-               (int)threadIdx.x, smem_u32(bar), parity);
-        __trap();
-      }
-    }
-  }
+// ----------------------------------------------------------------------------------------------
+// cp.async (16-byte, L2 only) and 128-bit shared-memory accesses (32-bit shared addresses, never
+// generic)
+// ----------------------------------------------------------------------------------------------
+// copies src_bytes (16 or 0) from src and zero-fills the rest of the 16 bytes at dst: a copy with
+// src_bytes = 0 reads nothing, so src need only be a valid address
+__device__ __forceinline__ void cp_async_zfill16(uint32_t dst, const void* src, int src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes)
+               : "memory");
 }
-// Pure polling variant (no suspend): lowest wake-up latency, costs issue slots while waiting.
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// waits until at most N of this thread's committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
-  if (mbar_test_wait(bar, parity)) return;
-  uint64_t t0 = global_timer_ns();
-  uint32_t spins = 0;
-  while (!mbar_test_wait(bar, parity)) {
-    if (((++spins) & 0xfffff) == 0) {
-      if (global_timer_ns() - t0 > 4000000000ull) {
-        printf("yamb: mbarrier timeout block %d thread %d bar %u parity %u\n", (int)blockIdx.x,
-               (int)threadIdx.x, smem_u32(bar), parity);
-        __trap();
-      }
-    }
-  }
+__device__ __forceinline__ uint4 lds128(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ float4 lds128f(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ void sts128(uint32_t a, uint4 v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z),
+               "r"(v.w) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -239,16 +228,6 @@ __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t da, uint64
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
 

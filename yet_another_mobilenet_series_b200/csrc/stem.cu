@@ -63,7 +63,7 @@ constexpr int kStemSW = kStemIW + 1;                  // 66 staged columns
 constexpr int kStemRowWords = kStemSW * 3 / 2;        // 99 words per staged row
 
 // All copies of a tile are issued as asynchronous 4-byte cp.async (zero-filled outside the image)
-// and awaited ONCE by the caller (stem_stage_wait): a plain load loop exposed one DRAM round
+// and awaited ONCE by the caller (commit, then wait): a plain load loop exposed one DRAM round
 // trip per iteration, 13 per tile.
 __device__ __forceinline__ void stem_stage_input(const StemDev& p, int n, int ty, int tx,
                                                  __nv_bfloat16* s_in) {
@@ -90,10 +90,6 @@ __device__ __forceinline__ void stem_stage_input(const StemDev& p, int n, int ty
       dst[e] = (uint32_t)lo | ((uint32_t)hi << 16);
     }
   }
-}
-__device__ __forceinline__ void stem_stage_wait() {
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
 // generic 2-byte path (odd image widths)
@@ -234,7 +230,8 @@ __device__ __forceinline__ void stem_fwd_body(const StemDev& p) {
     if constexpr (kStemU8<T>) {
       if (aligned) {
         stem_u8_issue(p, n, ty, tx, s_bytes);
-        stem_stage_wait();
+        cp_async_commit();
+        cp_async_wait<0>();
         __syncthreads();
         stem_u8_convert(p, ty, tx, s_bytes, s_lut, s_in);
       } else {
@@ -242,7 +239,8 @@ __device__ __forceinline__ void stem_fwd_body(const StemDev& p) {
       }
     } else if (aligned) {
       stem_stage_input(p, n, ty, tx, s_in);
-      stem_stage_wait();
+      cp_async_commit();
+      cp_async_wait<0>();
     } else {
       stem_stage_generic(p, n, ty, tx, s_in);
     }
@@ -385,12 +383,10 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__
       const void* src = ok ? (const void*)(reinterpret_cast<const uint4*>(
                                  p.dh + (((size_t)n * p.Ho + oy) * p.Wo + ox) * p.Cout) + v)
                            : (const void*)p.dh;
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(
-                       smem_u32(reinterpret_cast<uint4*>(s_dh) + e)),
-                   "l"(src), "r"(ok ? 16 : 0)
-                   : "memory");
+      cp_async_zfill16(smem_u32(reinterpret_cast<uint4*>(s_dh) + e), src, ok ? 16 : 0);
     }
-    stem_stage_wait();
+    cp_async_commit();
+    cp_async_wait<0>();
     __syncthreads();
     if constexpr (kStemU8<T>) {
       if (aligned) {

@@ -7,9 +7,8 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# YAMB_LIB_PATH: an alternative build of the same sources (e.g. the -DYAMB_GEMM_TIMERS variant the
-# profiling drivers use); the default is the in-tree library __graft_entry__.build() produces
-LIB_PATH = os.environ.get("YAMB_LIB_PATH") or os.path.join(_HERE, "libyamb200.so")
+# the in-tree library __graft_entry__.build() produces
+LIB_PATH = os.path.join(_HERE, "libyamb200.so")
 
 ACT_NONE, ACT_RELU, ACT_RELU6, ACT_SWISH, ACT_HSWISH = 0, 1, 2, 3, 4
 
