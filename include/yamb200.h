@@ -468,6 +468,44 @@ typedef struct yamb_head_pool_eval {
 
 int yamb_head_pool_eval_fwd(const yamb_head_pool_eval* args, yamb_stream_t stream);
 
+/* ---- training-mode head: BatchNorm (batch statistics) + activation + full-extent average pool ----
+ * Follows yamb_pointwise_gemm of the head 1x1 convolution run with `bn_fwd`, whose epilogue took
+ * the batch statistics of its output h and wrote scale / shift, mean / invstd and the running
+ * statistics.  Replaces yamb_bn_apply_fwd -> torch's mean over the pixels, and in backward the
+ * broadcast of the pooled gradient -> yamb_bn_reduce_bwd -> yamb_bn_bwd_apply_bwd:
+ *   forward : pooled[n][c] = bf16((1/HW) * sum_p bf16(act(scale[c] * h[n,p,c] + shift[c])))
+ *             (the activation a is never written; the sum is fp32 in a fixed order: per-thread
+ *             pixel lanes, lanes in order, then pixel-chunk slabs in order; no atomics)
+ *   backward: dz = act'(scale*h + shift) * (dpooled[n][c] * (1/HW)), formed from h on the fly;
+ *             pass 1: sum(dz), sum(dz * xhat) per channel -> bn (dgamma, dbeta +=; ca, cb, cc),
+ *             the BatchNorm-backward finalize of yamb_bn_reduce_bwd (double across CTAs);
+ *             pass 2: dh = bf16(ca*dz + cb*h + cc), skipped when dh is NULL.
+ * C a multiple of 8, N * HW < 2^31, bf16 operands 16-byte aligned; bn.count must be N * HW.
+ * Other arguments return YAMB_EINVAL, with or without a device.  The forward takes a
+ * stream-ordered scratch of its own when it splits the pixels of an image over several CTAs. */
+typedef struct yamb_head_pool_train {
+  int32_t N, HW, C;
+  const void* h;          /* bf16 [N][HW][C] (NHWC), the head convolution's raw output */
+  const float* scale;     /* [C] */
+  const float* shift;     /* [C] */
+  int32_t act;            /* YAMB_ACT_* */
+  void* pooled;           /* out bf16 [N][C] */
+} yamb_head_pool_train;
+
+typedef struct yamb_head_pool_train_grad {
+  int32_t N, HW, C;
+  const void* h;          /* bf16 [N][HW][C], as in the forward */
+  const float* scale;     /* [C] the forward's coefficients (z = scale*h + shift) */
+  const float* shift;     /* [C] */
+  int32_t act;            /* YAMB_ACT_* */
+  const void* dpooled;    /* bf16 [N][C], gradient of pooled */
+  yamb_bn_bwd bn;         /* the forward's mean / invstd; dgamma, dbeta +=; ca, cb, cc out */
+  void* dh;               /* out bf16 [N][HW][C], or NULL */
+} yamb_head_pool_train_grad;
+
+int yamb_head_pool_train_fwd(const yamb_head_pool_train* args, yamb_stream_t stream);
+int yamb_head_pool_train_bwd(const yamb_head_pool_train_grad* args, yamb_stream_t stream);
+
 /* ---- label-smoothed softmax cross entropy + top-k -------------------------------------------------
  * Replaces CrossEntropyLabelSmooth(reduction='none') (reference utils/optim.py:150-158), the
  * top-1 / top-5 `correct_k` bookkeeping of forward_loss (common.py:73-79) and their backward.
@@ -612,7 +650,8 @@ int yamb_max_ctas(void);
  * 6 bn_reduce, 7 se_pool, 8 rmsprop, 9 se_bwd_reduce, 10 se_bwd_apply, 11 bn_stats,
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
  * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
- * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8) so bindings can
+ * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8, 29 expand_bwd_args,
+ * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad) so bindings can
  * self-check */
 int yamb_struct_size(int which);
 

@@ -14,49 +14,6 @@
 
 namespace yamb {
 
-__device__ __forceinline__ void unpack8(const uint4& u, float (&v)[8]) {
-  v[0] = bf16lo(u.x); v[1] = bf16hi(u.x); v[2] = bf16lo(u.y); v[3] = bf16hi(u.y);
-  v[4] = bf16lo(u.z); v[5] = bf16hi(u.z); v[6] = bf16lo(u.w); v[7] = bf16hi(u.w);
-}
-__device__ __forceinline__ uint4 pack8(const float (&v)[8]) {
-  return make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]),
-                    pack_bf16(v[6], v[7]));
-}
-
-// Merge the per-thread partial sums (s, q: 8 channels each) of the threads of a CTA that own the
-// same 8-channel group (tid = px * CG + cg, px < PX) into the CTA's statistics slots WITHOUT
-// atomics: staged through shared memory and summed in pixel-lane order by the px == 0 thread, in
-// double.  (Shared-memory double atomics are CAS loops; PX threads contending for every slot cost
-// bn_reduce 20 %.)  Must be called by ALL threads of the CTA; `active` = this thread holds sums.
-__device__ __forceinline__ void cta_stats_merge(stat_t* s_part, int C, int CG, int PX, int cg, int px,
-                                                bool active, const float (&s)[8],
-                                                const float (&q)[8]) {
-  __shared__ float red[256][17];
-  if (active) {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      red[threadIdx.x][e] = s[e];
-      red[threadIdx.x][8 + e] = q[e];
-    }
-  }
-  __syncthreads();
-  if (active && px == 0) {
-    const int c0 = cg * 8;
-    const int base = threadIdx.x;              // = cg (relative to this pass) when px == 0
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      stat_t a = 0.0, b = 0.0;
-      for (int j = 0; j < PX; ++j) {
-        a += (stat_t)red[base + j * CG][e];
-        b += (stat_t)red[base + j * CG][8 + e];
-      }
-      s_part[c0 + e] += a;
-      s_part[C + c0 + e] += b;
-    }
-  }
-  __syncthreads();
-}
-
 struct BnApplyDev {
   long long M;
   int C, ldh, ldr, ldy;

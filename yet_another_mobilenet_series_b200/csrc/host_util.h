@@ -52,6 +52,8 @@ int stem_conv_u8_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
 int stem_conv_u8_wgrad_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
 int stem_conv_u8_eval_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
 int head_pool_eval_launch(const yamb_head_pool_eval* a, cudaStream_t stream);
+int head_pool_train_fwd_launch(const yamb_head_pool_train* a, cudaStream_t stream);
+int head_pool_train_bwd_launch(const yamb_head_pool_train_grad* a, cudaStream_t stream);
 int nl_gram_launch(const yamb_nl_gram* a, cudaStream_t stream);
 int nl_rowmat_launch(const yamb_nl_rowmat* a, cudaStream_t stream);
 int block_eval_launch(const yamb_block_eval* a, cudaStream_t stream);

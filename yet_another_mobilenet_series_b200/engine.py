@@ -1405,6 +1405,16 @@ EVAL_FUSED_CALLS = 0     # blocks that went through yamb_block_eval_fwd (tests /
 EVAL_TAIL_FUSED = False
 EVAL_TAIL_CALLS = 0      # stem / head calls that went through the one-launch kernels (tests)
 
+# ---- training mode: head BatchNorm + activation + average pool (tail_ops.head_pool_train) ---------
+# Off by default: the pool's fixed summation order is not torch's, so turning it on changes the bits
+# of a training step.  When True (trainer.TrainStep(fused_tail=True) turns it on for its own
+# forwards and backwards) the head ConvBNReLU 1x1 followed by the full-extent average pool runs as
+# the head GEMM + yamb_head_pool_train_fwd, backward yamb_head_pool_train_bwd, whenever the
+# BatchNorm uses batch statistics and the kernels cover the shape: the activation and its broadcast
+# gradient never reach HBM.  Otherwise the unfused sequence runs.
+TRAIN_TAIL_FUSED = False
+TRAIN_TAIL_CALLS = 0     # head calls that went through yamb_head_pool_train_fwd (tests)
+
 
 def _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p):
     """bf16 tensor-core operands of the expand / project weights (the optimizer's mirrors when

@@ -57,7 +57,7 @@ def _full_extent(pool, x):
 # step includes the input's conversion to bf16 channels_last), each block, the head, the pool and
 # model.classifier (its step includes the cast of the logits to fp32).  The time between two
 # consecutive events is the device time of the step the second one ends.  A head run together with
-# the pool (engine.EVAL_TAIL_FUSED) is one step, recorded for the head.
+# the pool (engine.EVAL_TAIL_FUSED, engine.TRAIN_TAIL_FUSED) is one step, recorded for the head.
 STEPS = None
 
 
@@ -95,10 +95,14 @@ def run_features(model, x):
                     _step_done(stream, layer)
                     continue
                 nxt = layers[i + 1] if i + 1 < len(layers) else None
-                if (engine.EVAL_TAIL_FUSED and isinstance(layer, ConvBNReLU)
+                if ((engine.EVAL_TAIL_FUSED or engine.TRAIN_TAIL_FUSED)
+                        and isinstance(layer, ConvBNReLU)
                         and isinstance(nxt, nn.AvgPool2d) and _full_extent(nxt, x)):
-                    # eval: head 1x1 ConvBNReLU + global average pool in one launch (when covered)
-                    y = tail_ops.head_pool_eval(layer, x)
+                    # head 1x1 ConvBNReLU + global average pool: in eval one launch, in training
+                    # the head GEMM + one pooling kernel (when covered)
+                    y = tail_ops.head_pool_eval(layer, x) if engine.EVAL_TAIL_FUSED else None
+                    if y is None and engine.TRAIN_TAIL_FUSED:
+                        y = tail_ops.head_pool_train(layer, x)
                     if y is not None:
                         x, skip = y, True
                         _step_done(stream, layer)

@@ -262,6 +262,24 @@ class HeadPoolEval(C.Structure):
     ]
 
 
+class HeadPoolTrain(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32),
+        ("h", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p), ("act", C.c_int32),
+        ("pooled", C.c_void_p),
+    ]
+
+
+class HeadPoolTrainGrad(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32),
+        ("h", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p), ("act", C.c_int32),
+        ("dpooled", C.c_void_p),
+        ("bn", BnBwd),
+        ("dh", C.c_void_p),
+    ]
+
+
 class BnEval(C.Structure):
     _fields_ = [
         ("gamma", C.c_void_p), ("beta", C.c_void_p),
@@ -354,11 +372,11 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
             14: NlRowmat, 15: SeFc, 16: SeFcBwd, 17: SoftmaxCe, 18: SoftmaxCeGrad,
             19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd, 24: Sgd,
             25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
-            29: ExpandBwd, 30: ExpandBwdPlanInfo}
+            29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_head_pool_eval_fwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -410,6 +428,8 @@ def lib():
         for fn in (l.yamb_stem_conv_u8_fwd, l.yamb_stem_conv_u8_wgrad, l.yamb_stem_conv_u8_eval_fwd):
             fn.argtypes = [C.POINTER(StemConvU8), C.c_void_p]
         l.yamb_head_pool_eval_fwd.argtypes = [C.POINTER(HeadPoolEval), C.c_void_p]
+        l.yamb_head_pool_train_fwd.argtypes = [C.POINTER(HeadPoolTrain), C.c_void_p]
+        l.yamb_head_pool_train_bwd.argtypes = [C.POINTER(HeadPoolTrainGrad), C.c_void_p]
         l.yamb_se_fc_fwd.argtypes = [C.POINTER(SeFc), C.c_void_p]
         l.yamb_se_fc_bwd.argtypes = [C.POINTER(SeFcBwd), C.c_void_p]
         l.yamb_nl_gram_fwd.argtypes = [C.POINTER(NlGram), C.c_void_p]

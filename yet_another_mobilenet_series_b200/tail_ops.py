@@ -145,6 +145,79 @@ def head_pool_eval(mod, x):
     return pooled.view(N, Cout, 1, 1)
 
 
+class _HeadPoolTrainFn(torch.autograd.Function):
+    """pooled[N, C] = the pixel mean of act(BatchNorm(h)), BatchNorm on the batch statistics the
+    head GEMM's epilogue took (yamb_head_pool_train_fwd); backward: dh from dpooled in two passes
+    (yamb_head_pool_train_bwd), dgamma / dbeta through engine.GradTargets."""
+
+    @staticmethod
+    def forward(ctx, h, bn, act, weight, bias):
+        b = engine._bn_act_state(bn, h.device).bn
+        N, Cc, H, W = h.shape
+        pooled = torch.empty(N, Cc, device=h.device, dtype=torch.bfloat16)
+        a = nat.HeadPoolTrain()
+        a.N, a.HW, a.C = N, H * W, Cc
+        a.h, a.scale, a.shift, a.act = h.data_ptr(), b.scale.data_ptr(), b.shift.data_ptr(), act
+        a.pooled = pooled.data_ptr()
+        engine.launch(nat.lib().yamb_head_pool_train_fwd, a, "head_pool_train",
+                      2 * N * Cc * (H * W + 1))
+        ctx.bn, ctx.act = bn, act
+        # this call's coefficients, as _BnActFn keeps them (another forward through the module
+        # before this backward, e.g. the next micro-batch, rewrites the live ones)
+        coef = torch.stack((b.scale, b.shift, b.mean, b.invstd)) if any(ctx.needs_input_grad) \
+            else None
+        ctx.save_for_backward(h, coef)
+        return pooled
+
+    @staticmethod
+    def backward(ctx, dpooled):
+        h, coef = ctx.saved_tensors
+        bn = ctx.bn
+        b = engine._bn_act_state(bn, h.device).bn
+        N, Cc, H, W = h.shape
+        M = N * H * W
+        dpooled = dpooled.to(torch.bfloat16).contiguous()
+        gt = engine.GradTargets((bn.weight, bn.bias))
+        g = nat.HeadPoolTrainGrad()
+        g.N, g.HW, g.C = N, H * W, Cc
+        g.h, g.act = h.data_ptr(), ctx.act
+        g.scale, g.shift = coef[0].data_ptr(), coef[1].data_ptr()
+        g.dpooled = dpooled.data_ptr()
+        g.bn = b.bwd_struct(M, [(gt.of(bn.weight), gt.of(bn.bias))])
+        g.bn.mean, g.bn.invstd = coef[2].data_ptr(), coef[3].data_ptr()
+        dh = None
+        if ctx.needs_input_grad[0]:
+            dh = torch.empty_like(h, memory_format=torch.channels_last)
+            g.dh = dh.data_ptr()
+        engine.launch(nat.lib().yamb_head_pool_train_bwd, g, "head_pool_train_bwd",
+                      2 * M * Cc * (3 if dh is not None else 1))
+        return (dh, None, None) + gt.result()
+
+
+def head_pool_train_covered(mod, x):
+    """Whether head_pool_train runs ConvBNReLU `mod` on x: engine.TRAIN_TAIL_FUSED is on, the
+    BatchNorm normalises with batch statistics and the GEMM and the kernels cover the layer (the
+    caller checks that an average pool over the whole map follows)."""
+    bn = mod[1]
+    return (engine.TRAIN_TAIL_FUSED and (bn.training or not bn.track_running_stats)
+            and pw_conv_supported(mod, x))
+
+
+def head_pool_train(mod, x):
+    """Training-mode head ConvBNReLU 1x1 followed by the full-extent average pool: the head GEMM
+    (BatchNorm statistics in its epilogue) -> yamb_head_pool_train_fwd, bf16 [N, Cout, 1, 1]; or
+    None when the call is not covered (head_pool_train_covered) and the caller runs the unfused
+    sequence."""
+    if not head_pool_train_covered(mod, x):
+        return None
+    x = engine.to_nhwc_bf16(x)
+    conv, bn, act = mod[0], mod[1], mod[2]
+    h = _PwConvFn.apply(x, conv, bn, conv.weight)
+    pooled = _HeadPoolTrainFn.apply(h, bn, engine.act_code_of(act), bn.weight, bn.bias)
+    engine.TRAIN_TAIL_CALLS += 1
+    return pooled.view(pooled.shape[0], pooled.shape[1], 1, 1)
+
+
 def pw_conv_supported(mod, x):
     conv, bn, act = mod[0], mod[1], mod[2]
     return (x.is_cuda and conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.groups == 1

@@ -85,7 +85,7 @@ class TrainStep:
                  alpha=0.9, momentum=0.9, eps=1e-3, weight_decay=1e-5, label_smoothing=0.1,
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
-                 input_norm=None, micro_batch=None):
+                 input_norm=None, micro_batch=None, fused_tail=False):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
@@ -99,7 +99,13 @@ class TrainStep:
         reference's per-GPU local BatchNorm at per_gpu_batch_size = micro_batch: batch statistics
         are those of each micro-batch, the running statistics are updated once per micro-batch (k
         times per step), and their EMA shadow once per step.  `micro_batch` is not part of a
-        checkpoint: one written with any k loads into a TrainStep with any other."""
+        checkpoint: one written with any k loads into a TrainStep with any other.
+
+        `fused_tail=True` runs the head BatchNorm + activation and the global average pool of this
+        step's forwards and backwards as one kernel each way (engine.TRAIN_TAIL_FUSED): the
+        activation and its broadcast gradient stay out of HBM.  Off by default: the pool sums in
+        its own fixed order, not torch's, so a step with it differs from the default in the last
+        bits.  A plain `model(x)` outside the step is not affected."""
         self.world = udist.get_world_size_fallback()
         self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
             per_gpu_batch, micro_batch, self.world, base_lr, base_total_batch, ema_decay,
@@ -111,6 +117,7 @@ class TrainStep:
             raise RuntimeError("TrainStep needs the model on a CUDA device (no CPU path)")
         self.dev = dev
         self.batch = per_gpu_batch
+        self.fused_tail = bool(fused_tail)
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
                                eps=eps, eps_inside_sqrt=True, weight_decay=0)
@@ -178,8 +185,13 @@ class TrainStep:
         their number k); any other batch of n rows (a partial last batch) weights the mean of a
         pass of n_i rows by n_i / n, a device scalar, so its gradient is that of the mean over the
         n rows."""
-        x = self.x if x is None else x
-        t = self.t if t is None else t
+        engine.TRAIN_TAIL_FUSED = self.fused_tail
+        try:
+            self._passes(self.x if x is None else x, self.t if t is None else t)
+        finally:
+            engine.TRAIN_TAIL_FUSED = False
+
+    def _passes(self, x, t):
         n, b = x.shape[0], self.micro_batch
         self.opt.zero_grad()
         if n <= b:
