@@ -78,8 +78,8 @@ def test_cluster_size_rule_limits():
     # the tile plan: two 7x7 images per tile below 161 output channels, one above
     assert engine.eval_tiles(3, 1, 5, 7, 7, 160) == 3
     assert engine.eval_tiles(3, 1, 5, 7, 7, 320) == 5
-    assert engine.eval_tiles(3, 1, 1, 28, 28, 32) == 8      # 7x14 tiles
-    assert engine.eval_tiles(3, 1, 1, 56, 56, 24) == 32     # 7x14 and 7x16 tie
+    assert engine.eval_tiles(3, 1, 1, 28, 28, 32) == 8      # 7x16 tiles
+    assert engine.eval_tiles(3, 1, 1, 56, 56, 24) == 32     # 7x16 tiles (two 7x7 images: 64)
     assert engine.eval_tiles(5, 2, 1, 56, 56, 32) == 80     # k5 stride 2: 6x7 outputs
     assert engine.eval_tiles(7, 2, 1, 28, 28, 40) == 28     # k7 stride 2: 4x7 outputs
 
@@ -126,7 +126,11 @@ def ptxas_report(tmp_path_factory):
     return r.stdout + r.stderr
 
 
-def test_cluster_instantiations_spill_nothing(ptxas_report):
+def test_cluster_instantiations_match_the_tile_plan_and_spill_nothing(ptxas_report):
+    """One cluster kernel per (tile geometry, expansion) pair the launcher names (parsed out of the
+    header, tests/block_eval_cases.py) x (lean, generic activation) x (plain, gate, pool), and none
+    of them spills."""
+    import block_eval_cases as bc
     kernels, cur = {}, None
     for line in ptxas_report.splitlines():
         m = re.search(r"Compiling entry function '(\w+)'", line)
@@ -137,9 +141,21 @@ def test_cluster_instantiations_spill_nothing(ptxas_report):
             continue
         if cur:
             kernels[cur].append(line)
-    # 17 tile geometries x (lean, generic activation) x (plain, gate, pool), all with CLUSTER
-    assert len(kernels) == 102, sorted(kernels)
     assert all(name.endswith("Lb1EEEv14CUtensorMap_stS3_S3_NS_12BlockEvalDevE") for name in kernels)
+    # block_eval_kernel<EvGeom<K, S, TOH, TOW, TI, CPT>, EXPAND, LEAN, MODE, CLUSTER = true>
+    pat = re.compile(r"EvGeomILi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)EEELb([01])ELb([01])"
+                     r"ELi(\d)ELb1E")
+    got = set()
+    for name in kernels:
+        m = pat.search(name)
+        assert m, name
+        v = tuple(int(g) for g in m.groups())
+        got.add((bc.Geom(*v[:6]), bool(v[6]), bool(v[7]), v[8]))
+    want = {(g, ex, lean, mode) for g, ex in bc.compiled_instantiations()
+            for lean in (False, True) for mode in (0, 1, 2)}
+    assert got == want, (sorted(got - want), sorted(want - got))
+    # 14 (tile geometry, expansion) pairs x (lean, generic activation) x (plain, gate, pool)
+    assert len(kernels) == len(want) == 84, sorted(kernels)
     for name, lines in kernels.items():
         props = " ".join(lines)
         m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", props)

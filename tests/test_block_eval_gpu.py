@@ -53,7 +53,7 @@ def _make_block(cin, chid, cout, act, seed, stride=1, expand=True, k=3):
 # (cin, chid, cout, N, H, W, act)
 CASES = [
     (24, 144, 24, 4, 56, 56, "relu"),      # MobileNetV2 block 3: K pad, N pad, partial slice
-    (32, 192, 32, 4, 28, 28, "relu6"),     # 7x14 tiles
+    (32, 192, 32, 4, 28, 28, "relu6"),     # 7x16 tiles, as many as two 7x7 images
     (64, 384, 64, 6, 14, 14, "relu"),
     (64, 384, 96, 5, 14, 14, "relu"),      # block 11: no skip connection
     (96, 576, 96, 3, 14, 14, "relu6"),
@@ -76,7 +76,7 @@ CASES = [
     (24, 24, 40, 2, 30, 30, "relu", 2, False),      # no expansion + stride 2
     # 5x5 / 7x7 depthwise (Proxyless-mobile, apps/mobilenet/proxyless_mobile_mnas.yml)
     (16, 48, 32, 2, 112, 112, "relu6", 2, True, 5),   # 112 -> 56, k5 s2: 6x7 outputs per tile
-    (40, 120, 40, 3, 28, 28, "relu6", 1, True, 5),    # k5 s1, 7x14 tiles
+    (40, 120, 40, 3, 28, 28, "relu6", 1, True, 5),    # k5 s1, 7x16 tiles
     (80, 240, 80, 3, 14, 14, "relu6", 1, True, 5),
     (96, 288, 96, 5, 7, 7, "relu", 1, True, 5),       # two images per tile, 5x5
     (32, 96, 40, 2, 56, 56, "relu6", 2, True, 7),     # k7 s2: 4x7 outputs from a 13x19 tile

@@ -7,8 +7,8 @@
 // under torch.no_grad()).  With the statistics known up front the block is a pure function of an
 // input tile plus a one-pixel halo: SURVEY.md §7.1 step 2 / §7.2, BASELINE.json's "fused block".
 //
-// Persistent CTAs (one per SM) walk output tiles of <= 112 pixels (k = 3, stride 1: 7x16, 7x14 or
-// two 7x7 images; stride 2, k = 5 / 7 and wide outputs: smaller tiles) whose input tile with its
+// Persistent CTAs (one per SM) walk output tiles of <= 112 pixels (k = 3 / 5, stride 1: 7x16 or
+// two 7x7 images; stride 2, k = 7 and wide outputs: smaller tiles) whose input tile with its
 // halo fits 256 rows.  Per tile:
 //   x tile (+halo, <= 256 pixels) --TMA 4-D box, zero fill outside the image--> smem (A operand)
 //   for every 64-channel slice of the hidden dimension:
@@ -805,6 +805,8 @@ static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, boo
   p.NC = (a->Chid + 63) / 64;
   const bool ex = a->w_expand != nullptr;
   // fewest tiles among the geometries of (k, stride); each holds its input tile in <= 256 rows.
+  // Stride 1, k = 3 / 5: 7x16 unless two 7x7 images per tile take fewer (a 7x14 tile never would:
+  // ceil(Wo / 16) <= ceil(Wo / 14)).
   // Tiles of more than 64 output pixels keep 64 x Npad project accumulators per thread: wide
   // outputs (Npad > 160) take one 7x7 image per tile instead.
   const bool wide = p.Npad > 16 * kMaxProjChunks;
@@ -818,22 +820,17 @@ static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, boo
     if (wide)
       return ex ? launch_eval<EvGeom<3, 1, 7, 7, 1, 4>, true, CLUSTER>(p, a, st)
                 : launch_eval<EvGeom<3, 1, 7, 7, 1, 4>, false, CLUSTER>(p, a, st);
-    const long long t0 = tiles_of(7, 16, 1), t1 = tiles_of(7, 14, 1), t2 = tiles_of(7, 7, 2);
-    if (t0 <= t1 && t0 <= t2)
+    if (tiles_of(7, 16, 1) <= tiles_of(7, 7, 2))
       return ex ? launch_eval<EvGeom<3, 1, 7, 16, 1, 4>, true, CLUSTER>(p, a, st)
                 : launch_eval<EvGeom<3, 1, 7, 16, 1, 4>, false, CLUSTER>(p, a, st);
-    if (t1 <= t2)
-      return ex ? launch_eval<EvGeom<3, 1, 7, 14, 1, 4>, true, CLUSTER>(p, a, st)
-                : launch_eval<EvGeom<3, 1, 7, 14, 1, 4>, false, CLUSTER>(p, a, st);
     return ex ? launch_eval<EvGeom<3, 1, 7, 7, 2, 4>, true, CLUSTER>(p, a, st)
               : launch_eval<EvGeom<3, 1, 7, 7, 2, 4>, false, CLUSTER>(p, a, st);
   }
   if (a->kernel == 5) {
     if (a->stride == 2) return launch_eval<EvGeom<5, 2, 6, 7, 1, 2>, true, CLUSTER>(p, a, st);
     if (wide) return launch_eval<EvGeom<5, 1, 7, 7, 1, 4>, true, CLUSTER>(p, a, st);
-    const long long t0 = tiles_of(7, 16, 1), t1 = tiles_of(7, 14, 1), t2 = tiles_of(7, 7, 2);
-    if (t0 <= t1 && t0 <= t2) return launch_eval<EvGeom<5, 1, 7, 16, 1, 4>, true, CLUSTER>(p, a, st);
-    if (t1 <= t2) return launch_eval<EvGeom<5, 1, 7, 14, 1, 4>, true, CLUSTER>(p, a, st);
+    if (tiles_of(7, 16, 1) <= tiles_of(7, 7, 2))
+      return launch_eval<EvGeom<5, 1, 7, 16, 1, 4>, true, CLUSTER>(p, a, st);
     return launch_eval<EvGeom<5, 1, 7, 7, 2, 4>, true, CLUSTER>(p, a, st);
   }
   if (a->stride == 2) return launch_eval<EvGeom<7, 2, 4, 7, 1, 2>, true, CLUSTER>(p, a, st);

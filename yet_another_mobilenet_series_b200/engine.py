@@ -1498,7 +1498,7 @@ def eval_tiles(k, stride, N, Ho, Wo, Cout):
         return tiles({3: 7, 5: 6, 7: 4}[k], 7, 1)
     if k == 7 or (Cout + 15) // 16 * 16 > 160:   # 7x7 depthwise, or a project wider than 160
         return tiles(7, 7, 1)
-    return min(tiles(7, 16, 1), tiles(7, 14, 1), tiles(7, 7, 2))
+    return min(tiles(7, 16, 1), tiles(7, 7, 2))
 
 
 def eval_cluster_size(k, stride, N, Ho, Wo, Chid, Cout, sms):
