@@ -448,6 +448,46 @@ int yamb_stem_conv_u8_fwd(const yamb_stem_conv_u8* args, yamb_stream_t stream);
 int yamb_stem_conv_u8_wgrad(const yamb_stem_conv_u8* args, yamb_stream_t stream);
 int yamb_stem_conv_u8_eval_fwd(const yamb_stem_conv_u8* args, yamb_stream_t stream);
 
+/* ---- training-mode stem: BatchNorm statistics in the convolution, BatchNorm backward on load ------
+ * For a stem ConvBNReLU whose only consumer applies the stem's BatchNorm + activation on load and
+ * returns dz = da * act'(z) with the BatchNorm-backward statistics (yamb_dw_fwd in_scale /
+ * in_shift, yamb_dw_bwd dx / bn: the depthwise of a first block without expansion), so neither the
+ * activation nor its gradient nor dh reaches HBM:
+ *   fwd  : y = the bits of yamb_stem_conv_fwd, plus the batch statistics of y finalised through
+ *          `bn` (scale / shift, saved mean / invstd, running statistics, num_batches_tracked) as
+ *          yamb_bn_stats_fwd does; per-thread fp32 sums in a fixed order, double across warps
+ *          and CTAs
+ *   wgrad: dw += sum dh * x with dh = bf16(fmaf(ca, dz, fmaf(cb, h, cc))) formed on load (the
+ *          expression of yamb_bn_bwd_apply_bwd, 0 outside the image), the partial slabs and their
+ *          order those of yamb_stem_conv_wgrad: dw is bitwise yamb_bn_bwd_apply_bwd followed by
+ *          yamb_stem_conv_wgrad, the same on every run
+ * x_u8 = 1: x is uint8 [N][H][W][3] normalised while staged, as yamb_stem_conv_u8 with mean / std.
+ * Cout in {8, 16, 32, 64}; y, dz, h 16-byte aligned; bn.count = N*Ho*Wo.  Other arguments return
+ * YAMB_EINVAL before any device work, with or without a device; YAMB_ENODEV without one. */
+typedef struct yamb_stem_conv_train {
+  int32_t N, H, W, Cout;
+  const void* x;          /* bf16, or uint8 with x_u8 = 1: [N][H][W][3] */
+  int32_t x_u8;
+  float mean[3], std[3];  /* x_u8 = 1: staged x = bf16(((float)u / 255 - mean[c]) / std[c]) */
+  const float* w;         /* [Cout][3][3][3] */
+  void* y;                /* out bf16 [N][Ho][Wo][Cout], the raw convolution output h */
+  const yamb_bn_fwd* bn;  /* the BatchNorm of y (batch statistics) */
+} yamb_stem_conv_train;
+
+typedef struct yamb_stem_conv_train_grad {
+  int32_t N, H, W, Cout;
+  const void* x;          /* as in the forward */
+  int32_t x_u8;
+  float mean[3], std[3];
+  const void* dz;         /* bf16 [N][Ho][Wo][Cout]: gradient of the BatchNorm's output z */
+  const void* h;          /* bf16 [N][Ho][Wo][Cout]: the forward's y */
+  const float* ca; const float* cb; const float* cc;   /* [Cout] BatchNorm-backward coefficients */
+  float* dw;              /* [Cout][3][3][3] += */
+} yamb_stem_conv_train_grad;
+
+int yamb_stem_conv_train_fwd(const yamb_stem_conv_train* args, yamb_stream_t stream);
+int yamb_stem_conv_train_wgrad(const yamb_stem_conv_train_grad* args, yamb_stream_t stream);
+
 /* ---- eval-mode head: 1x1 ConvBNReLU + full-extent average pool, ONE launch ------------------------
  * Replaces, in eval mode, the head ConvBNReLU (reference models/mobilenet_supernet.py:152-158) and
  * the AvgPool2d over the whole final feature map (:159):
@@ -651,8 +691,8 @@ int yamb_max_ctas(void);
  * 12 bn_bwd_apply, 13 nl_gram, 14 nl_rowmat, 15 se_fc, 16 se_fc_grad, 17 softmax_ce,
  * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
  * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8, 29 expand_bwd_args,
- * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad) so bindings can
- * self-check */
+ * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad, 33 stem_conv_train,
+ * 34 stem_conv_train_grad) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

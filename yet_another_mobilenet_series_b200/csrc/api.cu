@@ -144,6 +144,8 @@ int yamb_struct_size(int which) {
     case 30: return (int)sizeof(yamb_expand_bwd_plan_info);
     case 31: return (int)sizeof(yamb_head_pool_train);
     case 32: return (int)sizeof(yamb_head_pool_train_grad);
+    case 33: return (int)sizeof(yamb_stem_conv_train);
+    case 34: return (int)sizeof(yamb_stem_conv_train_grad);
     default: return -1;
   }
 }
@@ -185,6 +187,8 @@ int yamb_stem_conv_eval_fwd(const yamb_stem_conv_eval* a, yamb_stream_t s) { ret
 int yamb_stem_conv_u8_fwd(const yamb_stem_conv_u8* a, yamb_stream_t s) { return yamb::stem_conv_u8_fwd_launch(a, YAMB_ST(s)); }
 int yamb_stem_conv_u8_wgrad(const yamb_stem_conv_u8* a, yamb_stream_t s) { return yamb::stem_conv_u8_wgrad_launch(a, YAMB_ST(s)); }
 int yamb_stem_conv_u8_eval_fwd(const yamb_stem_conv_u8* a, yamb_stream_t s) { return yamb::stem_conv_u8_eval_fwd_launch(a, YAMB_ST(s)); }
+int yamb_stem_conv_train_fwd(const yamb_stem_conv_train* a, yamb_stream_t s) { return yamb::stem_conv_train_fwd_launch(a, YAMB_ST(s)); }
+int yamb_stem_conv_train_wgrad(const yamb_stem_conv_train_grad* a, yamb_stream_t s) { return yamb::stem_conv_train_wgrad_launch(a, YAMB_ST(s)); }
 int yamb_head_pool_eval_fwd(const yamb_head_pool_eval* a, yamb_stream_t s) { return yamb::head_pool_eval_launch(a, YAMB_ST(s)); }
 int yamb_head_pool_train_fwd(const yamb_head_pool_train* a, yamb_stream_t s) { return yamb::head_pool_train_fwd_launch(a, YAMB_ST(s)); }
 int yamb_head_pool_train_bwd(const yamb_head_pool_train_grad* a, yamb_stream_t s) { return yamb::head_pool_train_bwd_launch(a, YAMB_ST(s)); }

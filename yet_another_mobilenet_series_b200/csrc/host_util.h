@@ -51,6 +51,8 @@ int stem_conv_eval_fwd_launch(const yamb_stem_conv_eval* a, cudaStream_t stream)
 int stem_conv_u8_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
 int stem_conv_u8_wgrad_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
 int stem_conv_u8_eval_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t stream);
+int stem_conv_train_fwd_launch(const yamb_stem_conv_train* a, cudaStream_t stream);
+int stem_conv_train_wgrad_launch(const yamb_stem_conv_train_grad* a, cudaStream_t stream);
 int head_pool_eval_launch(const yamb_head_pool_eval* a, cudaStream_t stream);
 int head_pool_train_fwd_launch(const yamb_head_pool_train* a, cudaStream_t stream);
 int head_pool_train_bwd_launch(const yamb_head_pool_train_grad* a, cudaStream_t stream);

@@ -23,12 +23,17 @@
 // values come from a [3][256] table each CTA builds once.  From the staged tile on, the code is
 // that of the bf16 instantiation, so the results are bitwise those of the bf16 entry points on the
 // host-normalised image.
+//
+// Training variants (yamb_stem_conv_train_*): the forward also takes the BatchNorm statistics of
+// h, the wgrad forms dh from dz and h on load; both for either input type, the kernels above
+// unchanged.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 #include <cmath>
 #include <type_traits>
 
+#include "bn_finalize.cuh"
 #include "host_util.h"
 #include "prims.cuh"
 
@@ -197,8 +202,20 @@ __device__ __forceinline__ bool stem_aligned(const StemDev& p) {
 // between the accumulators and the staging, with the expression and rounding points of
 // bn_apply_kernel (elementwise.cu): y = bf16(act(fmaf(scale, bf16(conv), shift))).
 // T: the type of x (__nv_bfloat16, or uint8_t normalised while it is staged).
-template <bool EVAL, typename T>
-__device__ __forceinline__ void stem_fwd_body(const StemDev& p) {
+// STATS (training forward, yamb_stem_conv_train_fwd): the batch statistics of the stored bf16 y,
+// read back from each warp's output staging: lane = (channel cl, pixel group pg), fp32 sums over
+// the warp's valid pixels in a fixed order, carried across tiles; at the end the 8 warps' and the
+// pixel groups' sums are added in double in a fixed order, published to `bn` and finalised by the
+// last CTA (bn_finalize.cuh).  Cout in {8, 16, 32, 64}.
+// The BatchNorm finalize of the bf16 training forward as a call: inlined at the kernel's
+// 80-register bound it spilled 4 bytes (ptxas -v), while the uint8 kernel spilled with the call and
+// not with the inlined code.
+__device__ __noinline__ void stem_bn_fwd_finalize(const yamb_bn_fwd* f, int C) {
+  bn_fwd_finalize(*f, C);
+}
+
+template <bool EVAL, typename T, bool STATS = false>
+__device__ __forceinline__ void stem_fwd_body(const StemDev& p, const yamb_bn_fwd* bn = nullptr) {
   extern __shared__ __align__(16) unsigned char stem_smem[];
   float* s_w = reinterpret_cast<float*>(stem_smem);                // [tap*3+ci][co], 27*64 floats
   __nv_bfloat16* s_in = reinterpret_cast<__nv_bfloat16*>(s_w + 27 * 64);   // [IH][SW][3]
@@ -223,6 +240,19 @@ __device__ __forceinline__ void stem_fwd_body(const StemDev& p) {
   }
   const int ry = threadIdx.x / 16, cp = threadIdx.x % 16;          // output row, column pair
   const bool aligned = stem_aligned<T>(p);
+  // STATS: channels cl and cl + 32 (Cout = 64) of every G-th pixel of the warp's staging; the
+  // running sums [sum_j0, sum_j1, sq_j0, sq_j1][thread] live in shared memory after the output
+  // staging and the uint8 area (in registers they spilled the bf16 kernel at its 80-register
+  // bound); the pointer is formed where it is used, for the same reason
+  auto stat_area = [&]() {
+    return reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(reinterpret_cast<uint4*>(
+               s_in + ((kStemIH * kStemSW * 3 + 7) & ~7)) + 8 * 64 * (p.Cout / 8)) +
+               (kStemU8<T> ? kStemU8Smem : 0));
+  };
+  if constexpr (STATS) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) stat_area()[k * 256 + threadIdx.x] = 0.f;
+  }
   for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
     const int n = t / (p.tiles_h * p.tiles_w), r = t % (p.tiles_h * p.tiles_w);
     const int ty = r / p.tiles_w, tx = r % p.tiles_w;
@@ -315,7 +345,62 @@ __device__ __forceinline__ void stem_fwd_body(const StemDev& p) {
         reinterpret_cast<uint4*>(p.y + (((size_t)n * p.Ho + oy) * p.Wo + ox0) * p.Cout)[within] =
             s_out[q];
     }
+    if constexpr (STATS) {
+      const __nv_bfloat16* sb = reinterpret_cast<const __nv_bfloat16*>(s_out);   // [64][Cout]
+      const int CL = p.Cout < 32 ? p.Cout : 32, G = 32 / CL, cl = lane % CL;
+      float* s_stat = stat_area();
+      float st_s[2], st_q[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        st_s[j] = s_stat[j * 256 + threadIdx.x];
+        st_q[j] = s_stat[(2 + j) * 256 + threadIdx.x];
+      }
+#pragma unroll 1
+      for (int q = lane / CL; q < 64; q += G) {
+        if (ty * kStemTH + wrow + (q >> 5) < p.Ho && ox0 + (q & 31) < p.Wo) {
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            if (j == 0 || p.Cout == 64) {
+              const float v = __bfloat162float(sb[q * p.Cout + cl + j * 32]);
+              st_s[j] += v;
+              st_q[j] = fmaf(v, v, st_q[j]);
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        s_stat[j * 256 + threadIdx.x] = st_s[j];
+        s_stat[(2 + j) * 256 + threadIdx.x] = st_q[j];
+      }
+    }
     __syncwarp();
+  }
+  if constexpr (STATS) {
+    // the CTA's sums in double go to the input tile, free now
+    __syncthreads();
+    stat_t* s_part = reinterpret_cast<stat_t*>(s_in);
+    const float* s_stat = stat_area();
+    const int CL = p.Cout < 32 ? p.Cout : 32, G = 32 / CL;
+    if (threadIdx.x < p.Cout) {
+      const int c = threadIdx.x, j = c / 32, cl = c % 32;
+      stat_t a = 0.0, b = 0.0;
+      for (int w = 0; w < 8; ++w)
+        for (int g = 0; g < G; ++g) {
+          const int tid = w * 32 + g * CL + cl;
+          a += (stat_t)s_stat[j * 256 + tid];
+          b += (stat_t)s_stat[(2 + j) * 256 + tid];
+        }
+      s_part[c] = a;
+      s_part[p.Cout + c] = b;
+    }
+    __syncthreads();
+    if (publish_partials(s_part, p.Cout, bn->partials, bn->counter)) {
+      if constexpr (kStemU8<T>) bn_fwd_finalize(*bn, p.Cout);
+      else stem_bn_fwd_finalize(bn, p.Cout);
+      __syncthreads();
+      if (threadIdx.x == 0) *bn->counter = 0;
+    }
   }
 }
 
@@ -332,19 +417,50 @@ __global__ void __launch_bounds__(256, EVAL ? 2 : 3) stem_fwd_u8_kernel(
   stem_fwd_body<EVAL, uint8_t>(p);
 }
 
+// training forward: the stem forward with the BatchNorm statistics of y.  Min-blocks 3 keeps both
+// input types at the three CTAs per SM of the forward without statistics.
+struct StemTrainDev {
+  StemDev s;
+  yamb_bn_fwd bn;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(256, 3) stem_fwd_train_kernel(const __grid_constant__ StemTrainDev p) {
+  stem_fwd_body<false, T, true>(p.s, &p.bn);
+}
+
 // wgrad: thread = (8 output channels co8, 4 positions jq, pixel subset ps): 256 threads =
 // (Cout/8) x 8 x PS.  32 FMAs per 2 + 4 shared-memory loads.  Positions are walked in
 // staging order jj = (ky*3 + kx)*3 + ci and mapped to the parameter's j = ci*9 + ky*3 + kx at the end.
-template <typename T>
-__global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__ StemDev p) {
+// FORM (training wgrad, yamb_stem_conv_train_wgrad): p.dh holds dz; once the tile has landed, each
+// vector of it is replaced in shared memory by dh = bf16(fmaf(ca, dz, fmaf(cb, h, cc))) with h
+// read from global memory, the expression of bn_bwd_apply_kernel (elementwise.cu), 0 outside the
+// image; the coefficients are staged in shared memory after the dh tile.
+struct StemFormDh {
+  const __nv_bfloat16* h;
+  const float* ca;
+  const float* cb;
+  const float* cc;
+};
+
+template <typename T, bool FORM = false>
+__device__ __forceinline__ void stem_wgrad_body(const StemDev& p, const StemFormDh* f = nullptr) {
   extern __shared__ __align__(16) unsigned char stem_smem[];
   __nv_bfloat16* s_in = reinterpret_cast<__nv_bfloat16*>(stem_smem);          // [IH][SW][3]
   __nv_bfloat16* s_dh = s_in + ((kStemIH * kStemSW * 3 + 7) & ~7);            // [TH*TW][Cout]
-  // uint8 x: table and byte tile after s_dh
+  float* s_coef = reinterpret_cast<float*>(s_dh + kStemTH * kStemTW * p.Cout);  // FORM: [3][Cout]
+  if constexpr (FORM) {
+    for (int e = threadIdx.x; e < 3 * p.Cout; e += 256) {
+      const int k = e / p.Cout, c = e - k * p.Cout;
+      s_coef[e] = (k == 0 ? f->ca : k == 1 ? f->cb : f->cc)[c];
+    }
+  }
+  // uint8 x: table and byte tile after s_dh (and the coefficients)
   uint16_t* s_lut = nullptr;
   unsigned char* s_bytes = nullptr;
   if constexpr (kStemU8<T>) {
-    s_lut = reinterpret_cast<uint16_t*>(s_dh + kStemTH * kStemTW * p.Cout);
+    s_lut = reinterpret_cast<uint16_t*>(FORM ? (void*)(s_coef + 3 * 64)
+                                             : (void*)(s_dh + kStemTH * kStemTW * p.Cout));
     s_bytes = reinterpret_cast<unsigned char*>(s_lut + 3 * 256);
     stem_u8_table(p, s_lut);
   }
@@ -388,12 +504,35 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__
     cp_async_commit();
     cp_async_wait<0>();
     __syncthreads();
+    if constexpr (FORM) {
+      uint4* sd = reinterpret_cast<uint4*>(s_dh);
+#pragma unroll 2
+      for (int e = threadIdx.x; e < kStemTH * kStemTW * V; e += 256) {
+        const int pix = e / V, c0 = (e % V) * 8;
+        const int oy = ty * kStemTH + pix / kStemTW, ox = tx * kStemTW + pix % kStemTW;
+        uint4 r = make_uint4(0u, 0u, 0u, 0u);
+        if (oy < p.Ho && ox < p.Wo) {
+          float d[8], hv[8];
+          unpack8(sd[e], d);
+          unpack8(__ldg(reinterpret_cast<const uint4*>(
+                            f->h + (((size_t)n * p.Ho + oy) * p.Wo + ox) * p.Cout + c0)),
+                  hv);
+#pragma unroll
+          for (int k = 0; k < 8; ++k)
+            d[k] = fmaf(s_coef[c0 + k], d[k], fmaf(s_coef[p.Cout + c0 + k], hv[k],
+                                                   s_coef[2 * p.Cout + c0 + k]));
+          r = pack8(d);
+        }
+        sd[e] = r;
+      }
+    }
     if constexpr (kStemU8<T>) {
       if (aligned) {
         stem_u8_convert(p, ty, tx, s_bytes, s_lut, s_in);
         __syncthreads();
       }
     }
+    if constexpr (FORM) __syncthreads();
 #pragma unroll 2
     for (int pix = ps; pix < kStemTH * kStemTW; pix += PS) {
       const uint4 d = reinterpret_cast<const uint4*>(s_dh + (size_t)pix * p.Cout)[co8];
@@ -424,6 +563,24 @@ __global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__
       }
     }
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) stem_wgrad_kernel(const __grid_constant__ StemDev p) {
+  stem_wgrad_body<T>(p);
+}
+
+struct StemWgradTrainDev {
+  StemDev s;
+  StemFormDh f;
+};
+
+// min-blocks 3: the CTAs per SM of the bf16 wgrad, whose grid it takes (98 registers, two CTAs
+// per SM, at the default bound)
+template <typename T>
+__global__ void __launch_bounds__(256, 3) stem_wgrad_train_kernel(
+    const __grid_constant__ StemWgradTrainDev p) {
+  stem_wgrad_body<T, true>(p.s, &p.f);
 }
 
 // Shape checks and the tile plan; touches no device.  Every launcher finishes its own argument
@@ -556,6 +713,106 @@ int stem_conv_u8_eval_fwd_launch(const yamb_stem_conv_u8* a, cudaStream_t st) {
 int stem_conv_u8_wgrad_launch(const yamb_stem_conv_u8* a, cudaStream_t st) {
   if (!a) return set_error(YAMB_EINVAL, "stem conv u8: bad arguments");
   return stem_wgrad(&a->ev.conv, a, st);
+}
+
+// ---- training entry points: the shape, input-type and normalisation checks of the entries above
+template <typename A>
+static int stem_train_fill(const A* a, StemDev& p) {
+  if (a->x_u8 != 0 && a->x_u8 != 1)
+    return set_error(YAMB_EINVAL, "stem conv train: x_u8=%d must be 0 or 1", a->x_u8);
+  yamb_stem_conv c = {};
+  c.N = a->N; c.H = a->H; c.W = a->W; c.Cout = a->Cout; c.x = a->x;
+  yamb_stem_conv_u8 u = {};
+  for (int k = 0; k < 3; ++k) {
+    u.mean[k] = a->mean[k];
+    u.std[k] = a->std[k];
+  }
+  const int rc = stem_fill(&c, a->x_u8 ? &u : nullptr, p);
+  if (rc) return rc;
+  if (256 % a->Cout) return set_error(YAMB_EINVAL, "stem conv train: Cout must be 8, 16, 32 or 64");
+  p.scale = p.shift = nullptr;
+  p.act = 0;
+  return 0;
+}
+
+int stem_conv_train_fwd_launch(const yamb_stem_conv_train* a, cudaStream_t st) {
+  if (!a) return set_error(YAMB_EINVAL, "stem conv train fwd: bad arguments");
+  StemTrainDev d;
+  int rc = stem_train_fill(a, d.s);
+  if (rc) return rc;
+  if (!a->w || !a->y || (reinterpret_cast<uintptr_t>(a->y) & 15))
+    return set_error(YAMB_EINVAL, "stem conv train fwd: w / y (16-byte aligned) required");
+  const yamb_bn_fwd* bn = a->bn;
+  if (!bn || !bn->partials || !bn->counter || !bn->scale || !bn->shift ||
+      (bn->running_mean == nullptr) != (bn->running_var == nullptr))
+    return set_error(YAMB_EINVAL, "stem conv train fwd: bn needs partials, counter, scale, shift");
+  if (bn->count != (long long)d.s.N * d.s.Ho * d.s.Wo)
+    return set_error(YAMB_EINVAL, "stem conv train fwd: bn.count=%lld, N*Ho*Wo=%lld",
+                     (long long)bn->count, (long long)d.s.N * d.s.Ho * d.s.Wo);
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  d.s.w = a->w;
+  d.s.y = (__nv_bfloat16*)a->y;
+  d.bn = *bn;
+  const bool u8 = a->x_u8 != 0;
+  const size_t smem = 27 * 64 * 4 + (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
+                      (size_t)8 * 64 * (a->Cout / 8) * 16 + (u8 ? kStemU8Smem : 0) + 4 * 256 * 4;
+  const void* kern = u8 ? (const void*)stem_fwd_train_kernel<uint8_t>
+                        : (const void*)stem_fwd_train_kernel<__nv_bfloat16>;
+  int per_sm = 0;
+  if ((rc = smem_optin("stem conv train fwd", kern, smem, &per_sm))) return rc;
+  const int res_f = max_ctas() * (per_sm > 0 ? per_sm : 1);   // one resident wave
+  const int grid = d.s.num_tiles < res_f ? d.s.num_tiles : res_f;
+  if (u8) stem_fwd_train_kernel<uint8_t><<<grid, 256, smem, st>>>(d);
+  else stem_fwd_train_kernel<__nv_bfloat16><<<grid, 256, smem, st>>>(d);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv train fwd: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int stem_conv_train_wgrad_launch(const yamb_stem_conv_train_grad* a, cudaStream_t st) {
+  if (!a) return set_error(YAMB_EINVAL, "stem conv train wgrad: bad arguments");
+  StemWgradTrainDev d;
+  int rc = stem_train_fill(a, d.s);
+  if (rc) return rc;
+  if (!a->dz || !a->h || !a->dw || !a->ca || !a->cb || !a->cc ||
+      ((reinterpret_cast<uintptr_t>(a->dz) | reinterpret_cast<uintptr_t>(a->h)) & 15))
+    return set_error(YAMB_EINVAL,
+                     "stem conv train wgrad: dz / h (16-byte aligned), ca / cb / cc, dw required");
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  d.s.dh = (const __nv_bfloat16*)a->dz;
+  d.s.dw = a->dw;
+  d.f.h = (const __nv_bfloat16*)a->h;
+  d.f.ca = a->ca;
+  d.f.cb = a->cb;
+  d.f.cc = a->cc;
+  const bool u8 = a->x_u8 != 0;
+  const size_t smem = (size_t)((kStemIH * kStemSW * 3 + 7) & ~7) * 2 +
+                      (size_t)kStemTH * kStemTW * a->Cout * 2;
+  // the grid, and so the partial slabs and the order of their sum, of the bf16 wgrad of
+  // yamb_stem_conv_wgrad: dw is bitwise yamb_bn_bwd_apply_bwd followed by that entry
+  int per_sm = 0;
+  if ((rc = smem_optin("stem conv wgrad", (const void*)stem_wgrad_kernel<__nv_bfloat16>, smem,
+                       &per_sm)))
+    return rc;
+  const size_t smem_t = smem + 3 * 64 * sizeof(float) + (u8 ? kStemU8Smem : 0);
+  if ((rc = smem_optin("stem conv train wgrad",
+                       u8 ? (const void*)stem_wgrad_train_kernel<uint8_t>
+                          : (const void*)stem_wgrad_train_kernel<__nv_bfloat16>,
+                       smem_t)))
+    return rc;
+  const int res_w = max_ctas() * (per_sm > 0 ? per_sm : 1);
+  const int grid = d.s.num_tiles < res_w ? d.s.num_tiles : res_w;
+  const int slots = grid * (256 / d.s.Cout);
+  rc = det_alloc((size_t)slots * d.s.Cout * 27 * sizeof(float), st, &d.s.part);
+  if (rc) return rc;
+  if (u8) stem_wgrad_train_kernel<uint8_t><<<grid, 256, smem_t, st>>>(d);
+  else stem_wgrad_train_kernel<__nv_bfloat16><<<grid, 256, smem_t, st>>>(d);
+  if (cudaPeekAtLastError() != cudaSuccess) det_free(d.s.part, st);
+  else if ((rc = det_reduce_launch(d.s.part, slots, (long long)d.s.Cout * 27, d.s.dw, st)) != 0)
+    return rc;
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "stem conv train wgrad: %s", cudaGetErrorString(e));
+  return 0;
 }
 
 }  // namespace yamb

@@ -760,8 +760,10 @@ class BlockPlan:
         side["pending"] = True
 
     # -- forward ---------------------------------------------------------------------------------
-    def forward(self, x):
-        """x: channels_last bf16 [N,Cin,H,W]; returns channels_last bf16 [N,Cout,Ho,Wo]."""
+    def forward(self, x, pre=None):
+        """x: channels_last bf16 [N,Cin,H,W]; returns channels_last bf16 [N,Cout,Ho,Wo].
+        pre = (scale, shift, act) of an input BatchNorm + activation (a block without expansion
+        whose x is the raw output of the layer before): the depthwise applies it to x on load."""
         lib = nat.lib()
         self.generation += 1
         self._refresh_weights()
@@ -793,7 +795,7 @@ class BlockPlan:
             s = slice(c0, c0 + cb)
             _dw_fwd(conv, (self.N, self.H, self.W), self.h1[:, s] if self.expand else xm,
                     self.h2[:, s], "dw_fwd",
-                    pre=(self.bn1.scale[s], self.bn1.shift[s], self.act) if self.expand else None,
+                    pre=(self.bn1.scale[s], self.bn1.shift[s], self.act) if self.expand else pre,
                     stats=self.bn2.fwd_struct(self.M_out, c0, cb) if self.bn2.batch_stats
                     else None)
         # 2b. Squeeze-and-Excitation gate (reference mobilenet_base.py:110-113): spatial mean of
@@ -872,10 +874,12 @@ class BlockPlan:
             launch(lib.yamb_se_bwd_apply_bwd, a, "se_bwd_apply", 6 * self.M_out * cb)
 
     # -- backward --------------------------------------------------------------------------------
-    def backward(self, x, dy, grads):
+    def backward(self, x, dy, grads, pre=None, pre_stats=None):
         """grads: dict with fp32 accumulation targets:
            'exp' [Chid,Cin], 'proj' [Cout,Chid], 'dw' list[[C,1,k,k]], 'bn1'/'bn2'/'bn3' lists of
-           (dgamma, dbeta) per reference BN module.  Returns dx (channels_last bf16)."""
+           (dgamma, dbeta) per reference BN module.  Returns dx (channels_last bf16).  With the
+           `pre` of the forward, dx is the gradient dz = da * act'(z) of the input BatchNorm's
+           output, and `pre_stats` (a yamb_bn_bwd) takes that BatchNorm's backward statistics."""
         lib = nat.lib()
         bf = torch.bfloat16
         if self.dz2 is None:
@@ -946,7 +950,8 @@ class BlockPlan:
                         stats=self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb))
             else:
                 _dw_bwd(conv, (self.N, self.H, self.W), self.dz2[:, s], self.h2[:, s], coef, dw,
-                        xm, dx, "dw_bwd", residual=dym_skip if self.residual else None)
+                        xm, dx, "dw_bwd", pre=pre, residual=dym_skip if self.residual else None,
+                        stats=pre_stats)
         if not self.expand:
             return dx
         # 5+6. dh1 = ca1*dz1 + cb1*h1 + cc1 formed once, dx = dh1 * W1 (+ dy) and
@@ -1092,7 +1097,15 @@ def run_backward(block, plan, x, dy):
     `block.parameters()` (`GradTargets.result`)."""
     dy = to_nhwc_bf16(dy)
     gt = GradTargets(block.parameters())
+    dx = plan.backward(x, dy, block_grads(gt, plan))
+    if not DEFER_JOIN or gt.host_reads:
+        join_side(plan.dev)
+    return dx, gt.result()
 
+
+def block_grads(gt, plan):
+    """The `grads` argument of `plan.backward`: the accumulation targets in `gt` (a GradTargets
+    over the block's parameters, possibly among others) of every parameter of the plan's block."""
     def bn_targets(bn):
         return [] if bn is None else [(gt.of(m.weight), gt.of(m.bias)) for m in bn.mods]
 
@@ -1111,10 +1124,7 @@ def run_backward(block, plan, x, dy):
     if plan.nl is not None:
         g["bn4"] = bn_targets(plan.bn4)
         g["nl_dw"] = gt.of(plan.nl.depthwise_conv.weight)
-    dx = plan.backward(x, dy, g)
-    if not DEFER_JOIN or gt.host_reads:
-        join_side(plan.dev)
-    return dx, gt.result()
+    return g
 
 
 # ---- channel padding ---------------------------------------------------------------------------
@@ -1414,6 +1424,18 @@ EVAL_TAIL_CALLS = 0      # stem / head calls that went through the one-launch ke
 # gradient never reach HBM.  Otherwise the unfused sequence runs.
 TRAIN_TAIL_FUSED = False
 TRAIN_TAIL_CALLS = 0     # head calls that went through yamb_head_pool_train_fwd (tests)
+
+# ---- training mode: stem BatchNorm + activation inside the first block (tail_ops.stem_block_train) --
+# Off by default: the stem's statistics are summed in another order and, with Swish, dz is rounded
+# after the act' product instead of before, so turning it on changes the bits of a training step.
+# When True (trainer.TrainStep(fused_stem=True) turns it on for its own forwards and backwards) the
+# stem ConvBNReLU and a first block without expansion or skip connection (the stem activation's
+# only consumer, tail_ops.stem_block_fused_covered) run as one autograd function: the stem kernel
+# takes the BatchNorm statistics of h, the block's depthwise applies BatchNorm + activation on load
+# and writes dz with the BatchNorm-backward statistics, and the stem weight gradient forms dh on
+# load; the activation, its gradient and dh never reach HBM.  Otherwise the unfused sequence runs.
+TRAIN_STEM_FUSED = False
+TRAIN_STEM_CALLS = 0     # stem + first block calls that went through stem_block_train (tests)
 
 
 def _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p):

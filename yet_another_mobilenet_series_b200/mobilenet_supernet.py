@@ -57,7 +57,9 @@ def _full_extent(pool, x):
 # step includes the input's conversion to bf16 channels_last), each block, the head, the pool and
 # model.classifier (its step includes the cast of the logits to fp32).  The time between two
 # consecutive events is the device time of the step the second one ends.  A head run together with
-# the pool (engine.EVAL_TAIL_FUSED, engine.TRAIN_TAIL_FUSED) is one step, recorded for the head.
+# the pool (engine.EVAL_TAIL_FUSED, engine.TRAIN_TAIL_FUSED) is one step, recorded for the head; a
+# stem run together with the first block (engine.TRAIN_STEM_FUSED) is one step, recorded for the
+# stem.
 STEPS = None
 
 
@@ -90,11 +92,18 @@ def run_features(model, x):
                 if skip:
                     skip = False
                     continue
+                nxt = layers[i + 1] if i + 1 < len(layers) else None
+                if (i == 0 and engine.TRAIN_STEM_FUSED and nxt is not None
+                        and tail_ops.stem_block_fused_covered(layer, nxt, x)):
+                    # training: stem ConvBNReLU + its only consumer, the first block, as one
+                    # autograd function (the stem's BatchNorm + activation inside the depthwise)
+                    x, skip = tail_ops.stem_block_train(layer, nxt, x, norm), True
+                    _step_done(stream, layer)
+                    continue
                 if i == 0 and norm is not None:
                     x = tail_ops.stem_u8(layer, x, norm)
                     _step_done(stream, layer)
                     continue
-                nxt = layers[i + 1] if i + 1 < len(layers) else None
                 if ((engine.EVAL_TAIL_FUSED or engine.TRAIN_TAIL_FUSED)
                         and isinstance(layer, ConvBNReLU)
                         and isinstance(nxt, nn.AvgPool2d) and _full_extent(nxt, x)):

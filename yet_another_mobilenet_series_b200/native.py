@@ -253,6 +253,26 @@ class StemConvU8(C.Structure):
     ]
 
 
+class StemConvTrain(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("Cout", C.c_int32),
+        ("x", C.c_void_p), ("x_u8", C.c_int32),
+        ("mean", C.c_float * 3), ("std", C.c_float * 3),
+        ("w", C.c_void_p), ("y", C.c_void_p), ("bn", C.POINTER(BnFwd)),
+    ]
+
+
+class StemConvTrainGrad(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("Cout", C.c_int32),
+        ("x", C.c_void_p), ("x_u8", C.c_int32),
+        ("mean", C.c_float * 3), ("std", C.c_float * 3),
+        ("dz", C.c_void_p), ("h", C.c_void_p),
+        ("ca", C.c_void_p), ("cb", C.c_void_p), ("cc", C.c_void_p),
+        ("dw", C.c_void_p),
+    ]
+
+
 class HeadPoolEval(C.Structure):
     _fields_ = [
         ("N", C.c_int32), ("HW", C.c_int32), ("Cin", C.c_int32), ("Cout", C.c_int32),
@@ -372,11 +392,12 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
             14: NlRowmat, 15: SeFc, 16: SeFcBwd, 17: SoftmaxCe, 18: SoftmaxCeGrad,
             19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd, 24: Sgd,
             25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
-            29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad}
+            29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad,
+            33: StemConvTrain, 34: StemConvTrainGrad}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -430,6 +451,8 @@ def lib():
         l.yamb_head_pool_eval_fwd.argtypes = [C.POINTER(HeadPoolEval), C.c_void_p]
         l.yamb_head_pool_train_fwd.argtypes = [C.POINTER(HeadPoolTrain), C.c_void_p]
         l.yamb_head_pool_train_bwd.argtypes = [C.POINTER(HeadPoolTrainGrad), C.c_void_p]
+        l.yamb_stem_conv_train_fwd.argtypes = [C.POINTER(StemConvTrain), C.c_void_p]
+        l.yamb_stem_conv_train_wgrad.argtypes = [C.POINTER(StemConvTrainGrad), C.c_void_p]
         l.yamb_se_fc_fwd.argtypes = [C.POINTER(SeFc), C.c_void_p]
         l.yamb_se_fc_bwd.argtypes = [C.POINTER(SeFcBwd), C.c_void_p]
         l.yamb_nl_gram_fwd.argtypes = [C.POINTER(NlGram), C.c_void_p]

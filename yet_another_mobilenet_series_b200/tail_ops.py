@@ -499,3 +499,113 @@ def stem_u8(mod, x, norm):
     if isinstance(mod, torch.nn.Sequential) and len(mod) == 3 and stem_supported(mod, x):
         return stem_conv_bn_act(mod, x, norm)
     return mod(normalize_u8(x, norm))
+
+
+# ---- training mode: the stem and its only consumer ----------------------------------------------
+def stem_block_fused_covered(stem, block, x):
+    """Whether stem_block_train runs the stem ConvBNReLU `stem` on image x together with the next
+    layer `block`: the direct stem kernels cover the stem, its BatchNorm normalises with batch
+    statistics, `block` is an inverted-residual block (either class, with or without SE or
+    non-local) without expansion, with one branch and no skip connection, whose input width is the
+    stem's output width, and that runs on the training path (not engine.eval_forward).  Then the
+    block's depthwise is the only reader of the stem activation.  Host-only: reads shapes and
+    modules, no device."""
+    from .mobilenet_base import _FusedBlockBase
+    if not (isinstance(stem, torch.nn.Sequential) and len(stem) == 3 and stem_supported(stem, x)):
+        return False
+    bn = stem[1]
+    if not (isinstance(bn, torch.nn.BatchNorm2d) and (bn.training or not bn.track_running_stats)):
+        return False
+    cout = stem[0].out_channels
+    if not (isinstance(block, _FusedBlockBase) and not block.expand and len(block.channels) == 1
+            and not block.use_res_connect and block.input_dim == cout
+            and block.channels[0] == cout):
+        return False
+    N, _, H, W = x.shape
+    h = torch.empty((N, cout, (H - 1) // 2 + 1, (W - 1) // 2 + 1), device="meta")
+    return not engine.eval_supported(block, h)
+
+
+def _stem_train_args(st, x, conv, norm):
+    st.N, st.H, st.W, st.Cout = x.shape[0], x.shape[2], x.shape[3], conv.out_channels
+    st.x = x.data_ptr()
+    if norm is not None:
+        st.x_u8 = 1
+        st.mean[:] = norm[0]
+        st.std[:] = norm[1]
+
+
+class _StemBlockFn(torch.autograd.Function):
+    """Stem ConvBNReLU + the first block (stem_block_fused_covered) as one autograd function.
+    Forward: yamb_stem_conv_train_fwd writes the raw stem output h and finalises the stem
+    BatchNorm's batch statistics; the block's BlockPlan runs with the stem's BatchNorm +
+    activation applied by its depthwise on load.  Backward: the BlockPlan backward, whose
+    depthwise writes dz_stem = da * act'(z) and the stem BatchNorm's backward statistics
+    (dgamma, dbeta, ca / cb / cc), then yamb_stem_conv_train_wgrad forms dh on load.  Gradients
+    of the stem weight, the stem BatchNorm and the block go through engine.GradTargets."""
+
+    @staticmethod
+    def forward(ctx, x, stem, block, norm, *params):
+        lib = nat.lib()
+        conv, bn = stem[0], stem[1]
+        act = engine.act_code_of(stem[2])
+        b = engine._bn_act_state(bn, x.device).bn
+        N, _, H, W = x.shape
+        Cout = conv.out_channels
+        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+        h = torch.empty((N, Cout, Ho, Wo), device=x.device, dtype=torch.bfloat16,
+                        memory_format=torch.channels_last)
+        a = nat.StemConvTrain()
+        _stem_train_args(a, x, conv, norm)
+        a.w, a.y = conv.weight.data_ptr(), h.data_ptr()
+        stats = b.fwd_struct(N * Ho * Wo)
+        a.bn = C.pointer(stats)
+        engine.launch(lib.yamb_stem_conv_train_fwd, a, "stem_conv_train_fwd",
+                      _stem_bytes(x, Ho, Wo, Cout), 2 * N * Ho * Wo * Cout * 27)
+        # this call's coefficients, as _BnActFn keeps them (another forward through the stem
+        # before this backward, e.g. the next micro-batch, rewrites the live ones)
+        coef = torch.stack((b.scale, b.shift, b.mean, b.invstd))
+        plan = engine._plan_for(block, h)
+        y = plan.forward(h, pre=(coef[0], coef[1], act))
+        ctx.stem, ctx.block, ctx.norm, ctx.act = stem, block, norm, act
+        ctx.plan, ctx.generation = plan, plan.generation
+        ctx.save_for_backward(x, h, coef)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        plan = ctx.plan
+        if plan.generation != ctx.generation:
+            raise RuntimeError("yamb: the first block ran another forward before the backward of "
+                               "the previous one (see engine._BlockFn)")
+        x, h, coef = ctx.saved_tensors
+        conv, bn = ctx.stem[0], ctx.stem[1]
+        b = engine._bn_act_state(bn, h.device).bn
+        N, Cout, Ho, Wo = h.shape
+        dy = engine.to_nhwc_bf16(dy)
+        gt = engine.GradTargets([conv.weight, bn.weight, bn.bias] + list(ctx.block.parameters()))
+        stats = b.bwd_struct(N * Ho * Wo, [(gt.of(bn.weight), gt.of(bn.bias))])
+        stats.mean, stats.invstd = coef[2].data_ptr(), coef[3].data_ptr()
+        dz = plan.backward(h, dy, engine.block_grads(gt, plan), pre=(coef[0], coef[1], ctx.act),
+                           pre_stats=stats)
+        a = nat.StemConvTrainGrad()
+        _stem_train_args(a, x, conv, ctx.norm)
+        a.dz, a.h = dz.data_ptr(), h.data_ptr()
+        a.ca, a.cb, a.cc = b.ca.data_ptr(), b.cb.data_ptr(), b.cc.data_ptr()
+        a.dw = gt.of(conv.weight).data_ptr()
+        engine.launch(nat.lib().yamb_stem_conv_train_wgrad, a, "stem_conv_train_wgrad",
+                      _stem_bytes(x, Ho, Wo, Cout) + 2 * N * Ho * Wo * Cout,
+                      2 * N * Ho * Wo * Cout * 27)
+        if not engine.DEFER_JOIN or gt.host_reads:
+            engine.join_side(plan.dev)
+        return (None, None, None, None) + gt.result()
+
+
+def stem_block_train(stem, block, x, norm=None):
+    """y = block(stem(x)) in training through _StemBlockFn, for a pair stem_block_fused_covered
+    accepts (the caller checks).  x: bf16 channels_last, or with `norm` a uint8 image the
+    kernels normalise."""
+    params = [stem[0].weight, stem[1].weight, stem[1].bias] + list(block.parameters())
+    y = _StemBlockFn.apply(x, stem, block, norm, *params)
+    engine.TRAIN_STEM_CALLS += 1
+    return y

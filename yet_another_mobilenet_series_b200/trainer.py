@@ -85,7 +85,7 @@ class TrainStep:
                  alpha=0.9, momentum=0.9, eps=1e-3, weight_decay=1e-5, label_smoothing=0.1,
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
-                 input_norm=None, micro_batch=None, fused_tail=False):
+                 input_norm=None, micro_batch=None, fused_tail=False, fused_stem=False):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
@@ -105,7 +105,17 @@ class TrainStep:
         step's forwards and backwards as one kernel each way (engine.TRAIN_TAIL_FUSED): the
         activation and its broadcast gradient stay out of HBM.  Off by default: the pool sums in
         its own fixed order, not torch's, so a step with it differs from the default in the last
-        bits.  A plain `model(x)` outside the step is not affected."""
+        bits.  A plain `model(x)` outside the step is not affected.
+
+        `fused_stem=True` runs the stem ConvBNReLU of this step's forwards and backwards together
+        with the first block when that block is the stem activation's only consumer (no
+        expansion, no skip connection; engine.TRAIN_STEM_FUSED): the stem convolution takes the
+        BatchNorm statistics, the block's depthwise applies the BatchNorm + activation on load
+        and returns their backward, and the stem weight gradient forms dh on load, so the stem's
+        activation, its gradient and dh stay out of HBM.  Off by default: the statistics are
+        summed in another order (and with Swish dz is rounded after the act' product), so a step
+        with it differs from the default in the last bits, the same bits on every run.  It
+        combines with `fused_tail`; a plain `model(x)` outside the step is not affected."""
         self.world = udist.get_world_size_fallback()
         self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
             per_gpu_batch, micro_batch, self.world, base_lr, base_total_batch, ema_decay,
@@ -118,6 +128,7 @@ class TrainStep:
         self.dev = dev
         self.batch = per_gpu_batch
         self.fused_tail = bool(fused_tail)
+        self.fused_stem = bool(fused_stem)
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
                                eps=eps, eps_inside_sqrt=True, weight_decay=0)
@@ -186,10 +197,12 @@ class TrainStep:
         pass of n_i rows by n_i / n, a device scalar, so its gradient is that of the mean over the
         n rows."""
         engine.TRAIN_TAIL_FUSED = self.fused_tail
+        engine.TRAIN_STEM_FUSED = self.fused_stem
         try:
             self._passes(self.x if x is None else x, self.t if t is None else t)
         finally:
             engine.TRAIN_TAIL_FUSED = False
+            engine.TRAIN_STEM_FUSED = False
 
     def _passes(self, x, t):
         n, b = x.shape[0], self.micro_batch
