@@ -638,6 +638,65 @@ int yamb_block_eval_cluster_fwd(const yamb_block_eval* args, int32_t cluster, ya
 int yamb_block_eval_cluster_pool_fwd(const yamb_block_eval* args, int32_t cluster,
                                      yamb_stream_t stream);
 
+/* ---- eval-mode multi-branch block (several depthwise kernels: AtomNAS), ONE launch ---------------
+ * In eval mode a block of several branches (reference models/mobilenet_base.py:330-342 and
+ * :446-451) is one single-branch block over the concatenated hidden dimension whose depthwise kernel
+ * varies by channel: the project sums over the hidden channels, so their order is free.
+ * yamb_block_eval_mb_pack lays the branches out as groups of decreasing k (each branch padded to a
+ * multiple of 8 channels: zero W1 rows and W3 columns, BatchNorm gamma = beta = mean = 0, var = 1,
+ * so a padded channel's a1 and a2 are exactly 0), with every tap table zero-embedded in the centre
+ * of K_MAX x K_MAX.  yamb_block_eval_mb_fwd / _pool_fwd then run the yamb_block_eval_fwd / _pool_fwd
+ * tile walk over the packed tensors, every 64-channel slice with the stencil of the group of its
+ * first channel (the largest k among its channels; the smaller-k channels of a boundary slice add
+ * products with zero taps, which leaves the fp32 sums unchanged).
+ *
+ * Pack: one branch's fp32 tensors as the modules hold them.  `w_project` and `se_reduce` point at
+ * the branch's first column of row-major matrices with row stride `ld`. */
+typedef struct yamb_mb_branch {
+  int32_t k;                  /* 3, 5 or 7 */
+  int32_t C;                  /* hidden channels of the branch */
+  int32_t ld;                 /* row stride of w_project / se_reduce (>= C) */
+  const float* w_expand;      /* [C][Cin] */
+  yamb_bn_eval bn1, bn2;      /* over the branch's C channels (eps: that of the block call) */
+  const float* w_dw;          /* [C][k][k] */
+  const float* w_project;     /* [Cout][ld], the branch's columns */
+  const float* se_reduce;     /* [R][ld], the branch's columns; NULL without Squeeze-and-Excitation */
+  const float* se_expand;     /* [C][R] */
+  const float* se_expand_bias;/* [C] */
+} yamb_mb_branch;
+
+typedef struct yamb_block_eval_mb_pack_args {
+  int32_t Cin, Cout, R;       /* R: SE reduced width (0 without SE) */
+  int32_t nbranch;            /* 1..3 */
+  yamb_mb_branch branch[3];
+  int32_t Chid, kmax;         /* packed hidden width (multiple of 8); largest k of the branches */
+  const int32_t* map;         /* device [Chid]: (branch << 16) | channel, or -1 for a padded channel */
+  void* w_expand;             /* out bf16 [Chid][Cin] */
+  void* w_project;            /* out bf16 [Cout][Chid] */
+  float* w_dw;                /* out [Chid][kmax][kmax] */
+  float* bn1; float* bn2;     /* out [4][Chid]: gamma, beta, running mean, running var */
+  float* se_reduce;           /* out [R][Chid] (with SE) */
+  float* se_expand;           /* out [Chid][R] */
+  float* se_expand_bias;      /* out [Chid] */
+} yamb_block_eval_mb_pack_args;
+
+/* base: the yamb_block_eval of the packed block (kernel = kmax in {5, 7}, with expansion, Chid the
+ * packed width, w_expand / w_dw / w_project / bn1 / bn2 the packed tensors, gate / pooled over Chid).
+ * Hidden channels [group_c0[i], group_c0[i+1]) (the last group up to Chid) have kernel group_k[i];
+ * group_k strictly decreasing from group_k[0] = kmax, group_c0 increasing multiples of 8 from 0.
+ * No cluster split.  YAMB_EINVAL for what yamb_block_eval_fwd does not cover or bad groups
+ * (nothing enqueued), YAMB_ENODEV without a device. */
+typedef struct yamb_block_eval_mb {
+  yamb_block_eval base;
+  int32_t ngroups;            /* 1..3 */
+  int32_t group_k[3];
+  int32_t group_c0[3];
+} yamb_block_eval_mb;
+
+int yamb_block_eval_mb_pack(const yamb_block_eval_mb_pack_args* args, yamb_stream_t stream);
+int yamb_block_eval_mb_fwd(const yamb_block_eval_mb* args, yamb_stream_t stream);
+int yamb_block_eval_mb_pool_fwd(const yamb_block_eval_mb* args, yamb_stream_t stream);
+
 /* ---- fused flat-arena RMSprop (+L2 decay, +DDP mean, +EMA, +bf16 repack) -------------------------
  * Replaces RMSprop.step (reference utils/rmsprop.py:67-129), the gradient of cal_l2_loss
  * (utils/optim.py:177-200; l2 * p added where bit 0 of wd_mask is set; bit 1 marks a parameter
@@ -692,7 +751,7 @@ int yamb_max_ctas(void);
  * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
  * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8, 29 expand_bwd_args,
  * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad, 33 stem_conv_train,
- * 34 stem_conv_train_grad) so bindings can self-check */
+ * 34 stem_conv_train_grad, 35 block_eval_mb_pack_args, 36 block_eval_mb) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

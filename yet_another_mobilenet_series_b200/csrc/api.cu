@@ -146,6 +146,8 @@ int yamb_struct_size(int which) {
     case 32: return (int)sizeof(yamb_head_pool_train_grad);
     case 33: return (int)sizeof(yamb_stem_conv_train);
     case 34: return (int)sizeof(yamb_stem_conv_train_grad);
+    case 35: return (int)sizeof(yamb_block_eval_mb_pack_args);
+    case 36: return (int)sizeof(yamb_block_eval_mb);
     default: return -1;
   }
 }
@@ -201,6 +203,15 @@ int yamb_block_eval_cluster_fwd(const yamb_block_eval* a, int32_t cluster, yamb_
 }
 int yamb_block_eval_cluster_pool_fwd(const yamb_block_eval* a, int32_t cluster, yamb_stream_t s) {
   return yamb::block_eval_cluster_pool_launch(a, cluster, YAMB_ST(s));
+}
+int yamb_block_eval_mb_pack(const yamb_block_eval_mb_pack_args* a, yamb_stream_t s) {
+  return yamb::block_eval_mb_pack_launch(a, YAMB_ST(s));
+}
+int yamb_block_eval_mb_fwd(const yamb_block_eval_mb* a, yamb_stream_t s) {
+  return yamb::block_eval_mb_launch(a, false, YAMB_ST(s));
+}
+int yamb_block_eval_mb_pool_fwd(const yamb_block_eval_mb* a, yamb_stream_t s) {
+  return yamb::block_eval_mb_launch(a, true, YAMB_ST(s));
 }
 int yamb_instance_norm_fwd(const yamb_in_fwd* a, yamb_stream_t s) { return yamb::in_fwd_launch(a, YAMB_ST(s)); }
 int yamb_instance_norm_bwd(const yamb_in_bwd* a, yamb_stream_t s) { return yamb::in_bwd_launch(a, YAMB_ST(s)); }

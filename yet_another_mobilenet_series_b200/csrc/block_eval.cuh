@@ -62,6 +62,7 @@
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <type_traits>
 
 #include "host_util.h"
 #include "prims.cuh"
@@ -93,6 +94,8 @@ struct BlockEvalDev {
   int cs;            // CLUSTER: CTAs per cluster (2, 4 or 8)
   int off_red;       // CLUSTER, not kPool: fp32 partials [NPO][red_pitch] of this CTA's slices
   int red_pitch;     // Npad + 8 (a quarter warp's rows on distinct banks) where that fits, else Npad
+  int ngroups;       // G::MB: hidden channels [gc0[i], gc0[i+1]) have depthwise kernel gk[i]
+  int gk[3], gc0[3];
 };
 
 // What one launch computes:
@@ -126,6 +129,9 @@ struct EvGeom {
   static constexpr int PM = NPO > 64 ? 2 : 1;           // 64-row halves of the project MMAs
   static_assert(NPO <= 128 && NPI <= 256 && TOW % RUN == 0 && NRUN * NCG <= 224,
                 "tile geometry (warp 7 must stay free of stencil work)");
+  // multi-branch blocks (block_eval_mb.cu): K is the largest kernel of the block and every 64-channel
+  // slice runs the stencil of its own k <= K over the centred k x k window of the tile
+  static constexpr bool MB = false;
 };
 
 template <class G, bool EXPAND, bool LEAN, int MODE, bool CLUSTER>
@@ -370,37 +376,88 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         for (int j = 0; j < RUN; ++j)
 #pragma unroll
           for (int v = 0; v < NV; ++v) o2[j][v] = make_float2(0.f, 0.f);
+        if constexpr (G::MB) {
+          // G::MB: KS x KS stencil over the centred window of the K x K tile and tap table
+          // (OFF = (K - KS) / 2); the single-branch kernels run the loop below
+          auto stencil = [&](auto ks) {
+            constexpr int KS = decltype(ks)::value, OFF = (K - KS) / 2;
 #pragma unroll
-        for (int ky = 0; ky < K; ++ky) {
-          float2 w2[K][NV];
+            for (int ky = 0; ky < KS; ++ky) {
+              float2 w2[KS][NV];
 #pragma unroll
-          for (int kx = 0; kx < K; ++kx) {
-            const float* wp = tb + 256 + (ky * K + kx) * 64 + cg * CPT;
-            if (CPT == 4) {
-              const float4 wv = *reinterpret_cast<const float4*>(wp);
-              w2[kx][0] = make_float2(wv.x, wv.y);
-              w2[kx][NV - 1] = make_float2(wv.z, wv.w);
-            } else {
-              w2[kx][0] = *reinterpret_cast<const float2*>(wp);
+              for (int kx = 0; kx < KS; ++kx) {
+                const float* wp = tb + 256 + ((ky + OFF) * K + kx + OFF) * 64 + cg * CPT;
+                if (CPT == 4) {
+                  const float4 wv = *reinterpret_cast<const float4*>(wp);
+                  w2[kx][0] = make_float2(wv.x, wv.y);
+                  w2[kx][NV - 1] = make_float2(wv.z, wv.w);
+                } else {
+                  w2[kx][0] = *reinterpret_cast<const float2*>(wp);
+                }
+              }
+#pragma unroll
+              for (int ixx = 0; ixx < (RUN - 1) * S + KS; ++ixx) {
+                float2 av[NV];
+                const uint8_t* ap_ = s_hb + ((ky + OFF) * IW + ixx + OFF) * kH1Pitch;
+                if (CPT == 4) {
+                  const uint2 a = *reinterpret_cast<const uint2*>(ap_);
+                  av[0] = make_float2(bf16lo(a.x), bf16hi(a.x));
+                  av[NV - 1] = make_float2(bf16lo(a.y), bf16hi(a.y));
+                } else {
+                  const uint32_t a = *reinterpret_cast<const uint32_t*>(ap_);
+                  av[0] = make_float2(bf16lo(a), bf16hi(a));
+                }
+#pragma unroll
+                for (int j = 0; j < RUN; ++j) {
+                  const int kx = ixx - j * S;   // compile-time after unrolling
+                  if (kx >= 0 && kx < KS) {
+#pragma unroll
+                    for (int v = 0; v < NV; ++v) o2[j][v] = ffma2(w2[kx][v], av[v], o2[j][v]);
+                  }
+                }
+              }
             }
-          }
+          };
+          // the slice's kernel: that of the group of its first channel (groups by decreasing k)
+          int kc = p.gk[0];
+          for (int i = 1; i < p.ngroups; ++i)
+            if (c * 64 >= p.gc0[i]) kc = p.gk[i];
+          if (kc == 3) stencil(std::integral_constant<int, 3>{});
+          else if (K == 7 && kc == 5) stencil(std::integral_constant<int, K == 7 ? 5 : K>{});
+          else stencil(std::integral_constant<int, K>{});
+        } else {
 #pragma unroll
-          for (int ixx = 0; ixx < (RUN - 1) * S + K; ++ixx) {
-            float2 av[NV];
-            if (CPT == 4) {
-              const uint2 a = *reinterpret_cast<const uint2*>(s_hb + (ky * IW + ixx) * kH1Pitch);
-              av[0] = make_float2(bf16lo(a.x), bf16hi(a.x));
-              av[NV - 1] = make_float2(bf16lo(a.y), bf16hi(a.y));
-            } else {
-              const uint32_t a = *reinterpret_cast<const uint32_t*>(s_hb + (ky * IW + ixx) * kH1Pitch);
-              av[0] = make_float2(bf16lo(a), bf16hi(a));
+          for (int ky = 0; ky < K; ++ky) {
+            float2 w2[K][NV];
+#pragma unroll
+            for (int kx = 0; kx < K; ++kx) {
+              const float* wp = tb + 256 + (ky * K + kx) * 64 + cg * CPT;
+              if (CPT == 4) {
+                const float4 wv = *reinterpret_cast<const float4*>(wp);
+                w2[kx][0] = make_float2(wv.x, wv.y);
+                w2[kx][NV - 1] = make_float2(wv.z, wv.w);
+              } else {
+                w2[kx][0] = *reinterpret_cast<const float2*>(wp);
+              }
             }
 #pragma unroll
-            for (int j = 0; j < RUN; ++j) {
-              const int kx = ixx - j * S;   // compile-time after unrolling
-              if (kx >= 0 && kx < K) {
+            for (int ixx = 0; ixx < (RUN - 1) * S + K; ++ixx) {
+              float2 av[NV];
+              if (CPT == 4) {
+                const uint2 a = *reinterpret_cast<const uint2*>(s_hb + (ky * IW + ixx) * kH1Pitch);
+                av[0] = make_float2(bf16lo(a.x), bf16hi(a.x));
+                av[NV - 1] = make_float2(bf16lo(a.y), bf16hi(a.y));
+              } else {
+                const uint32_t a = *reinterpret_cast<const uint32_t*>(s_hb + (ky * IW + ixx) * kH1Pitch);
+                av[0] = make_float2(bf16lo(a), bf16hi(a));
+              }
 #pragma unroll
-                for (int v = 0; v < NV; ++v) o2[j][v] = ffma2(w2[kx][v], av[v], o2[j][v]);
+              for (int j = 0; j < RUN; ++j) {
+                const int kx = ixx - j * S;   // compile-time after unrolling
+                if (kx >= 0 && kx < K) {
+#pragma unroll
+                  for (int v = 0; v < NV; ++v) o2[j][v] = ffma2(w2[kx][v], av[v], o2[j][v]);
+                }
               }
             }
           }
@@ -744,13 +801,8 @@ static int launch_eval(BlockEvalDev& p, const yamb_block_eval* a, cudaStream_t s
   return launch_eval_mode<G, EXPAND, kPlain, CLUSTER>(p, a, st);
 }
 
-// CLUSTER: the hidden slices of every tile split over clusters of `cs` CTAs (2, 4 or 8); else cs = 1
-template <bool CLUSTER>
-static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, bool pool, int cs) {
-  if (!a) return set_error(YAMB_EINVAL, "null args");
-  if (CLUSTER ? (cs != 2 && cs != 4 && cs != 8) : cs != 1)
-    return set_error(YAMB_EINVAL, "block_eval: cluster size must be 2, 4 or 8 (got %d)", cs);
-  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+// argument checks and the launch-independent fields of p (the pool pass when `pool`)
+static int block_eval_setup(const yamb_block_eval* a, bool pool, int cs, BlockEvalDev& p) {
   if (a->N <= 0 || a->H <= 0 || a->W <= 0) return set_error(YAMB_EINVAL, "block_eval: bad shape");
   if (a->Cin % 8 || a->Chid % 8 || a->Cout % 8 || a->Cin <= 0 || a->Chid <= 0 || a->Cout <= 0)
     return set_error(YAMB_EINVAL, "block_eval: channel counts must be positive multiples of 8");
@@ -780,7 +832,6 @@ static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, boo
     return set_error(YAMB_EINVAL, "block_eval: gate must be 8-byte aligned");
   if ((long long)a->N * a->H * a->W > 0x7fffffffLL / 2)
     return set_error(YAMB_EINVAL, "block_eval: too many pixels");
-  BlockEvalDev p;
   memset(&p, 0, sizeof(p));
   p.N = a->N; p.H = a->H; p.W = a->W;
   p.Ho = (a->H - 1) / a->stride + 1;      // pad 1, k 3
@@ -803,6 +854,19 @@ static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, boo
   p.KB = (kpad + 63) / 64;
   p.Npad = (a->Cout + 15) / 16 * 16;
   p.NC = (a->Chid + 63) / 64;
+  return 0;
+}
+
+// CLUSTER: the hidden slices of every tile split over clusters of `cs` CTAs (2, 4 or 8); else cs = 1
+template <bool CLUSTER>
+static int block_eval_launch_impl(const yamb_block_eval* a, cudaStream_t st, bool pool, int cs) {
+  if (!a) return set_error(YAMB_EINVAL, "null args");
+  if (CLUSTER ? (cs != 2 && cs != 4 && cs != 8) : cs != 1)
+    return set_error(YAMB_EINVAL, "block_eval: cluster size must be 2, 4 or 8 (got %d)", cs);
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  BlockEvalDev p;
+  int rc = block_eval_setup(a, pool, cs, p);
+  if (rc) return rc;
   const bool ex = a->w_expand != nullptr;
   // fewest tiles among the geometries of (k, stride); each holds its input tile in <= 256 rows.
   // Stride 1, k = 3 / 5: 7x16 unless two 7x7 images per tile take fewer (a 7x14 tile never would:

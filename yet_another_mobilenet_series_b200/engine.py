@@ -477,16 +477,19 @@ def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, sta
     launch(nat.lib().yamb_depthwise_bwd, d, tag, 4 * Cc * (m_in + m_out), 4 * m_out * Cc * k * k)
 
 
-def _se_fc(se, pooled, u, v, gate):
+def _se_fc(se, pooled, u, v, gate, packed=None):
     """gate = sigmoid(W_e act(W_r pooled + b_r) + b_e) of the Squeeze-and-Excitation module `se`
-    on pooled [N, C], keeping u = W_r pooled + b_r and v = act(u) [N, R] (fp32 throughout)."""
+    on pooled [N, C], keeping u = W_r pooled + b_r and v = act(u) [N, R] (fp32 throughout).
+    packed: (W_r, W_e, b_e) over another hidden order (the multi-branch eval path) instead of the
+    module's own."""
     N, Cc = pooled.shape
     R = se.se_reduce.weight.shape[0]
+    w_r, w_e, b_e = packed or (se.se_reduce.weight, se.se_expand.weight, se.se_expand.bias)
     f = nat.SeFc()
     f.N, f.C, f.R, f.act = N, Cc, R, act_code_of(se.active_fn)
     f.pooled = pooled.data_ptr()
-    f.w_r, f.b_r = se.se_reduce.weight.data_ptr(), se.se_reduce.bias.data_ptr()
-    f.w_e, f.b_e = se.se_expand.weight.data_ptr(), se.se_expand.bias.data_ptr()
+    f.w_r, f.b_r = w_r.data_ptr(), se.se_reduce.bias.data_ptr()
+    f.w_e, f.b_e = w_e.data_ptr(), b_e.data_ptr()
     f.u, f.v, f.gate = u.data_ptr(), v.data_ptr(), gate.data_ptr()
     launch(nat.lib().yamb_se_fc_fwd, f, "se_fc", 4 * N * Cc * 2, 4 * N * Cc * R)
 
@@ -1668,6 +1671,208 @@ def eval_forward(block, x):
     return y
 
 
+# ---- eval mode: multi-branch blocks (several depthwise kernel sizes: AtomNAS) in one launch ---------
+# (csrc/block_eval_mb.cu).  Off by default, so that a plain model.eval() forward launches what it
+# always launched: the hidden channels are regrouped by kernel size, so the project sums in another
+# order and the block's output differs from the four-launch sequence in the last bits.  When True
+# (trainer.EvalStep(fused_multi_branch=True) turns it on for its evaluation forwards) every block
+# eval_mb_supported covers runs as yamb_block_eval_mb_pack + the block kernel (+ the SE pool pass
+# and gate FCs first).
+EVAL_MULTI_BRANCH = False
+EVAL_MB_CALLS = 0        # blocks that went through yamb_block_eval_mb_fwd (tests / bench)
+
+# Kinds of block (K_MAX, stride, fused class; the path has the expansion only) that measured at
+# least as fast as the four-launch sequence with its _PadShadow gathers.
+# tests/gpu_eval_bench_multi_branch.py on one H100 80GB HBM3 (700 W power limit), N = 256, device time
+# of every multi-branch block of AtomNAS-C / C+ summed per kind, new path vs four launches:
+# (7, 1, unfused) 5.24 vs 4.71 ms over 16 blocks (faster on the 14x14 / 7x7 blocks of < 400 hidden
+# channels, slower on the 56x56 / 28x28 ones and the widest), (7, 2, unfused) 3.57 vs 2.86 ms,
+# (5, 1, unfused) 0.41 vs 0.40 ms; with SE the pool pass runs the expand and the stencil a second
+# time: (7, 1, fused) 13.97 vs 6.90 ms, (7, 2, fused) 10.37 vs 3.90, (5, 1, fused) 1.16 vs 0.50.
+# No kind measured at least as fast, so none takes the path by default.  MB_SHAPE_RULE = False:
+# every block the kernel covers takes it (tests, the benchmark).
+MB_SHAPE_RULE = True
+MB_FASTER = frozenset()
+
+MbLayout = collections.namedtuple("MbLayout", "map Chid kmax groups")
+
+
+def mb_layout(kernel_sizes, channels):
+    """Packed hidden dimension of a multi-branch block: the branches in order of decreasing kernel
+    size (stable), each padded to a multiple of 8 channels.  map[j] = (branch << 16) | channel, or
+    -1 for a padded channel; groups = [(k, first packed channel)] of decreasing k."""
+    ks, cs = list(kernel_sizes), list(channels)
+    m, groups = [], []
+    for i in sorted(range(len(ks)), key=lambda i: -ks[i]):
+        if not groups or groups[-1][0] != ks[i]:
+            groups.append((ks[i], len(m)))
+        m += [(i << 16) | c for c in range(cs[i])] + [-1] * (_ceil8(cs[i]) - cs[i])
+    return MbLayout(m, len(m), groups[0][0], groups)
+
+
+def mb_kind(block):
+    """(K_MAX, stride, fused class) of a multi-branch block: what MB_SHAPE_RULE decides on."""
+    return max(block.kernel_sizes), block.stride, hasattr(block, "expand_conv")
+
+
+def eval_mb_supported(block, x):
+    """True when the multi-branch eval path covers this block for this call: EVAL_MULTI_BRANCH on,
+    no gradient wanted, 2 or 3 branches with the expansion and 3x3 / 5x5 / 7x7 depthwise kernels
+    (K_MAX 5 or 7), stride 1 or 2, Cin <= 256 and Cout <= 320 multiples of 8, every BatchNorm
+    normalising with running statistics and one eps, an activation the kernel has, no non-local
+    block, and a kind MB_SHAPE_RULE lets through."""
+    if not (EVAL_MULTI_BRANCH and EVAL_FUSED) or torch.is_grad_enabled():
+        return False
+    ks, chans = list(block.kernel_sizes), list(block.channels)
+    if not 2 <= len(ks) <= 3 or not block.expand or block.stride not in (1, 2):
+        return False
+    if any(k not in (3, 5, 7) for k in ks) or max(ks) == 3 or min(chans) <= 0:
+        return False
+    cin, cout = block.input_dim, block.output_dim
+    if cin % 8 or cout % 8 or cin > 256 or cout > 320:
+        return False
+    if x.dim() != 4 or x.shape[0] * x.shape[2] * x.shape[3] >= 2 ** 30:
+        return False
+    parts = block_parts(block)
+    bns = parts.bn1s + [bn for _, bn in parts.dws] + [parts.bn3]
+    if not all(_bn_eval_ready(bn) for bn in bns) or len({bn.eps for bn in bns[:-1]}) != 1:
+        return False
+    if parts.nl is not None:
+        return False
+    try:
+        act_code_of(block.active_fn)
+        if parts.se is not None:
+            act_code_of(parts.se.active_fn)
+    except ValueError:
+        return False
+    return not MB_SHAPE_RULE or mb_kind(block) in MB_FASTER
+
+
+def _mb_state(block, dev, R):
+    """The packed tensors of a multi-branch block on `dev` and its layout (device index map
+    included), in the `_yamb_eval` scratch that deepcopy / pickle drop."""
+    st = block.__dict__.get("_yamb_eval")
+    if st is None:
+        st = block.__dict__["_yamb_eval"] = _ScratchDict()
+    key = ("mb", dev.index)
+    ms = st.get(key)
+    if ms is None:
+        lay = mb_layout(block.kernel_sizes, block.channels)
+        Chid, K, Cin, Cout = lay.Chid, lay.kmax, block.input_dim, block.output_dim
+        f32, bf = torch.float32, torch.bfloat16
+        ms = st[key] = {
+            "layout": lay,
+            "map": torch.tensor(lay.map, dtype=torch.int32, device=dev),
+            "w1": torch.empty(Chid, Cin, device=dev, dtype=bf),
+            "w3": torch.empty(Cout, Chid, device=dev, dtype=bf),
+            "wdw": torch.empty(Chid, K, K, device=dev, dtype=f32),
+            "bn1": torch.empty(4, Chid, device=dev, dtype=f32),
+            "bn2": torch.empty(4, Chid, device=dev, dtype=f32),
+            "se": (torch.empty(R, Chid, device=dev, dtype=f32),
+                   torch.empty(Chid, R, device=dev, dtype=f32),
+                   torch.empty(Chid, device=dev, dtype=f32)) if R else None,
+        }
+    return ms
+
+
+def _mb_pack_args(block, parts, ms):
+    """yamb_block_eval_mb_pack_args of a multi-branch block into its packed tensors `ms`."""
+    lay, se = ms["layout"], parts.se
+    pk = nat.BlockEvalMbPack()
+    pk.Cin, pk.Cout = block.input_dim, block.output_dim
+    pk.R = se.se_reduce.weight.shape[0] if se is not None else 0
+    pk.nbranch = len(block.channels)
+    c0 = 0
+    for i, (k, c) in enumerate(zip(block.kernel_sizes, block.channels)):
+        b = pk.branch[i]
+        b.k, b.C = k, c
+        b.ld = sum(block.channels) if parts.fused else c
+        conv_d, bn2 = parts.dws[i]
+        if parts.fused:     # one expand conv / BN1 / project conv: the branch's rows / columns
+            w1, bn1, w3 = parts.expand_convs[0].weight, parts.bn1s[0], parts.project_convs[0].weight
+            off = c0
+        else:
+            w1, bn1, w3 = parts.expand_convs[i].weight, parts.bn1s[i], parts.project_convs[i].weight
+            off = 0
+        b.w_expand = w1.data_ptr() + 4 * off * pk.Cin
+        for dst, bn, o in ((b.bn1, bn1, off), (b.bn2, bn2, 0)):
+            dst.gamma, dst.beta = _at(bn.weight, o), _at(bn.bias, o)
+            dst.running_mean, dst.running_var = _at(bn.running_mean, o), _at(bn.running_var, o)
+            dst.eps = bn.eps
+        b.w_dw = conv_d.weight.data_ptr()
+        b.w_project = w3.data_ptr() + 4 * off
+        if se is not None:
+            b.se_reduce = se.se_reduce.weight.data_ptr() + 4 * off
+            b.se_expand = se.se_expand.weight.data_ptr() + 4 * off * pk.R
+            b.se_expand_bias = se.se_expand.bias.data_ptr() + 4 * off
+        c0 += c
+    pk.Chid, pk.kmax = lay.Chid, lay.kmax
+    pk.map = ms["map"].data_ptr()
+    pk.w_expand, pk.w_project, pk.w_dw = ms["w1"].data_ptr(), ms["w3"].data_ptr(), ms["wdw"].data_ptr()
+    pk.bn1, pk.bn2 = ms["bn1"].data_ptr(), ms["bn2"].data_ptr()
+    if se is not None:
+        pk.se_reduce, pk.se_expand, pk.se_expand_bias = (t.data_ptr() for t in ms["se"])
+    return pk
+
+
+def eval_forward_mb(block, x):
+    """y = block(x) in eval mode for a multi-branch block; x channels_last bf16 on CUDA.  C-ABI
+    calls: the packing kernel and the block kernel (2); with SE the pool pass and the gate FCs
+    between them (+2)."""
+    global EVAL_MB_CALLS
+    dev = x.device
+    N, Cin, H, W = x.shape
+    parts = block_parts(block)
+    se = parts.se
+    R = se.se_reduce.weight.shape[0] if se is not None else 0
+    ms = _mb_state(block, dev, R)
+    lay = ms["layout"]
+    Chid, Cout, stride = lay.Chid, block.output_dim, block.stride
+    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+    lib = nat.lib()
+    pk = _mb_pack_args(block, parts, ms)
+    w_bytes = 4 * Chid * (Cin + Cout + lay.kmax ** 2 + 8 + 2 * R)
+    launch(lib.yamb_block_eval_mb_pack, pk, "block_eval_mb_pack", 2 * w_bytes, 0)
+    y = torch.empty((N, Cout, Ho, Wo), device=dev, dtype=torch.bfloat16,
+                    memory_format=torch.channels_last)
+    m = nat.BlockEvalMb()
+    a = m.base
+    a.N, a.H, a.W = N, H, W
+    a.Cin, a.Chid, a.Cout = Cin, Chid, Cout
+    a.kernel, a.stride = lay.kmax, stride
+    a.act = act_code_of(block.active_fn)
+    a.residual = 1 if block.use_res_connect else 0
+    a.x, a.y = x.data_ptr(), y.data_ptr()
+    a.w_expand, a.w_project, a.w_dw = ms["w1"].data_ptr(), ms["w3"].data_ptr(), ms["wdw"].data_ptr()
+    eps = parts.dws[0][1].eps
+    for dst, t in ((a.bn1, ms["bn1"]), (a.bn2, ms["bn2"])):
+        dst.gamma, dst.beta, dst.running_mean, dst.running_var = (r.data_ptr() for r in t)
+        dst.eps = eps
+    bn3 = parts.bn3
+    a.bn3.gamma, a.bn3.beta = nat.ptr(bn3.weight), nat.ptr(bn3.bias)
+    a.bn3.running_mean, a.bn3.running_var = bn3.running_mean.data_ptr(), bn3.running_var.data_ptr()
+    a.bn3.eps = bn3.eps
+    m.ngroups = len(lay.groups)
+    for i, (k, c0) in enumerate(lay.groups):
+        m.group_k[i], m.group_c0[i] = k, c0
+    flops = 2 * Chid * N * (H * W * Cin + Ho * Wo * Cout) + \
+        2 * N * Ho * Wo * sum(k * k * c for k, c in zip(block.kernel_sizes, block.channels))
+    act_bytes = 2 * N * H * W * Cin * (2 if a.residual else 1)
+    if se is not None:
+        pooled = torch.empty(N, Chid, device=dev, dtype=torch.float32)
+        gate = torch.empty(N, Chid, device=dev, dtype=torch.float32)
+        uv = torch.empty(2, N, R, device=dev, dtype=torch.float32)
+        a.pooled = pooled.data_ptr()
+        launch(lib.yamb_block_eval_mb_pool_fwd, m, "block_eval_mb_pool", act_bytes + 4 * N * Chid,
+               flops)
+        _se_fc(se, pooled, uv[0], uv[1], gate, packed=ms["se"])
+        a.pooled = None
+        a.gate = gate.data_ptr()
+    launch(lib.yamb_block_eval_mb_fwd, m, "block_eval_mb", act_bytes + 2 * N * Ho * Wo * Cout, flops)
+    EVAL_MB_CALLS += 1
+    return y
+
+
 def block_apply(block, x):
     """Forward of a reference-compatible block module through the sm_90a path."""
     if not x.is_cuda:
@@ -1677,6 +1882,8 @@ def block_apply(block, x):
     x = to_nhwc_bf16(x)
     if eval_supported(block, x):
         return eval_forward(block, x)
+    if eval_mb_supported(block, x):
+        return eval_forward_mb(block, x)
     params = list(block.parameters())
     if needs_padding(block):
         return _PadFn.apply(x, block, *params)

@@ -322,6 +322,34 @@ class BlockEval(C.Structure):
     ]
 
 
+class MbBranch(C.Structure):
+    _fields_ = [
+        ("k", C.c_int32), ("C", C.c_int32), ("ld", C.c_int32),
+        ("w_expand", C.c_void_p), ("bn1", BnEval), ("bn2", BnEval),
+        ("w_dw", C.c_void_p), ("w_project", C.c_void_p),
+        ("se_reduce", C.c_void_p), ("se_expand", C.c_void_p), ("se_expand_bias", C.c_void_p),
+    ]
+
+
+class BlockEvalMbPack(C.Structure):
+    _fields_ = [
+        ("Cin", C.c_int32), ("Cout", C.c_int32), ("R", C.c_int32),
+        ("nbranch", C.c_int32), ("branch", MbBranch * 3),
+        ("Chid", C.c_int32), ("kmax", C.c_int32),
+        ("map", C.c_void_p),
+        ("w_expand", C.c_void_p), ("w_project", C.c_void_p), ("w_dw", C.c_void_p),
+        ("bn1", C.c_void_p), ("bn2", C.c_void_p),
+        ("se_reduce", C.c_void_p), ("se_expand", C.c_void_p), ("se_expand_bias", C.c_void_p),
+    ]
+
+
+class BlockEvalMb(C.Structure):
+    _fields_ = [
+        ("base", BlockEval),
+        ("ngroups", C.c_int32), ("group_k", C.c_int32 * 3), ("group_c0", C.c_int32 * 3),
+    ]
+
+
 class NlGram(C.Structure):
     _fields_ = [
         ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("sub", C.c_int32),
@@ -393,11 +421,11 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
             19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd, 24: Sgd,
             25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
             29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad,
-            33: StemConvTrain, 34: StemConvTrainGrad}
+            33: StemConvTrain, 34: StemConvTrainGrad, 35: BlockEvalMbPack, 36: BlockEvalMb}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -461,6 +489,9 @@ def lib():
         l.yamb_block_eval_pool_fwd.argtypes = [C.POINTER(BlockEval), C.c_void_p]
         for fn in (l.yamb_block_eval_cluster_fwd, l.yamb_block_eval_cluster_pool_fwd):
             fn.argtypes = [C.POINTER(BlockEval), C.c_int32, C.c_void_p]
+        l.yamb_block_eval_mb_pack.argtypes = [C.POINTER(BlockEvalMbPack), C.c_void_p]
+        for fn in (l.yamb_block_eval_mb_fwd, l.yamb_block_eval_mb_pool_fwd):
+            fn.argtypes = [C.POINTER(BlockEvalMb), C.c_void_p]
         l.yamb_instance_norm_fwd.argtypes = [C.POINTER(InFwd), C.c_void_p]
         l.yamb_instance_norm_bwd.argtypes = [C.POINTER(InBwd), C.c_void_p]
         l.yamb_rmsprop_step.argtypes = [C.POINTER(Rmsprop), C.c_void_p]

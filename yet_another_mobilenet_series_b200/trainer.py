@@ -85,7 +85,8 @@ class TrainStep:
                  alpha=0.9, momentum=0.9, eps=1e-3, weight_decay=1e-5, label_smoothing=0.1,
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
-                 input_norm=None, micro_batch=None, fused_tail=False, fused_stem=False):
+                 input_norm=None, micro_batch=None, fused_tail=False, fused_stem=False,
+                 fused_multi_branch=False):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
@@ -115,7 +116,9 @@ class TrainStep:
         activation, its gradient and dh stay out of HBM.  Off by default: the statistics are
         summed in another order (and with Swish dz is rounded after the act' product), so a step
         with it differs from the default in the last bits, the same bits on every run.  It
-        combines with `fused_tail`; a plain `model(x)` outside the step is not affected."""
+        combines with `fused_tail`; a plain `model(x)` outside the step is not affected.
+
+        `fused_multi_branch=True` is handed to the EvalStep that `validate` builds (see there)."""
         self.world = udist.get_world_size_fallback()
         self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
             per_gpu_batch, micro_batch, self.world, base_lr, base_total_batch, ema_decay,
@@ -129,6 +132,7 @@ class TrainStep:
         self.batch = per_gpu_batch
         self.fused_tail = bool(fused_tail)
         self.fused_stem = bool(fused_stem)
+        self.fused_multi_branch = bool(fused_multi_branch)
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
                                eps=eps, eps_inside_sqrt=True, weight_decay=0)
@@ -409,7 +413,8 @@ class TrainStep:
             self._eval_step = EvalStep(model, self.batch, image_size=self.x.shape[-1],
                                        calib_batch=calib_batch, use_graph=self.use_graph,
                                        input_dtype=self.x.dtype,
-                                       input_norm=dataflow.input_norm_of(self.model))
+                                       input_norm=dataflow.input_norm_of(self.model),
+                                       fused_multi_branch=self.fused_multi_branch)
         es = self._eval_step
         if calib_batches is not None:
             es.calibrate(calib_batches, calib_steps)
@@ -484,7 +489,14 @@ class EvalStep:
     SUM at the end when the world is larger than one."""
 
     def __init__(self, model, per_gpu_batch, image_size=224, calib_batch=None, use_graph=True,
-                 input_dtype=torch.bfloat16, optimizer=None, input_norm=None):
+                 input_dtype=torch.bfloat16, optimizer=None, input_norm=None,
+                 fused_multi_branch=False):
+        """`fused_multi_branch=True` runs the multi-branch blocks (several depthwise kernel sizes:
+        AtomNAS) of the evaluation forwards as one packing launch and one block kernel each
+        (engine.EVAL_MULTI_BRANCH) where engine.eval_mb_supported covers them.  Off by default: the
+        hidden channels are regrouped by kernel size, so the project sums in another order and
+        the logits differ from the default in the last bits (the same bits on every run).  A plain
+        `model(x)` outside the step is not affected."""
         _attach_input_norm(model, input_dtype, input_norm)
         dev = next(model.parameters()).device
         if dev.type != "cuda":
@@ -494,6 +506,7 @@ class EvalStep:
         self.world = udist.get_world_size_fallback()
         self.optimizer = optimizer
         self.use_graph = use_graph
+        self.fused_multi_branch = bool(fused_multi_branch)
         self.phases = {"eval": _Phase(per_gpu_batch, image_size, input_dtype, dev),
                        "calib": _Phase(calib_batch or per_gpu_batch, image_size, input_dtype, dev)}
         self.loss_sum = torch.zeros((), device=dev, dtype=torch.float64)
@@ -528,10 +541,12 @@ class EvalStep:
 
     def _eval_body(self, x, t):
         engine.EVAL_TAIL_FUSED = True
+        engine.EVAL_MULTI_BRANCH = self.fused_multi_branch
         try:
             logits = self.model(x)
         finally:
             engine.EVAL_TAIL_FUSED = False
+            engine.EVAL_MULTI_BRANCH = False
         loss, c1, c5 = tail_ops.softmax_ce(logits, t.to(self.dev), 0.0)
         self.loss_sum.add_(loss.double().sum())
         self.counts[0].add_(c1.sum().long())
