@@ -315,6 +315,61 @@ typedef struct yamb_se_fc_grad {
 int yamb_se_fc_fwd(const yamb_se_fc* args, yamb_stream_t stream);
 int yamb_se_fc_bwd(const yamb_se_fc_grad* args, yamb_stream_t stream);
 
+/* ---- training-mode Squeeze-and-Excitation backward without a pass over the hidden tensor --------
+ * The three calls below take the place of yamb_se_bwd_reduce_bwd, yamb_se_bwd_apply_bwd and
+ * yamb_depthwise_bwd in the backward of a block with SE:
+ *   yamb_se_bwd_stats -> yamb_se_fc_bwd -> yamb_se_bn_bwd_finalize (per BatchNorm-2 slice)
+ *   -> yamb_depthwise_bwd_se (per branch)
+ * so that dz2 = (dY*gate + dpool)*act'(z2) is never written: the depthwise backward forms it while
+ * it stages dY.  z2 = scale*h + shift is BatchNorm-2's output, xhat2 = (h - mean)*invstd.
+ *
+ * se_bwd_stats reads dY and h once and writes
+ *   dgate[n][c]: the bits of yamb_se_bwd_reduce_bwd on the same arguments (same pixel chunks,
+ *                order and bf16 rounding of a2);
+ *   sums [4][N][C] (double): A = sum_HW dY*act'(z2), B = sum_HW act'(z2),
+ *                A' = sum_HW dY*act'(z2)*xhat2, B' = sum_HW act'(z2)*xhat2.
+ *   Each thread sums in fp32 in a fixed order; its partials are added across threads and pixel
+ *   chunks in double, in a fixed order.  No float atomics: the same bits on every call.
+ * N <= 65535, C a multiple of 8, dy / h 16-byte aligned with pitches >= C and multiples of 8. */
+typedef struct yamb_se_bwd_stats {
+  int32_t N, HW, C, ldd, ldh;
+  const void* dy; const void* h;            /* bf16 [N*HW][ldd], [N*HW][ldh] */
+  const float* scale; const float* shift;   /* [C] BatchNorm-2 coefficients */
+  int32_t act;                              /* YAMB_ACT_* after BatchNorm-2 */
+  const float* mean; const float* invstd;   /* [C] BatchNorm-2 statistics of the forward */
+  float* dgate;                             /* out [N][C] */
+  double* sums;                             /* out [4][N][C]: A, B, A', B' */
+} yamb_se_bwd_stats;
+
+/* The BatchNorm-2 backward of one BatchNorm slice once dpool exists (yamb_se_fc_bwd):
+ *   sum_HW dz2 = gate*A + dpool*B,  sum_HW dz2*xhat2 = gate*A' + dpool*B'  per (n, c), added over n
+ *   in sample order in double, then bn's finalize (dgamma, dbeta +=; ca, cb, cc) as
+ *   yamb_se_bwd_apply_bwd finalizes it.  bn->partials / bn->counter are not used.  sums, gate and
+ *   dpool are pre-offset to the slice's first channel; lds, ldg >= C. */
+typedef struct yamb_se_bn_bwd_finalize_args {
+  int32_t N, C;
+  const double* sums; int32_t lds;          /* [4][N][lds] from yamb_se_bwd_stats */
+  const float* gate; const float* dpool; int32_t ldg;   /* [N][ldg] */
+  const yamb_bn_bwd* bn;
+} yamb_se_bn_bwd_finalize_args;
+
+/* yamb_depthwise_bwd with dw.dz = dY = d(a2*gate), the project dgrad's output, instead of dz2: every
+ * staged dY element becomes dz2 = bf16((dY*gate[n][c] + dpool[n][c]) * act'(scale*h + shift)), the
+ * fp32 expression and rounding of yamb_se_bwd_apply_bwd, then dh = ca*dz2 + cb*h + cc as in
+ * yamb_depthwise_bwd.  dx, dw and the statistics in dw.bn are bitwise those of
+ * yamb_se_bwd_apply_bwd followed by yamb_depthwise_bwd with the same ca / cb / cc.  gate, dpool,
+ * scale and shift are pre-offset to the slice and 16-byte aligned, ldg >= dw.C a multiple of 4. */
+typedef struct yamb_dw_bwd_se {
+  yamb_dw_bwd dw;
+  const float* gate; const float* dpool; int32_t ldg;   /* [N][ldg] */
+  const float* scale; const float* shift;               /* [C] BatchNorm-2 coefficients */
+  int32_t act;                                          /* YAMB_ACT_* after BatchNorm-2 */
+} yamb_dw_bwd_se;
+
+int yamb_se_bwd_stats_bwd(const yamb_se_bwd_stats* args, yamb_stream_t stream);
+int yamb_se_bn_bwd_finalize(const yamb_se_bn_bwd_finalize_args* args, yamb_stream_t stream);
+int yamb_depthwise_bwd_se(const yamb_dw_bwd_se* args, yamb_stream_t stream);
+
 int yamb_bn_apply_fwd(const yamb_bn_apply* args, yamb_stream_t stream);
 int yamb_se_bwd_reduce_bwd(const yamb_se_bwd_reduce* args, yamb_stream_t stream);
 int yamb_se_bwd_apply_bwd(const yamb_se_bwd_apply* args, yamb_stream_t stream);
@@ -751,7 +806,8 @@ int yamb_max_ctas(void);
  * 18 softmax_ce_grad, 19 stem_conv, 20 bn_eval, 21 block_eval, 22 in_fwd, 23 in_bwd, 24 sgd,
  * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8, 29 expand_bwd_args,
  * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad, 33 stem_conv_train,
- * 34 stem_conv_train_grad, 35 block_eval_mb_pack_args, 36 block_eval_mb) so bindings can self-check */
+ * 34 stem_conv_train_grad, 35 block_eval_mb_pack_args, 36 block_eval_mb, 37 se_bwd_stats,
+ * 38 se_bn_bwd_finalize_args, 39 dw_bwd_se) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

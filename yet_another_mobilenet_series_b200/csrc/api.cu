@@ -148,6 +148,9 @@ int yamb_struct_size(int which) {
     case 34: return (int)sizeof(yamb_stem_conv_train_grad);
     case 35: return (int)sizeof(yamb_block_eval_mb_pack_args);
     case 36: return (int)sizeof(yamb_block_eval_mb);
+    case 37: return (int)sizeof(yamb_se_bwd_stats);
+    case 38: return (int)sizeof(yamb_se_bn_bwd_finalize_args);
+    case 39: return (int)sizeof(yamb_dw_bwd_se);
     default: return -1;
   }
 }
@@ -176,6 +179,9 @@ int yamb_bn_bwd_apply_bwd(const yamb_bn_bwd_apply* a, yamb_stream_t s) { return 
 int yamb_se_pool_fwd(const yamb_se_pool* a, yamb_stream_t s) { return yamb::se_pool_launch(a, YAMB_ST(s)); }
 int yamb_se_bwd_reduce_bwd(const yamb_se_bwd_reduce* a, yamb_stream_t s) { return yamb::se_bwd_reduce_launch(a, YAMB_ST(s)); }
 int yamb_se_bwd_apply_bwd(const yamb_se_bwd_apply* a, yamb_stream_t s) { return yamb::se_bwd_apply_launch(a, YAMB_ST(s)); }
+int yamb_se_bwd_stats_bwd(const yamb_se_bwd_stats* a, yamb_stream_t s) { return yamb::se_bwd_stats_launch(a, YAMB_ST(s)); }
+int yamb_se_bn_bwd_finalize(const yamb_se_bn_bwd_finalize_args* a, yamb_stream_t s) { return yamb::se_bn_bwd_finalize_launch(a, YAMB_ST(s)); }
+int yamb_depthwise_bwd_se(const yamb_dw_bwd_se* a, yamb_stream_t s) { return yamb::dw_bwd_se_launch(a, YAMB_ST(s)); }
 int yamb_se_fc_fwd(const yamb_se_fc* a, yamb_stream_t s) { return yamb::se_fc_fwd_launch(a, YAMB_ST(s)); }
 int yamb_se_fc_bwd(const yamb_se_fc_grad* a, yamb_stream_t s) { return yamb::se_fc_bwd_launch(a, YAMB_ST(s)); }
 int yamb_softmax_ce_fwd(const yamb_softmax_ce* a, yamb_stream_t s) { return yamb::softmax_ce_fwd_launch(a, YAMB_ST(s)); }

@@ -123,21 +123,27 @@ __device__ __forceinline__ void bn_fwd_finalize(const yamb_bn_fwd& f, int C) {
   }
 }
 
+// channel c of the backward finalize from its totals s = sum(dz), q = sum(dz * xhat);
+// inv_count = 1 / f.count
+__device__ __forceinline__ void bn_bwd_coeffs(const yamb_bn_bwd& f, int c, double s, double q,
+                                              double inv_count) {
+  if (f.dgamma) f.dgamma[c] += (float)q;
+  if (f.dbeta) f.dbeta[c] += (float)s;
+  float g = f.gamma ? f.gamma[c] : 1.f;
+  float r = f.invstd[c];
+  float mu = f.mean[c];
+  float sc = g * r;
+  float m1 = (float)(s * inv_count), m2 = (float)(q * inv_count);
+  f.ca[c] = sc;
+  f.cb[c] = f.use_batch_stats ? -sc * r * m2 : 0.f;
+  f.cc[c] = f.use_batch_stats ? sc * (mu * r * m2 - m1) : 0.f;
+}
+
 __device__ __forceinline__ void bn_bwd_finalize(const yamb_bn_bwd& f, int C) {
   const double inv_count = 1.0 / (double)f.count;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     double s = take_total(f.partials + c), q = take_total(f.partials + C + c);
-    // s = sum(dz), q = sum(dz * xhat)
-    if (f.dgamma) f.dgamma[c] += (float)q;
-    if (f.dbeta) f.dbeta[c] += (float)s;
-    float g = f.gamma ? f.gamma[c] : 1.f;
-    float r = f.invstd[c];
-    float mu = f.mean[c];
-    float sc = g * r;
-    float m1 = (float)(s * inv_count), m2 = (float)(q * inv_count);
-    f.ca[c] = sc;
-    f.cb[c] = f.use_batch_stats ? -sc * r * m2 : 0.f;
-    f.cc[c] = f.use_batch_stats ? sc * (mu * r * m2 - m1) : 0.f;
+    bn_bwd_coeffs(f, c, s, q, inv_count);
   }
 }
 

@@ -73,7 +73,7 @@ int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
   return set_error(YAMB_ECUDA, "dw fwd launch: no kernel for k=%d stride=%d ct=%d tw=%d", k, s, ct, tw);
 }
 
-int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
+int dw_bwd_setup(const yamb_dw_bwd* a, DwBwdDev* out, int* ct_out, size_t* smem_out) {
   if (!a) return set_error(YAMB_EINVAL, "null args");
   int rc = check_common(a->N, a->H, a->W, a->C, a->ldc, a->k, a->stride);
   if (rc) return rc;
@@ -88,7 +88,7 @@ int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   const int k = a->k, s = a->stride, pad = (k - 1) / 2;
   const int ct = pick_ct(a->C, a->H);
-  DwBwdDev p;
+  DwBwdDev& p = *out;
   p.N = a->N; p.H = a->H; p.W = a->W; p.C = a->C; p.ldc = a->ldc;
   p.Ho = (a->H + 2 * pad - k) / s + 1;
   p.Wo = (a->W + 2 * pad - k) / s + 1;
@@ -117,6 +117,18 @@ int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
       ((size_t)(2 * rh * rw + tih * tiw) * ct + (size_t)(7 + 2 * k * k) * ct) * sizeof(float) +
       2 * (size_t)ct * sizeof(stat_t);
   if (smem > 220 * 1024) return set_error(YAMB_EINVAL, "depthwise bwd: slice too wide for smem");
+  *ct_out = ct;
+  *smem_out = smem;
+  return 0;
+}
+
+int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
+  DwBwdDev p;
+  int ct;
+  size_t smem;
+  int rc = dw_bwd_setup(a, &p, &ct, &smem);
+  if (rc) return rc;
+  const int k = a->k, s = a->stride;
   if (ct <= 16) rc = dw_bwd_dispatch_narrow(p, k, s, ct, smem, st);
   else if (k == 3 && s == 1 && ct == 64) YAMB_DW_BWD(3, 1, 64, p, smem, p.num_tiles, st);
   else if (k == 3 && s == 2 && ct == 64) YAMB_DW_BWD(3, 2, 64, p, smem, p.num_tiles, st);

@@ -294,12 +294,20 @@ struct SePoolDev {
 // are read (every lane busy whatever C is), 4 rows in flight per thread, lanes reduced through
 // shared memory, then one plain store per (n, c) into the slab of this CTA's pixel chunk
 // (out + blockIdx.x * slab); the launcher adds the slabs in slab order.
-template <bool kBwd>
+// With kStats (se_bwd_stats) the same walk also takes the BatchNorm-2 backward sums of SeStatsDev
+// into double slabs [pixel chunk][4][st->plane], added over the pixel lanes in lane order.
+struct SeStatsDev {
+  const float *mean, *invstd;   // [C] BatchNorm-2 statistics
+  double* sums;                 // slab of pixel chunk b: sums + b * 4 * plane; [4][N][out_ld]
+  long long plane;              // N * out_ld
+};
+template <bool kBwd, bool kStats = false>
 __device__ __forceinline__ void se_rows_reduce(int N, int HW, int C, const __nv_bfloat16* h, int ldh,
                                                const __nv_bfloat16* dy, int ldd, const float* scale,
                                                const float* shift, int act, float out_scale,
-                                               float* out, int out_ld, long long slab) {
-  __shared__ float red[256][9];
+                                               float* out, int out_ld, long long slab,
+                                               const SeStatsDev* st = nullptr) {
+  __shared__ float red[256][kStats ? 41 : 9];
   const int CG = C / 8;
   const int PX = 256 / CG;                       // pixel lanes (host guarantees CG <= 256)
   const int cg = threadIdx.x % CG, px = threadIdx.x / CG;
@@ -307,27 +315,58 @@ __device__ __forceinline__ void se_rows_reduce(int N, int HW, int C, const __nv_
   const int rows_per = (HW + gridDim.x - 1) / gridDim.x;
   const int r0 = blockIdx.x * rows_per, r1 = min(HW, r0 + rows_per);
   float s[8];
+  float sA[8], sB[8], sA2[8], sB2[8];   // kStats: A, B, A', B' (see yamb_se_bwd_stats)
 #pragma unroll
   for (int e = 0; e < 8; ++e) s[e] = 0.f;
+  if constexpr (kStats) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) sA[e] = sB[e] = sA2[e] = sB2[e] = 0.f;
+  }
   if (px < PX) {
     const int c0 = cg * 8;
     const ActParam ap = make_act(act);
-    float sc[8], sh[8];
+    float sc[8], sh[8], mu[8], rs[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) { sc[e] = __ldg(scale + c0 + e); sh[e] = __ldg(shift + c0 + e); }
+    if constexpr (kStats) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { mu[e] = __ldg(st->mean + c0 + e); rs[e] = __ldg(st->invstd + c0 + e); }
+    }
     const __nv_bfloat16* hb = h + (size_t)n * HW * ldh + c0;
     const __nv_bfloat16* db = kBwd ? dy + (size_t)n * HW * ldd + c0 : nullptr;
     auto body = [&](const uint4& hr, const uint4& dr) {
       float v[8];
       unpack8(hr, v);
+      float hv[8], z[8];
+      if constexpr (kStats) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) hv[e] = v[e];
+      }
 #pragma unroll
       for (int e = 0; e < 8; ++e) v[e] = fmaf(sc[e], v[e], sh[e]);
+      if constexpr (kStats) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) z[e] = v[e];
+      }
       act_vec<8>(v, ap);
       if (kBwd) {
         float d[8];
         unpack8(dr, d);
 #pragma unroll
         for (int e = 0; e < 8; ++e) s[e] = fmaf(d[e], round_bf16(v[e]), s[e]);
+        if constexpr (kStats) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            // act' and xhat as se_bwd_apply_kernel forms them
+            const float g = act_bwd_rt(z[e], ap, act);
+            const float xh = (hv[e] - mu[e]) * rs[e];
+            const float t = d[e] * g;
+            sA[e] += t;
+            sB[e] += g;
+            sA2[e] = fmaf(t, xh, sA2[e]);
+            sB2[e] = fmaf(g, xh, sB2[e]);
+          }
+        }
       } else {
 #pragma unroll
         for (int e = 0; e < 8; ++e) s[e] += round_bf16(v[e]);
@@ -351,6 +390,15 @@ __device__ __forceinline__ void se_rows_reduce(int N, int HW, int C, const __nv_
   }
 #pragma unroll
   for (int e = 0; e < 8; ++e) red[threadIdx.x][e] = s[e];
+  if constexpr (kStats) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      red[threadIdx.x][8 + e] = sA[e];
+      red[threadIdx.x][16 + e] = sB[e];
+      red[threadIdx.x][24 + e] = sA2[e];
+      red[threadIdx.x][32 + e] = sB2[e];
+    }
+  }
   __syncthreads();
   if (px == 0) {
 #pragma unroll
@@ -358,6 +406,17 @@ __device__ __forceinline__ void se_rows_reduce(int N, int HW, int C, const __nv_
       float t = 0.f;
       for (int j = 0; j < PX; ++j) t += red[j * CG + cg][e];
       out[(size_t)blockIdx.x * slab + (size_t)n * out_ld + cg * 8 + e] = t * out_scale;
+    }
+    if constexpr (kStats) {
+      double* o = st->sums + (size_t)blockIdx.x * 4 * st->plane + (size_t)n * out_ld + cg * 8;
+      for (int k = 0; k < 4; ++k) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          double t = 0.0;
+          for (int j = 0; j < PX; ++j) t += (double)red[j * CG + cg][8 + 8 * k + e];
+          o[(size_t)k * st->plane + e] = t;
+        }
+      }
     }
   }
 }
@@ -382,6 +441,65 @@ struct SeBwdReduceDev {
 __global__ void __launch_bounds__(256) se_bwd_reduce_kernel(const __grid_constant__ SeBwdReduceDev p) {
   se_rows_reduce<true>(p.N, p.HW, p.C, p.h, p.ldh, p.dy, p.ldd, p.scale, p.shift, p.act, 1.f,
                        p.dgate, p.out_ld, p.slab);
+}
+
+// dgate of se_bwd_reduce_kernel (the same bits) plus the BatchNorm-2 backward sums A, B, A', B'
+// (yamb_se_bwd_stats), so that se_bn_bwd_finalize and dw_bwd_se_kernel replace se_bwd_apply.
+struct SeBwdStatsDev {
+  SeBwdReduceDev r;
+  SeStatsDev st;
+};
+__global__ void __launch_bounds__(256) se_bwd_stats_kernel(const __grid_constant__ SeBwdStatsDev p) {
+  se_rows_reduce<true, true>(p.r.N, p.r.HW, p.r.C, p.r.h, p.r.ldh, p.r.dy, p.r.ldd, p.r.scale,
+                             p.r.shift, p.r.act, 1.f, p.r.dgate, p.r.out_ld, p.r.slab, &p.st);
+}
+
+// out[i] = sum over s = 0 .. nslab-1 of part[s * n + i], in that order (double slabs of
+// se_bwd_stats_kernel)
+__global__ void __launch_bounds__(256) se_sums_reduce_kernel(const double* __restrict__ part,
+                                                             int nslab, long long n,
+                                                             double* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    double s = 0.0;
+    for (int k = 0; k < nslab; ++k) s += part[(size_t)k * n + i];
+    out[i] = s;
+  }
+}
+
+// BatchNorm-2 backward of one slice from the sums of se_bwd_stats_kernel and the SE FC backward's
+// dpool: per channel sum(dz) = sum_n gate*A + dpool*B, sum(dz*xhat) = sum_n gate*A' + dpool*B'.
+// A CTA owns 32 channels; its 8 sample lanes (warps) take n = lane, lane + 8, ... and are added in
+// lane order, in double, before the finalize of bn_finalize.cuh.
+struct SeBnFinalizeDev {
+  int N, C, lds, ldg;
+  const double* sums;
+  const float *gate, *dpool;
+  yamb_bn_bwd bn;
+};
+__global__ void __launch_bounds__(256) se_bn_bwd_finalize_kernel(const __grid_constant__ SeBnFinalizeDev p) {
+  __shared__ double red[8][2][32];
+  const int lane = threadIdx.x % 32, nl = threadIdx.x / 32;
+  const int c = blockIdx.x * 32 + lane;
+  double s = 0.0, q = 0.0;
+  if (c < p.C) {
+    const long long plane = (long long)p.N * p.lds;
+    for (int n = nl; n < p.N; n += 8) {
+      const double* a = p.sums + (size_t)n * p.lds + c;
+      const double g = __ldg(p.gate + (size_t)n * p.ldg + c), d = __ldg(p.dpool + (size_t)n * p.ldg + c);
+      s += g * __ldg(a) + d * __ldg(a + plane);
+      q += g * __ldg(a + 2 * plane) + d * __ldg(a + 3 * plane);
+    }
+  }
+  red[nl][0][lane] = s;
+  red[nl][1][lane] = q;
+  __syncthreads();
+  if (nl == 0 && c < p.C) {
+    for (int j = 1; j < 8; ++j) {
+      s += red[j][0][lane];
+      q += red[j][1][lane];
+    }
+    bn_bwd_coeffs(p.bn, c, s, q, 1.0 / (double)p.bn.count);
+  }
 }
 
 // dz = (dY * gate[n][c] + dpool[n][c]) * act'(scale*h + shift)   (in place allowed: dz == dY)
@@ -693,6 +811,77 @@ int se_bwd_apply_launch(const yamb_se_bwd_apply* a, cudaStream_t st) {
   se_bwd_apply_kernel<<<grid, 256, smem, st>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_bwd_apply: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int se_bwd_stats_launch(const yamb_se_bwd_stats* a, cudaStream_t st) {
+  if (!a || a->N <= 0 || a->HW <= 0 || a->C <= 0 || (a->C % 8))
+    return set_error(YAMB_EINVAL, "se_bwd_stats shape");
+  int rc;
+  if ((rc = check_bf16("se_bwd_stats", "dy", a->dy, a->ldd, a->C)) ||
+      (rc = check_bf16("se_bwd_stats", "h", a->h, a->ldh, a->C)))
+    return rc;
+  if (!a->scale || !a->shift || !a->mean || !a->invstd || !a->dgate || !a->sums)
+    return set_error(YAMB_EINVAL, "se_bwd_stats: null pointer");
+  if (a->act < YAMB_ACT_NONE || a->act > YAMB_ACT_HSWISH)
+    return set_error(YAMB_EINVAL, "se_bwd_stats: act=%d", a->act);
+  if (a->N > 65535) return set_error(YAMB_EINVAL, "se_bwd_stats: N <= 65535");
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  // the launch plan and dgate slabs of se_bwd_reduce_launch
+  SeBwdStatsDev p;
+  p.r.N = a->N; p.r.HW = a->HW; p.r.C = a->C; p.r.ldd = a->ldd; p.r.ldh = a->ldh;
+  p.r.dy = (const __nv_bfloat16*)a->dy; p.r.h = (const __nv_bfloat16*)a->h;
+  p.r.scale = a->scale; p.r.shift = a->shift; p.r.act = a->act;
+  int chunks;
+  rc = se_slabs(a->N, a->HW, a->C, a->dgate, st, &chunks, &p.r.dgate);
+  if (rc) return rc;
+  p.r.out_ld = a->C;
+  p.r.slab = (long long)a->N * a->C;
+  p.st.mean = a->mean; p.st.invstd = a->invstd;
+  p.st.plane = (long long)a->N * a->C;
+  const long long nsum = 4 * p.st.plane;
+  p.st.sums = a->sums;
+  if (chunks > 1) {
+    float* part = nullptr;
+    if ((rc = det_alloc((size_t)chunks * nsum * sizeof(double), st, &part))) {
+      if (p.r.dgate != a->dgate) det_free(p.r.dgate, st);
+      return rc;
+    }
+    p.st.sums = reinterpret_cast<double*>(part);
+  }
+  for (int c0 = 0; c0 < a->C; c0 += 2048) {
+    SeBwdStatsDev q = p;
+    q.r.C = a->C - c0 < 2048 ? a->C - c0 : 2048;
+    q.r.h = p.r.h + c0; q.r.dy = p.r.dy + c0; q.r.scale = p.r.scale + c0; q.r.shift = p.r.shift + c0;
+    q.r.dgate = p.r.dgate + c0;
+    q.st.mean = p.st.mean + c0; q.st.invstd = p.st.invstd + c0; q.st.sums = p.st.sums + c0;
+    dim3 grid(chunks, a->N);
+    se_bwd_stats_kernel<<<grid, 256, 0, st>>>(q);
+  }
+  if (chunks > 1) {
+    const long long blocks = (nsum + 255) / 256, cap = 4LL * max_ctas();
+    se_sums_reduce_kernel<<<(int)(blocks < cap ? blocks : cap), 256, 0, st>>>(p.st.sums, chunks, nsum,
+                                                                               a->sums);
+    det_free(reinterpret_cast<float*>(p.st.sums), st);
+  }
+  return se_slabs_done(p.r.dgate, chunks, a->N, a->C, a->dgate, st, "se_bwd_stats");
+}
+
+int se_bn_bwd_finalize_launch(const yamb_se_bn_bwd_finalize_args* a, cudaStream_t st) {
+  if (!a || a->N <= 0 || a->C <= 0 || !a->bn) return set_error(YAMB_EINVAL, "se_bn_bwd_finalize shape");
+  if (a->lds < a->C || a->ldg < a->C)
+    return set_error(YAMB_EINVAL, "se_bn_bwd_finalize: lds=%d ldg=%d need >= C=%d", a->lds, a->ldg, a->C);
+  const yamb_bn_bwd& b = *a->bn;
+  if (!a->sums || !a->gate || !a->dpool || !b.mean || !b.invstd || !b.ca || !b.cb || !b.cc)
+    return set_error(YAMB_EINVAL, "se_bn_bwd_finalize: null pointer");
+  if (b.count <= 0) return set_error(YAMB_EINVAL, "se_bn_bwd_finalize: bn count %lld", (long long)b.count);
+  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  SeBnFinalizeDev p;
+  p.N = a->N; p.C = a->C; p.lds = a->lds; p.ldg = a->ldg;
+  p.sums = a->sums; p.gate = a->gate; p.dpool = a->dpool; p.bn = b;
+  se_bn_bwd_finalize_kernel<<<(a->C + 31) / 32, 256, 0, st>>>(p);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(YAMB_ECUDA, "se_bn_bwd_finalize: %s", cudaGetErrorString(e));
   return 0;
 }
 

@@ -39,6 +39,9 @@ int bn_bwd_apply_launch(const yamb_bn_bwd_apply* a, cudaStream_t stream);
 int se_pool_launch(const yamb_se_pool* a, cudaStream_t stream);
 int se_bwd_reduce_launch(const yamb_se_bwd_reduce* a, cudaStream_t stream);
 int se_bwd_apply_launch(const yamb_se_bwd_apply* a, cudaStream_t stream);
+int se_bwd_stats_launch(const yamb_se_bwd_stats* a, cudaStream_t stream);
+int se_bn_bwd_finalize_launch(const yamb_se_bn_bwd_finalize_args* a, cudaStream_t stream);
+int dw_bwd_se_launch(const yamb_dw_bwd_se* a, cudaStream_t stream);
 int se_fc_fwd_launch(const yamb_se_fc* a, cudaStream_t stream);
 int se_fc_bwd_launch(const yamb_se_fc_grad* a, cudaStream_t stream);
 int softmax_ce_fwd_launch(const yamb_softmax_ce* a, cudaStream_t stream);

@@ -127,6 +127,19 @@ class Workspace:
         # 2 * max_c doubles, kept in a float32 tensor
         self.partials = torch.zeros(4 * self.max_c, device=device, dtype=torch.float32)
         self.counter = torch.zeros(4, device=device, dtype=torch.int32)
+        self._se_sums = None
+        self._se_sums_old = []
+
+    def se_sums(self, n):
+        """A float64 buffer of >= n elements for the per-(sample, channel) sums that pass from
+        se_bwd_stats to se_bn_bwd_finalize within one block's backward (the kernels of one stream
+        use it one block after the other).  A buffer that is outgrown stays alive: a captured CUDA
+        graph may address it."""
+        if self._se_sums is None or self._se_sums.numel() < n:
+            if self._se_sums is not None:
+                self._se_sums_old.append(self._se_sums)
+            self._se_sums = torch.empty(n, device=self.partials.device, dtype=torch.float64)
+        return self._se_sums
 
     def stats(self, C):
         """(partials, counter) device pointers for a statistics kernel over C channels."""
@@ -455,11 +468,13 @@ def _dw_fwd(conv, nhw, x, y, tag, pre=None, stats=None):
     launch(nat.lib().yamb_depthwise_fwd, d, tag, 2 * Cc * (m_in + m_out), 2 * m_out * Cc * k * k)
 
 
-def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, stats=None):
+def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, stats=None, se=None):
     """Backward of `_dw_fwd` from the output gradient ca*dz + cb*h + cc (coef = (ca, cb, cc)):
     weight gradient += into dw, input gradient into dx, taken back through `pre` when given (its
     BatchNorm backward statistics into `stats`), + residual.  Every matrix is read with dz's
-    pitch."""
+    pitch.  se = (gate, dpool, scale, shift, act) of a Squeeze-and-Excitation block: dz is then
+    dY = d(a2*gate) and the kernel forms dz2 = (dY*gate + dpool)*act'(scale*h + shift) on load
+    (yamb_depthwise_bwd_se)."""
     k, s = conv.kernel_size[0], conv.stride[0]
     Cc = dz.shape[1]
     d = nat.DwBwd()
@@ -474,7 +489,16 @@ def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, sta
     if stats is not None:
         d.bn = C.pointer(stats)
     m_in, m_out = N * H * W, N * ((H - 1) // s + 1) * ((W - 1) // s + 1)
-    launch(nat.lib().yamb_depthwise_bwd, d, tag, 4 * Cc * (m_in + m_out), 4 * m_out * Cc * k * k)
+    if se is None:
+        launch(nat.lib().yamb_depthwise_bwd, d, tag, 4 * Cc * (m_in + m_out),
+               4 * m_out * Cc * k * k)
+        return
+    a = nat.DwBwdSe()
+    a.dw = d
+    a.gate, a.dpool, a.ldg = se[0].data_ptr(), se[1].data_ptr(), se[0].stride(0)
+    a.scale, a.shift, a.act = se[2].data_ptr(), se[3].data_ptr(), se[4]
+    launch(nat.lib().yamb_depthwise_bwd_se, a, tag + "_se", 4 * Cc * (m_in + m_out),
+           4 * m_out * Cc * k * k)
 
 
 def _se_fc(se, pooled, u, v, gate, packed=None):
@@ -844,7 +868,6 @@ class BlockPlan:
         (+ their parameter gradients) by yamb_se_fc_bwd, then
         dz2 = (d(a2*gate)*gate + dpool) * act'(z2) with the BN2-backward statistics."""
         lib = nat.lib()
-        se = self.se
         HW = self.Ho * self.Wo
         r = nat.SeBwdReduce()
         r.N, r.HW, r.C, r.ldd, r.ldh = self.N, HW, self.Chid, self.Chid, self.Chid
@@ -852,16 +875,7 @@ class BlockPlan:
         r.scale, r.shift, r.act = self.bn2.scale.data_ptr(), self.bn2.shift.data_ptr(), self.act
         r.dgate = self.dgate.data_ptr()
         launch(lib.yamb_se_bwd_reduce_bwd, r, "se_bwd_reduce", 4 * self.M_out * self.Chid)
-        b = nat.SeFcBwd()
-        b.N, b.C, b.R, b.act, b.inv_hw = self.N, self.Chid, self.se_r, self.se_act, 1.0 / HW
-        b.dgate, b.gate = self.dgate.data_ptr(), self.gate.data_ptr()
-        b.u, b.v, b.pooled = self.se_u.data_ptr(), self.se_v.data_ptr(), self.pooled.data_ptr()
-        b.w_r, b.w_e = se.se_reduce.weight.data_ptr(), se.se_expand.weight.data_ptr()
-        b.dpool, b.dt, b.du = self.dpool.data_ptr(), self.se_dt.data_ptr(), self.se_du.data_ptr()
-        tg = grads["se"]
-        b.g_wr, b.g_br, b.g_we, b.g_be = (tg[k].data_ptr() for k in ("wr", "br", "we", "be"))
-        launch(lib.yamb_se_fc_bwd, b, "se_fc_bwd", 4 * self.N * self.Chid * 4,
-               8 * self.N * self.Chid * self.se_r)
+        self._se_fc_backward(grads)
         for c0, cb in self.bn2.slices:
             s = slice(c0, c0 + cb)
             a = nat.SeBwdApply()
@@ -875,6 +889,49 @@ class BlockPlan:
             a.ldg = self.Chid
             a.bn = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
             launch(lib.yamb_se_bwd_apply_bwd, a, "se_bwd_apply", 6 * self.M_out * cb)
+
+    def _se_backward_fused(self, grads):
+        """SE backward of TRAIN_SE_FUSED: dgate and the per-(sample, channel) sums that the
+        BatchNorm-2 backward statistics factor into by one reduction kernel, the FC backward, then
+        the BatchNorm-2 finalize per slice from those sums, gate and dpool.  dz2 is not written:
+        the depthwise backward forms it from dY (`_dw_bwd` with `se`)."""
+        global TRAIN_SE_CALLS
+        lib = nat.lib()
+        HW = self.Ho * self.Wo
+        sums = Workspace.get(self.dev).se_sums(4 * self.N * self.Chid)
+        r = nat.SeBwdStats()
+        r.N, r.HW, r.C, r.ldd, r.ldh = self.N, HW, self.Chid, self.Chid, self.Chid
+        r.dy, r.h = self.dz2.data_ptr(), self.h2.data_ptr()
+        r.scale, r.shift, r.act = self.bn2.scale.data_ptr(), self.bn2.shift.data_ptr(), self.act
+        r.mean, r.invstd = self.bn2.mean.data_ptr(), self.bn2.invstd.data_ptr()
+        r.dgate, r.sums = self.dgate.data_ptr(), sums.data_ptr()
+        launch(lib.yamb_se_bwd_stats_bwd, r, "se_bwd_stats", 4 * self.M_out * self.Chid)
+        self._se_fc_backward(grads)
+        for c0, cb in self.bn2.slices:
+            f = nat.SeBnBwdFinalize()
+            f.N, f.C = self.N, cb
+            f.sums, f.lds = sums.data_ptr() + 8 * c0, self.Chid
+            f.gate, f.dpool, f.ldg = _at(self.gate, c0), _at(self.dpool, c0), self.Chid
+            f.bn = C.pointer(self.bn2.bwd_struct(self.M_out, grads["bn2"], c0, cb))
+            launch(lib.yamb_se_bn_bwd_finalize, f, "se_bn_bwd_finalize", 48 * self.N * cb)
+        TRAIN_SE_CALLS += 1
+
+    def _se_fc_backward(self, grads):
+        """The backward of the two fully connected layers (+ their parameter gradients) from dgate:
+        dpool for the BatchNorm-2 backward."""
+        lib = nat.lib()
+        se = self.se
+        HW = self.Ho * self.Wo
+        b = nat.SeFcBwd()
+        b.N, b.C, b.R, b.act, b.inv_hw = self.N, self.Chid, self.se_r, self.se_act, 1.0 / HW
+        b.dgate, b.gate = self.dgate.data_ptr(), self.gate.data_ptr()
+        b.u, b.v, b.pooled = self.se_u.data_ptr(), self.se_v.data_ptr(), self.pooled.data_ptr()
+        b.w_r, b.w_e = se.se_reduce.weight.data_ptr(), se.se_expand.weight.data_ptr()
+        b.dpool, b.dt, b.du = self.dpool.data_ptr(), self.se_dt.data_ptr(), self.se_du.data_ptr()
+        tg = grads["se"]
+        b.g_wr, b.g_br, b.g_we, b.g_be = (tg[k].data_ptr() for k in ("wr", "br", "we", "be"))
+        launch(lib.yamb_se_fc_bwd, b, "se_fc_bwd", 4 * self.N * self.Chid * 4,
+               8 * self.N * self.Chid * self.se_r)
 
     # -- backward --------------------------------------------------------------------------------
     def backward(self, x, dy, grads, pre=None, pre_stats=None):
@@ -924,7 +981,10 @@ class BlockPlan:
             launch(lib.yamb_pointwise_gemm, g, "pw_project_dgrad",
                    2 * self.M_out * (self.Cout + (1 if se else 2) * cb),
                    2 * self.M_out * cb * self.Cout)
-        if se:
+        se_fused = _se_fused(self.se)
+        if se_fused:
+            self._se_backward_fused(grads)
+        elif se:
             self._se_backward(grads)
         # 3. project wgrad: dW3[Cout,Chid] += dh3^T * a2
         g = nat.Gemm()
@@ -946,15 +1006,17 @@ class BlockPlan:
         for (c0, cb), conv, dw in zip(self.bn2.slices, self.conv_dw, grads["dw"]):
             s = slice(c0, c0 + cb)
             coef = (self.bn2.ca[s], self.bn2.cb[s], self.bn2.cc[s])
+            se_args = (self.gate[:, s], self.dpool[:, s], self.bn2.scale[s], self.bn2.shift[s],
+                       self.act) if se_fused else None
             if self.expand:
                 _dw_bwd(conv, (self.N, self.H, self.W), self.dz2[:, s], self.h2[:, s], coef, dw,
                         self.h1[:, s], self.dz1[:, s], "dw_bwd",
                         pre=(self.bn1.scale[s], self.bn1.shift[s], self.act),
-                        stats=self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb))
+                        stats=self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb), se=se_args)
             else:
                 _dw_bwd(conv, (self.N, self.H, self.W), self.dz2[:, s], self.h2[:, s], coef, dw,
                         xm, dx, "dw_bwd", pre=pre, residual=dym_skip if self.residual else None,
-                        stats=pre_stats)
+                        stats=pre_stats, se=se_args)
         if not self.expand:
             return dx
         # 5+6. dh1 = ca1*dz1 + cb1*h1 + cc1 formed once, dx = dh1 * W1 (+ dy) and
@@ -1439,6 +1501,27 @@ TRAIN_TAIL_CALLS = 0     # head calls that went through yamb_head_pool_train_fwd
 # load; the activation, its gradient and dh never reach HBM.  Otherwise the unfused sequence runs.
 TRAIN_STEM_FUSED = False
 TRAIN_STEM_CALLS = 0     # stem + first block calls that went through stem_block_train (tests)
+
+# ---- training mode: Squeeze-and-Excitation backward inside the depthwise backward ----------------
+# Off by default: BatchNorm-2's backward statistics are summed from per-(sample, channel) factors
+# instead of over the rounded dz2, so turning it on changes the bits of a training step (the same
+# bits on every run).  When True (trainer.TrainStep(fused_se=True) turns it on for its own forwards
+# and backwards) BlockPlan.backward of every block with SE runs se_bwd_stats -> se_fc_bwd ->
+# se_bn_bwd_finalize -> depthwise_bwd_se instead of se_bwd_reduce -> se_fc_bwd -> se_bwd_apply ->
+# depthwise_bwd: dz2 is formed by the depthwise backward while it stages dY and never reaches HBM.
+TRAIN_SE_FUSED = False
+TRAIN_SE_CALLS = 0       # block backwards that went through se_bwd_stats (tests)
+
+
+def _se_fused(se):
+    """Whether BlockPlan.backward of a block whose SE module is `se` (None: none) runs the SE
+    backward of TRAIN_SE_FUSED."""
+    return TRAIN_SE_FUSED and se is not None
+
+
+def se_backward_fused(block):
+    """Whether the training backward of `block` runs the SE backward of TRAIN_SE_FUSED."""
+    return _se_fused(block_parts(block).se)
 
 
 def _eval_operands(block, dev, Chid, Cin, Cout, conv_e, conv_p):

@@ -164,6 +164,34 @@ class SeBwdApply(C.Structure):
     ]
 
 
+class SeBwdStats(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("HW", C.c_int32), ("C", C.c_int32), ("ldd", C.c_int32),
+        ("ldh", C.c_int32),
+        ("dy", C.c_void_p), ("h", C.c_void_p), ("scale", C.c_void_p), ("shift", C.c_void_p),
+        ("act", C.c_int32),
+        ("mean", C.c_void_p), ("invstd", C.c_void_p),
+        ("dgate", C.c_void_p), ("sums", C.c_void_p),
+    ]
+
+
+class SeBnBwdFinalize(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("C", C.c_int32),
+        ("sums", C.c_void_p), ("lds", C.c_int32),
+        ("gate", C.c_void_p), ("dpool", C.c_void_p), ("ldg", C.c_int32),
+        ("bn", C.POINTER(BnBwd)),
+    ]
+
+
+class DwBwdSe(C.Structure):
+    _fields_ = [
+        ("dw", DwBwd),
+        ("gate", C.c_void_p), ("dpool", C.c_void_p), ("ldg", C.c_int32),
+        ("scale", C.c_void_p), ("shift", C.c_void_p), ("act", C.c_int32),
+    ]
+
+
 class Rmsprop(C.Structure):
     _fields_ = [
         ("n", C.c_int64),
@@ -421,11 +449,12 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
             19: StemConv, 20: BnEval, 21: BlockEval, 22: InFwd, 23: InBwd, 24: Sgd,
             25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
             29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad,
-            33: StemConvTrain, 34: StemConvTrainGrad, 35: BlockEvalMbPack, 36: BlockEvalMb}
+            33: StemConvTrain, 34: StemConvTrainGrad, 35: BlockEvalMbPack, 36: BlockEvalMb,
+            37: SeBwdStats, 38: SeBnBwdFinalize, 39: DwBwdSe}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_se_bwd_stats_bwd", "yamb_se_bn_bwd_finalize", "yamb_depthwise_bwd_se", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -467,6 +496,9 @@ def lib():
         l.yamb_se_pool_fwd.argtypes = [C.POINTER(SePool), C.c_void_p]
         l.yamb_se_bwd_reduce_bwd.argtypes = [C.POINTER(SeBwdReduce), C.c_void_p]
         l.yamb_se_bwd_apply_bwd.argtypes = [C.POINTER(SeBwdApply), C.c_void_p]
+        l.yamb_se_bwd_stats_bwd.argtypes = [C.POINTER(SeBwdStats), C.c_void_p]
+        l.yamb_se_bn_bwd_finalize.argtypes = [C.POINTER(SeBnBwdFinalize), C.c_void_p]
+        l.yamb_depthwise_bwd_se.argtypes = [C.POINTER(DwBwdSe), C.c_void_p]
         l.yamb_softmax_ce_fwd.argtypes = [C.POINTER(SoftmaxCe), C.c_void_p]
         l.yamb_softmax_ce_bwd.argtypes = [C.POINTER(SoftmaxCeGrad), C.c_void_p]
         l.yamb_colsum_bf16.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_void_p,

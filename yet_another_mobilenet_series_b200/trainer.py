@@ -86,7 +86,7 @@ class TrainStep:
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
                  input_norm=None, micro_batch=None, fused_tail=False, fused_stem=False,
-                 fused_multi_branch=False):
+                 fused_multi_branch=False, fused_se=False):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
@@ -118,6 +118,14 @@ class TrainStep:
         with it differs from the default in the last bits, the same bits on every run.  It
         combines with `fused_tail`; a plain `model(x)` outside the step is not affected.
 
+        `fused_se=True` runs the Squeeze-and-Excitation backward of this step's blocks without a
+        pass over the hidden tensor (engine.TRAIN_SE_FUSED): one reduction takes dgate and the
+        per-(sample, channel) factors of BatchNorm-2's backward statistics, and the depthwise
+        backward forms dz2 from dY, the gate and dpool while it stages its tiles, so dz2 is never
+        written.  Off by default: BatchNorm-2's backward statistics are summed in another order, so
+        a step with it differs from the default in the last bits, the same bits on every run.  It
+        combines with `fused_stem` and `fused_tail`; a plain `model(x)` is not affected.
+
         `fused_multi_branch=True` is handed to the EvalStep that `validate` builds (see there)."""
         self.world = udist.get_world_size_fallback()
         self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
@@ -132,6 +140,7 @@ class TrainStep:
         self.batch = per_gpu_batch
         self.fused_tail = bool(fused_tail)
         self.fused_stem = bool(fused_stem)
+        self.fused_se = bool(fused_se)
         self.fused_multi_branch = bool(fused_multi_branch)
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
@@ -202,11 +211,13 @@ class TrainStep:
         n rows."""
         engine.TRAIN_TAIL_FUSED = self.fused_tail
         engine.TRAIN_STEM_FUSED = self.fused_stem
+        engine.TRAIN_SE_FUSED = self.fused_se
         try:
             self._passes(self.x if x is None else x, self.t if t is None else t)
         finally:
             engine.TRAIN_TAIL_FUSED = False
             engine.TRAIN_STEM_FUSED = False
+            engine.TRAIN_SE_FUSED = False
 
     def _passes(self, x, t):
         n, b = x.shape[0], self.micro_batch
