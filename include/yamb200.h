@@ -752,6 +752,36 @@ int yamb_block_eval_mb_pack(const yamb_block_eval_mb_pack_args* args, yamb_strea
 int yamb_block_eval_mb_fwd(const yamb_block_eval_mb* args, yamb_stream_t stream);
 int yamb_block_eval_mb_pool_fwd(const yamb_block_eval_mb* args, yamb_stream_t stream);
 
+/* ---- training-mode expand + depthwise forward, the expanded tile recomputed from x ---------------
+ * Step 2 of a single-branch training block with expansion (reference models/mobilenet_base.py:
+ * 391-411) without reading h1 back: once the expand GEMM (yamb_pointwise_gemm with bn_fwd) has
+ * stored h1 = W1 x and finalised BatchNorm 1's batch coefficients, every depthwise output tile is a
+ * function of an x tile with its halo.  Per tile: x (+halo, TMA) -> wgmma with the GEMM's bf16 W1
+ * -> bf16 (the bits the GEMM stored) -> act(bn1_scale*h1 + bn1_shift) with yamb_depthwise_fwd's
+ * on-load expression, 0 outside the image -> k x k stencil with yamb_depthwise_fwd's tap order ->
+ * raw bf16 z2 -> h2, plus BatchNorm 2's batch statistics of the fp32 z2 into `bn` (last CTA
+ * finalises; count = N*Ho*Wo).  h2 has the bits yamb_depthwise_fwd writes from the GEMM's h1; the
+ * statistics agree with its to double rounding of the partial-sum order.
+ * Covers k in {3,5,7}, stride 1 / 2, 8 <= Cin <= 256, any Chid (multiples of 8).  YAMB_EINVAL for
+ * other shapes or bad pointers before any device work (with or without a device), and when the tile
+ * plan does not fit the device's shared memory (nothing enqueued); YAMB_ENODEV without a device. */
+typedef struct yamb_expand_dw_train {
+  int32_t N, H, W;            /* input pixels (NHWC); output (H-1)/stride+1 x (W-1)/stride+1 */
+  int32_t Cin, Chid;          /* multiples of 8; Cin <= 256 */
+  int32_t kernel, stride;     /* 3, 5 or 7; 1 or 2 */
+  int32_t act;                /* YAMB_ACT_* after BatchNorm 1 */
+  int32_t ldh;                /* row pitch of h2 in channels (>= Chid, multiple of 8) */
+  const void* x;              /* bf16 [N,H,W,Cin] */
+  const void* w_expand;       /* bf16 [Chid][Cin] (the expand GEMM's operand) */
+  const float* bn1_scale;     /* [Chid] BatchNorm-1 coefficients of the batch */
+  const float* bn1_shift;     /* [Chid] */
+  const float* w_dw;          /* fp32 [Chid][k][k] */
+  void* h2;                   /* out bf16 [N,Ho,Wo] rows of ldh channels, channels [0, Chid) */
+  const yamb_bn_fwd* bn;      /* BatchNorm-2 statistics of h2 */
+} yamb_expand_dw_train;
+
+int yamb_expand_dw_train_fwd(const yamb_expand_dw_train* args, yamb_stream_t stream);
+
 /* ---- fused flat-arena RMSprop (+L2 decay, +DDP mean, +EMA, +bf16 repack) -------------------------
  * Replaces RMSprop.step (reference utils/rmsprop.py:67-129), the gradient of cal_l2_loss
  * (utils/optim.py:177-200; l2 * p added where bit 0 of wd_mask is set; bit 1 marks a parameter
@@ -807,7 +837,7 @@ int yamb_max_ctas(void);
  * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8, 29 expand_bwd_args,
  * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad, 33 stem_conv_train,
  * 34 stem_conv_train_grad, 35 block_eval_mb_pack_args, 36 block_eval_mb, 37 se_bwd_stats,
- * 38 se_bn_bwd_finalize_args, 39 dw_bwd_se) so bindings can self-check */
+ * 38 se_bn_bwd_finalize_args, 39 dw_bwd_se, 40 expand_dw_train) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

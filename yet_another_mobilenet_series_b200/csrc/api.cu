@@ -151,6 +151,7 @@ int yamb_struct_size(int which) {
     case 37: return (int)sizeof(yamb_se_bwd_stats);
     case 38: return (int)sizeof(yamb_se_bn_bwd_finalize_args);
     case 39: return (int)sizeof(yamb_dw_bwd_se);
+    case 40: return (int)sizeof(yamb_expand_dw_train);
     default: return -1;
   }
 }
@@ -218,6 +219,9 @@ int yamb_block_eval_mb_fwd(const yamb_block_eval_mb* a, yamb_stream_t s) {
 }
 int yamb_block_eval_mb_pool_fwd(const yamb_block_eval_mb* a, yamb_stream_t s) {
   return yamb::block_eval_mb_launch(a, true, YAMB_ST(s));
+}
+int yamb_expand_dw_train_fwd(const yamb_expand_dw_train* a, yamb_stream_t s) {
+  return yamb::expand_dw_train_launch(a, YAMB_ST(s));
 }
 int yamb_instance_norm_fwd(const yamb_in_fwd* a, yamb_stream_t s) { return yamb::in_fwd_launch(a, YAMB_ST(s)); }
 int yamb_instance_norm_bwd(const yamb_in_bwd* a, yamb_stream_t s) { return yamb::in_bwd_launch(a, YAMB_ST(s)); }

@@ -64,6 +64,7 @@
 #include <tuple>
 #include <type_traits>
 
+#include "bn_finalize.cuh"
 #include "host_util.h"
 #include "prims.cuh"
 
@@ -96,6 +97,12 @@ struct BlockEvalDev {
   int red_pitch;     // Npad + 8 (a quarter warp's rows on distinct banks) where that fits, else Npad
   int ngroups;       // G::MB: hidden channels [gc0[i], gc0[i+1]) have depthwise kernel gk[i]
   int gk[3], gc0[3];
+  // kTrain (expand_dw_train.cu)
+  const float *s1, *t1;   // BatchNorm-1 scale / shift the expand GEMM finalised from the batch
+  __nv_bfloat16* h2;      // out: raw depthwise output [N][Ho][Wo] at row pitch ldh
+  int ldh;
+  int off_stat;           // double [2][Chid]: this CTA's BatchNorm-2 sums
+  yamb_bn_fwd bn2f;       // BatchNorm-2 statistics of h2
 };
 
 // What one launch computes:
@@ -103,7 +110,12 @@ struct BlockEvalDev {
 //   kGate   y = bn3(project(a2s)) (+ x),  a2s = bf16(a2 * gate[n][c])   (Squeeze-and-Excitation)
 //   kPool   no project: every tile writes the spatial sums of a2 over its output pixels inside the
 //           image, times 1 / (Ho * Wo), to its own slab of `part` (det_reduce adds the slabs)
-enum { kPlain = 0, kGate = 1, kPool = 2 };
+//   kTrain  training forward up to the depthwise (yamb_expand_dw_train_fwd): BatchNorm 1 from the
+//           batch coefficients s1 / t1 applied to bf16(h1) exactly as dw_fwd applies it on load,
+//           the raw stencil output z2 -> h2 (bf16), and BatchNorm 2's batch statistics of the fp32
+//           z2 (per-thread fp32 over a run, double from there on, last-CTA bn_fwd_finalize); no
+//           BatchNorm 2, no project
+enum { kPlain = 0, kGate = 1, kPool = 2, kTrain = 3 };
 
 constexpr int kMaxProjChunks = 10;   // 16-column project accumulators per thread (80 registers)
 
@@ -138,7 +150,8 @@ template <class G, bool EXPAND, bool LEAN, int MODE, bool CLUSTER>
 __global__ void __launch_bounds__(256, 1)
 block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW1,
                   const __grid_constant__ CUtensorMap tmW3, const __grid_constant__ BlockEvalDev p) {
-  constexpr bool POOL = MODE == kPool, GATE = MODE == kGate;
+  constexpr bool POOL = MODE == kPool, GATE = MODE == kGate, TRAIN = MODE == kTrain;
+  constexpr bool NOPROJ = POOL || TRAIN;
   constexpr int K = G::K, P = G::P, kTabFloats = tab_floats(G::K);
   constexpr int S = G::S, TOH = G::TOH, TOW = G::TOW, TI = G::TI, IH = G::IH, IW = G::IW;
   constexpr int NPI = G::NPI, NPO = G::NPO, RUN = G::RUN, NRUN = G::NRUN, CPT = G::CPT, NCG = G::NCG;
@@ -160,7 +173,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     mbar_init(bar_w3, 1);
     fence_barrier_init();
   }
-  for (int i = tid; i < (POOL ? 0 : p.Npad); i += 256) {
+  for (int i = tid; i < (NOPROJ ? 0 : p.Npad); i += 256) {
     float sc = 0.f, sh = 0.f;
     if (i < p.Cout) {
       const float r = rsqrtf(p.bn3.var[i] + p.bn3.eps);
@@ -171,12 +184,16 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
     c3[p.Npad + i] = sh;
   }
   // rows of the project A operand beyond the tile's pixels are never written: keep them zero
-  for (int i = tid; i < 16384 / 16; i += 256) reinterpret_cast<uint4*>(sH2)[i] = make_uint4(0u, 0u, 0u, 0u);
+  // (kTrain: sH2 holds only the stencil threads' statistics)
+  for (int i = tid; i < (TRAIN ? 0 : 16384 / 16); i += 256)
+    reinterpret_cast<uint4*>(sH2)[i] = make_uint4(0u, 0u, 0u, 0u);
+  if constexpr (TRAIN)
+    for (int i = tid; i < 2 * p.Chid; i += 256) reinterpret_cast<stat_t*>(smem + p.off_stat)[i] = 0.0;
   const bool control = warp == 7 && lane == 0;
   if (control) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW1);
-    if (!POOL) tma_prefetch_desc(&tmW3);
+    if (!NOPROJ) tma_prefetch_desc(&tmW3);
   }
   fence_proxy_async_smem();
   __syncthreads();
@@ -196,7 +213,12 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       const BnEvalDev& b = tid < 64 ? p.bn1 : p.bn2;
       const int hc = c * 64 + (tid & 63);
       pre_s = pre_t = 0.f;
-      if (hc < p.Chid && (EXPAND || tid >= 64)) {   // no expansion: there is no BatchNorm1
+      if constexpr (TRAIN) {   // BatchNorm 1 only; z2 is stored raw
+        if (tid < 64 && hc < p.Chid) {
+          pre_s = __ldg(p.s1 + hc);
+          pre_t = __ldg(p.t1 + hc);
+        }
+      } else if (hc < p.Chid && (EXPAND || tid >= 64)) {   // no expansion: there is no BatchNorm1
         const float r = rsqrtf(__ldg(b.var + hc) + b.eps);
         pre_s = (b.gamma ? __ldg(b.gamma + hc) : 1.f) * r;
         pre_t = (b.beta ? __ldg(b.beta + hc) : 0.f) - __ldg(b.mean + hc) * pre_s;
@@ -312,7 +334,12 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
               const int col = j * 8 + 2 * (lane & 3);
               const float2 ss = *reinterpret_cast<const float2*>(tb + col);
               const float2 tt = *reinterpret_cast<const float2*>(tb + 64 + col);
-              const float2 v = ffma2(ss, make_float2(e[4 * j + 2 * hh], e[4 * j + 2 * hh + 1]), tt);
+              float2 hv = make_float2(e[4 * j + 2 * hh], e[4 * j + 2 * hh + 1]);
+              if (TRAIN) {   // the bf16 h1 the expand GEMM stores, transformed as dw_fwd does on load
+                const uint32_t hb = pack_bf16(hv.x, hv.y);
+                hv = make_float2(bf16lo(hb), bf16hi(hb));
+              }
+              const float2 v = ffma2(ss, hv, tt);
               uint32_t o;
               if (lean) {
                 o = clamp_bf16x2(pack_bf16(v.x, v.y), lo2, hi2);
@@ -349,7 +376,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       if (warp == 7) {
         // ---- control: W3 slice in; the next slice's W1 (and the next tile's x) in ----
         if (lane == 0) {
-          if (!POOL) {
+          if (!NOPROJ) {
             mbar_arrive_expect_tx(bar_w3, (uint32_t)(p.Npad * 128));
             for (int h = 0; h < p_halves; ++h)
               tma_load_2d(&tmW3, bar_w3, smem + p.off_w3 + h * p_nn * 128, c * 64, h * p_nn);
@@ -462,59 +489,91 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
             }
           }
         }
-        float2 s2v[NV], t2v[NV];
-#pragma unroll
-        for (int v = 0; v < NV; ++v) {
-          s2v[v] = *reinterpret_cast<const float2*>(tb + 128 + cg * CPT + 2 * v);
-          t2v[v] = *reinterpret_cast<const float2*>(tb + 192 + cg * CPT + 2 * v);
-        }
-        // the image of this run's outputs (TI = 2: the second image of the last tile may be past N)
-        const int s_n = g * TI + s_ti;
-        float2 gv[NV];                       // kGate: gate of this run's image, 0 past N / Chid
-        if (GATE) {
+        if constexpr (TRAIN) {
+          // ---- raw z2 -> h2 (bf16) for the outputs inside the image; their sums and sums of
+          //      squares over the run in fp32 (dw_fwd's expressions) -> red[sp][channel] ----
+          const int s_n = g * TI + s_ti, yy = ty * TOH + s_oy, xx0 = tx * TOW + s_ox0;
           const int hc = c * 64 + cg * CPT;  // CPT | 8 | Chid: all CPT channels in range, or none
-          const bool ok = s_n < p.N && hc < p.Chid;
+          const bool row_ok = s_n < p.N && yy < p.Ho && hc < p.Chid;
+          float2 ssum[NV], ssq[NV];
 #pragma unroll
-          for (int v = 0; v < NV; ++v)
-            gv[v] = ok ? make_float2(__ldg(p.gate + (size_t)s_n * p.Chid + hc + 2 * v),
-                                     __ldg(p.gate + (size_t)s_n * p.Chid + hc + 2 * v + 1))
-                       : make_float2(0.f, 0.f);
-        }
-        float2 ps[NV];                       // kPool: sums of a2 over this run's outputs in the image
+          for (int v = 0; v < NV; ++v) ssum[v] = ssq[v] = make_float2(0.f, 0.f);
 #pragma unroll
-        for (int v = 0; v < NV; ++v) ps[v] = make_float2(0.f, 0.f);
-        const int boff = cg * CPT * 2;       // byte offset of this thread's channels inside a row
+          for (int j = 0; j < RUN; ++j) {
+            if (!(row_ok && xx0 + j < p.Wo)) continue;
+            uint32_t wv[NV];
 #pragma unroll
-        for (int j = 0; j < RUN; ++j) {
-          uint32_t wv[NV];
-#pragma unroll
-          for (int v = 0; v < NV; ++v) {
-            const float2 z = ffma2(s2v[v], o2[j][v], t2v[v]);
-            if (lean) {
-              wv[v] = clamp_bf16x2(pack_bf16(z.x, z.y), lo2, hi2);
-            } else {
-              float qq[2] = {z.x, z.y};
-              act_vec<2>(qq, ap);
-              wv[v] = pack_bf16(qq[0], qq[1]);
+            for (int v = 0; v < NV; ++v) {
+              const float2 z = o2[j][v];
+              wv[v] = pack_bf16(z.x, z.y);
+              ssum[v] = make_float2(ssum[v].x + z.x, ssum[v].y + z.y);
+              ssq[v] = make_float2(fmaf(z.x, z.x, ssq[v].x), fmaf(z.y, z.y, ssq[v].y));
             }
-            if (GATE) wv[v] = pack_bf16(bf16lo(wv[v]) * gv[v].x, bf16hi(wv[v]) * gv[v].y);
-          }
-          if (POOL) {
-            const bool in = s_n < p.N && ty * TOH + s_oy < p.Ho && tx * TOW + s_ox0 + j < p.Wo;
-#pragma unroll
-            for (int v = 0; v < NV; ++v)
-              if (in) ps[v] = make_float2(ps[v].x + bf16lo(wv[v]), ps[v].y + bf16hi(wv[v]));
-          } else {
-            const int r = r0 + j;
-            uint8_t* dst = sH2 + r * 128 + (((boff >> 4) ^ (r & 7)) << 4) + (boff & 15);
+            __nv_bfloat16* dst = p.h2 + ((size_t)(s_n * p.Ho + yy) * p.Wo + xx0 + j) * p.ldh + hc;
             if (CPT == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(wv[0], wv[NV - 1]);
             else *reinterpret_cast<uint32_t*>(dst) = wv[0];
           }
-        }
-        if (POOL) {   // -> red[sp][channel] (the sH2 buffer, unused without the project MMAs)
+          float* red = reinterpret_cast<float*>(sH2);
 #pragma unroll
-          for (int v = 0; v < NV; ++v)
-            *reinterpret_cast<float2*>(reinterpret_cast<float*>(sH2) + sp * 64 + cg * CPT + 2 * v) = ps[v];
+          for (int v = 0; v < NV; ++v) {
+            *reinterpret_cast<float2*>(red + sp * 64 + cg * CPT + 2 * v) = ssum[v];
+            *reinterpret_cast<float2*>(red + (NRUN + sp) * 64 + cg * CPT + 2 * v) = ssq[v];
+          }
+        } else {
+          float2 s2v[NV], t2v[NV];
+#pragma unroll
+          for (int v = 0; v < NV; ++v) {
+            s2v[v] = *reinterpret_cast<const float2*>(tb + 128 + cg * CPT + 2 * v);
+            t2v[v] = *reinterpret_cast<const float2*>(tb + 192 + cg * CPT + 2 * v);
+          }
+          // the image of this run's outputs (TI = 2: the second image of the last tile may be past N)
+          const int s_n = g * TI + s_ti;
+          float2 gv[NV];                       // kGate: gate of this run's image, 0 past N / Chid
+          if (GATE) {
+            const int hc = c * 64 + cg * CPT;  // CPT | 8 | Chid: all CPT channels in range, or none
+            const bool ok = s_n < p.N && hc < p.Chid;
+#pragma unroll
+            for (int v = 0; v < NV; ++v)
+              gv[v] = ok ? make_float2(__ldg(p.gate + (size_t)s_n * p.Chid + hc + 2 * v),
+                                       __ldg(p.gate + (size_t)s_n * p.Chid + hc + 2 * v + 1))
+                         : make_float2(0.f, 0.f);
+          }
+          float2 ps[NV];                       // kPool: sums of a2 over this run's outputs in the image
+#pragma unroll
+          for (int v = 0; v < NV; ++v) ps[v] = make_float2(0.f, 0.f);
+          const int boff = cg * CPT * 2;       // byte offset of this thread's channels inside a row
+#pragma unroll
+          for (int j = 0; j < RUN; ++j) {
+            uint32_t wv[NV];
+#pragma unroll
+            for (int v = 0; v < NV; ++v) {
+              const float2 z = ffma2(s2v[v], o2[j][v], t2v[v]);
+              if (lean) {
+                wv[v] = clamp_bf16x2(pack_bf16(z.x, z.y), lo2, hi2);
+              } else {
+                float qq[2] = {z.x, z.y};
+                act_vec<2>(qq, ap);
+                wv[v] = pack_bf16(qq[0], qq[1]);
+              }
+              if (GATE) wv[v] = pack_bf16(bf16lo(wv[v]) * gv[v].x, bf16hi(wv[v]) * gv[v].y);
+            }
+            if (POOL) {
+              const bool in = s_n < p.N && ty * TOH + s_oy < p.Ho && tx * TOW + s_ox0 + j < p.Wo;
+#pragma unroll
+              for (int v = 0; v < NV; ++v)
+                if (in) ps[v] = make_float2(ps[v].x + bf16lo(wv[v]), ps[v].y + bf16hi(wv[v]));
+            } else {
+              const int r = r0 + j;
+              uint8_t* dst = sH2 + r * 128 + (((boff >> 4) ^ (r & 7)) << 4) + (boff & 15);
+              if (CPT == 4) *reinterpret_cast<uint2*>(dst) = make_uint2(wv[0], wv[NV - 1]);
+              else *reinterpret_cast<uint32_t*>(dst) = wv[0];
+            }
+          }
+          if (POOL) {   // -> red[sp][channel] (the sH2 buffer, unused without the project MMAs)
+#pragma unroll
+            for (int v = 0; v < NV; ++v)
+              *reinterpret_cast<float2*>(reinterpret_cast<float*>(sH2) + sp * 64 + cg * CPT + 2 * v) = ps[v];
+          }
         }
       }
       if (has_next) tab_store(tab + ((gc + 1) & 1) * kTabFloats);   // its readers are behind S3
@@ -536,6 +595,19 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
         }
         continue;
       }
+      if (TRAIN) {
+        // ---- BatchNorm-2 statistics: per channel of the slice, the stencil threads' sums in run
+        //      order (double) -> this CTA's totals; red is rewritten only after the next S2 ----
+        if (tid < 128) {
+          const int which = tid >> 6, ch = tid & 63, hc = c * 64 + ch;
+          const float* red = reinterpret_cast<const float*>(sH2) + which * NRUN * 64;
+          stat_t s = 0.0;
+#pragma unroll 1
+          for (int r = 0; r < NRUN; ++r) s += (stat_t)red[r * 64 + ch];
+          if (hc < p.Chid) reinterpret_cast<stat_t*>(smem + p.off_stat)[which * p.Chid + hc] += s;
+        }
+        continue;
+      }
       // ---- project(c): [64 px x 64] x [64 x 16 j], accumulated over the slices, left in flight ----
       mbar_wait(bar_w3, w3_par);       // landed during the stencil
       w3_par ^= 1;
@@ -550,7 +622,7 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
       }
       wgmma_commit();
     }
-    if (POOL) continue;
+    if (NOPROJ) continue;
     // ---- epilogue 2: y = bf16(bn3(h3) (+ x)) ----
     wgmma_wait<0>();
     reg_fence(pacc);
@@ -624,6 +696,17 @@ block_eval_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant
           }
         }
       }
+    }
+  }
+  if constexpr (TRAIN) {
+    // ---- this CTA's BatchNorm-2 totals -> the global accumulator (double); the last CTA
+    //      finalises the statistics ----
+    __syncthreads();
+    const stat_t* st = reinterpret_cast<const stat_t*>(smem + p.off_stat);
+    if (publish_partials(st, p.Chid, p.bn2f.partials, p.bn2f.counter)) {
+      bn_fwd_finalize(p.bn2f, p.Chid);
+      __syncthreads();
+      if (tid == 0) *p.bn2f.counter = 0;
     }
   }
 }

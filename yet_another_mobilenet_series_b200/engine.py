@@ -731,6 +731,7 @@ class BlockPlan:
             self.dgate = _f32(N * Chid, dev).view(N, Chid)
             self.dpool = _f32(N * Chid, dev).view(N, Chid)
         self.conv_dw = [conv for conv, _ in parts.dws]
+        self.expand_dw_kind = expand_dw_kind(block, H, W)
         self.bn1 = _Bn(parts.bn1s, dev) if self.expand else None
         self.bn2 = _Bn([bn for _, bn in parts.dws], dev)
         self.bn3 = _Bn([parts.bn3], dev)
@@ -815,16 +816,19 @@ class BlockPlan:
                 launch(lib.yamb_pointwise_gemm, g, "pw_expand_fwd",
                        2 * self.M_in * (self.Cin + cb), 2 * self.M_in * self.Cin * cb)
         # 2. depthwise per branch (BN1+act applied on load) + BN2 statistics; without the
-        #    expansion hidden == inp, so x has the hidden pitch
+        #    expansion hidden == inp, so x has the hidden pitch.  TRAIN_EXPAND_DW_FUSED: the
+        #    expanded tile recomputed from x instead of reading h1 back, where the kernel covers it
         if not self.bn2.batch_stats:
             self.bn2.eval_coeffs()
-        for (c0, cb), conv in zip(self.bn2.slices, self.conv_dw):
-            s = slice(c0, c0 + cb)
-            _dw_fwd(conv, (self.N, self.H, self.W), self.h1[:, s] if self.expand else xm,
-                    self.h2[:, s], "dw_fwd",
-                    pre=(self.bn1.scale[s], self.bn1.shift[s], self.act) if self.expand else pre,
-                    stats=self.bn2.fwd_struct(self.M_out, c0, cb) if self.bn2.batch_stats
-                    else None)
+        if not (expand_dw_fused(self) and self._expand_dw_train(xm)):
+            for (c0, cb), conv in zip(self.bn2.slices, self.conv_dw):
+                s = slice(c0, c0 + cb)
+                _dw_fwd(conv, (self.N, self.H, self.W), self.h1[:, s] if self.expand else xm,
+                        self.h2[:, s], "dw_fwd",
+                        pre=(self.bn1.scale[s], self.bn1.shift[s], self.act) if self.expand
+                        else pre,
+                        stats=self.bn2.fwd_struct(self.M_out, c0, cb) if self.bn2.batch_stats
+                        else None)
         # 2b. Squeeze-and-Excitation gate (reference mobilenet_base.py:110-113): spatial mean of
         #     a2 = act(bn2(h2)) by a kernel, the two fully connected layers + sigmoid by another,
         #     the gate applied inside the project GEMM's operand transform
@@ -862,6 +866,28 @@ class BlockPlan:
         _bn_apply(self.bn3, self.h3, self.nl_tail.l, 0, "bn_apply")   # l: the non-local input
         self.nl_tail.forward(xm, y, self.residual)
         return y
+
+    def _expand_dw_train(self, xm):
+        """Step 2 of TRAIN_EXPAND_DW_FUSED: h2 and BN2's batch statistics from x, W1 and BN1's
+        batch coefficients (yamb_expand_dw_train_fwd); False, with nothing enqueued, when the
+        kernel declines the shape (the caller then runs dw_fwd)."""
+        global TRAIN_EXPAND_DW_CALLS
+        conv = self.conv_dw[0]
+        k, s = conv.kernel_size[0], conv.stride[0]
+        a = nat.ExpandDwTrain()
+        a.N, a.H, a.W, a.Cin, a.Chid = self.N, self.H, self.W, self.Cin, self.Chid
+        a.kernel, a.stride, a.act, a.ldh = k, s, self.act, self.Chid
+        a.x, a.w_expand = xm.data_ptr(), self.w_exp_bf.data_ptr()
+        a.bn1_scale, a.bn1_shift = self.bn1.scale.data_ptr(), self.bn1.shift.data_ptr()
+        a.w_dw, a.h2 = conv.weight.data_ptr(), self.h2.data_ptr()
+        stats = self.bn2.fwd_struct(self.M_out)
+        a.bn = C.pointer(stats)
+        if not try_launch(nat.lib().yamb_expand_dw_train_fwd, a, "expand_dw_train",
+                          2 * (self.M_in * self.Cin + self.M_out * self.Chid),
+                          2 * self.Chid * (self.M_in * self.Cin + self.M_out * k * k)):
+            return False
+        TRAIN_EXPAND_DW_CALLS += 1
+        return True
 
     def _se_backward(self, grads):
         """SE backward: dgate by a reduction kernel, the backward of the two fully connected layers
@@ -1511,6 +1537,51 @@ TRAIN_STEM_CALLS = 0     # stem + first block calls that went through stem_block
 # depthwise_bwd: dz2 is formed by the depthwise backward while it stages dY and never reaches HBM.
 TRAIN_SE_FUSED = False
 TRAIN_SE_CALLS = 0       # block backwards that went through se_bwd_stats (tests)
+
+
+# ---- training mode: expand + depthwise forward from x (yamb_expand_dw_train_fwd) ------------------
+# Off by default.  When True (trainer.TrainStep(fused_expand_dw=True) turns it on for its own
+# forwards) step 2 of BlockPlan.forward of a training block with one branch and an expansion whose
+# shape EXPAND_DW_SHAPE_RULE accepts recomputes each depthwise input tile from x (TMA halo tile ->
+# wgmma expand with the GEMM's bf16 W1 -> BatchNorm 1 + act -> stencil) instead of reading h1 back.
+# The expand GEMM still writes h1 for the backward.  h2 has dw_fwd's bits; BatchNorm 2's statistics
+# are summed in another order, so a step with it can differ from the default in the last bits.
+# Multi-branch blocks, blocks without expansion and shapes the kernel declines run dw_fwd.
+TRAIN_EXPAND_DW_FUSED = False
+TRAIN_EXPAND_DW_CALLS = 0    # block forwards whose step 2 went through expand_dw_train (tests)
+# EXPAND_DW_SHAPE_RULE sends a block down the path only when its kind (expand_dw_kind) is in
+# EXPAND_DW_FASTER: the kinds that measured at least as fast as the expand GEMM's h1 read back by
+# dw_fwd (tests/gpu_expand_dw_train_bench.py; BASELINE.md §5).  False: every covered block.
+EXPAND_DW_SHAPE_RULE = True
+EXPAND_DW_FASTER = frozenset()
+
+
+def expand_dw_kind(block, H, W):
+    """(k, stride, H, W, Cin, Chid) of a single-branch block with expansion on H x W inputs, the
+    key of EXPAND_DW_SHAPE_RULE; None for a block the path never takes (several branches, no
+    expansion)."""
+    parts = block_parts(block)
+    if not parts.expand_convs or len(parts.dws) != 1:
+        return None
+    conv = parts.dws[0][0]
+    return (conv.kernel_size[0], conv.stride[0], H, W, parts.expand_convs[0].in_channels,
+            conv.out_channels)
+
+
+def _expand_dw_rule(kind):
+    return kind is not None and (not EXPAND_DW_SHAPE_RULE or kind in EXPAND_DW_FASTER)
+
+
+def expand_dw_selected(block, H, W):
+    """Whether EXPAND_DW_SHAPE_RULE lets a training `block` on H x W inputs take the path."""
+    return _expand_dw_rule(expand_dw_kind(block, H, W))
+
+
+def expand_dw_fused(plan):
+    """Whether step 2 of `plan` (a BlockPlan) tries yamb_expand_dw_train_fwd."""
+    return (TRAIN_EXPAND_DW_FUSED and plan.expand and len(plan.conv_dw) == 1
+            and plan.bn1.batch_stats and plan.bn2.batch_stats
+            and _expand_dw_rule(plan.expand_dw_kind))
 
 
 def _se_fused(se):

@@ -438,6 +438,18 @@ class ExpandBwd(C.Structure):
     ]
 
 
+class ExpandDwTrain(C.Structure):
+    _fields_ = [
+        ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32),
+        ("Cin", C.c_int32), ("Chid", C.c_int32),
+        ("kernel", C.c_int32), ("stride", C.c_int32), ("act", C.c_int32), ("ldh", C.c_int32),
+        ("x", C.c_void_p), ("w_expand", C.c_void_p),
+        ("bn1_scale", C.c_void_p), ("bn1_shift", C.c_void_p),
+        ("w_dw", C.c_void_p), ("h2", C.c_void_p),
+        ("bn", C.POINTER(BnFwd)),
+    ]
+
+
 class ExpandBwdPlanInfo(C.Structure):
     _fields_ = [(name, C.c_int32) for name in (
         "block_n", "panels", "slabs", "slab_rows", "grid", "num_stages", "smem_bytes")]
@@ -450,11 +462,11 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
             25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
             29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad,
             33: StemConvTrain, 34: StemConvTrainGrad, 35: BlockEvalMbPack, 36: BlockEvalMb,
-            37: SeBwdStats, 38: SeBnBwdFinalize, 39: DwBwdSe}
+            37: SeBwdStats, 38: SeBnBwdFinalize, 39: DwBwdSe, 40: ExpandDwTrain}
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_se_bwd_stats_bwd", "yamb_se_bn_bwd_finalize", "yamb_depthwise_bwd_se", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_se_bwd_stats_bwd", "yamb_se_bn_bwd_finalize", "yamb_depthwise_bwd_se", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_expand_dw_train_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -524,6 +536,7 @@ def lib():
         l.yamb_block_eval_mb_pack.argtypes = [C.POINTER(BlockEvalMbPack), C.c_void_p]
         for fn in (l.yamb_block_eval_mb_fwd, l.yamb_block_eval_mb_pool_fwd):
             fn.argtypes = [C.POINTER(BlockEvalMb), C.c_void_p]
+        l.yamb_expand_dw_train_fwd.argtypes = [C.POINTER(ExpandDwTrain), C.c_void_p]
         l.yamb_instance_norm_fwd.argtypes = [C.POINTER(InFwd), C.c_void_p]
         l.yamb_instance_norm_bwd.argtypes = [C.POINTER(InBwd), C.c_void_p]
         l.yamb_rmsprop_step.argtypes = [C.POINTER(Rmsprop), C.c_void_p]

@@ -86,7 +86,7 @@ class TrainStep:
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
                  input_norm=None, micro_batch=None, fused_tail=False, fused_stem=False,
-                 fused_multi_branch=False, fused_se=False):
+                 fused_multi_branch=False, fused_se=False, fused_expand_dw=False):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
@@ -126,6 +126,14 @@ class TrainStep:
         a step with it differs from the default in the last bits, the same bits on every run.  It
         combines with `fused_stem` and `fused_tail`; a plain `model(x)` is not affected.
 
+        `fused_expand_dw=True` runs the depthwise forward of this step's single-branch blocks with
+        an expansion from x instead of reading h1 back (engine.TRAIN_EXPAND_DW_FUSED): each tile
+        recomputes its expanded input with the expand GEMM's bf16 weights and BatchNorm-1
+        coefficients, where engine.EXPAND_DW_SHAPE_RULE accepts the block's shape.  h2 has the
+        default's bits; BatchNorm-2's statistics are summed in another order, so a step with it can
+        differ from the default in the last bits.  It combines with `fused_stem`, `fused_tail`,
+        `fused_se` and `micro_batch`; a plain `model(x)` is not affected.
+
         `fused_multi_branch=True` is handed to the EvalStep that `validate` builds (see there)."""
         self.world = udist.get_world_size_fallback()
         self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
@@ -141,6 +149,7 @@ class TrainStep:
         self.fused_tail = bool(fused_tail)
         self.fused_stem = bool(fused_stem)
         self.fused_se = bool(fused_se)
+        self.fused_expand_dw = bool(fused_expand_dw)
         self.fused_multi_branch = bool(fused_multi_branch)
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
@@ -212,12 +221,14 @@ class TrainStep:
         engine.TRAIN_TAIL_FUSED = self.fused_tail
         engine.TRAIN_STEM_FUSED = self.fused_stem
         engine.TRAIN_SE_FUSED = self.fused_se
+        engine.TRAIN_EXPAND_DW_FUSED = self.fused_expand_dw
         try:
             self._passes(self.x if x is None else x, self.t if t is None else t)
         finally:
             engine.TRAIN_TAIL_FUSED = False
             engine.TRAIN_STEM_FUSED = False
             engine.TRAIN_SE_FUSED = False
+            engine.TRAIN_EXPAND_DW_FUSED = False
 
     def _passes(self, x, t):
         n, b = x.shape[0], self.micro_batch
