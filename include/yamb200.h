@@ -220,6 +220,41 @@ typedef struct yamb_dw_bwd {
 int yamb_depthwise_fwd(const yamb_dw_fwd* args, yamb_stream_t stream);
 int yamb_depthwise_bwd(const yamb_dw_bwd* args, yamb_stream_t stream);
 
+/* ---- the depthwise of up to three branches in one launch each way ---------------------------------
+ * The branches of a multi-branch block (AtomNAS, the single-path supernet: one per kernel size) are
+ * channel slices of one hidden tensor, each a yamb_depthwise_fwd / _bwd call of its own.  The grouped
+ * launch's grid is the concatenation of those calls' grids: its CTA j finds its branch b from the
+ * prefix sums of `grid` and runs what CTA j - (grid[0] + ... + grid[b-1]) of branch b's own launch
+ * runs (same kernel instantiation, tile walk, pointers, statistics slice), so every output has the
+ * bits of the per-branch calls.  Each branch with `bn` finalises its statistics in its own last CTA,
+ * so each needs its own counter and partials.  The backward reduces each branch's weight-gradient
+ * slabs in slab order after the kernel, as yamb_depthwise_bwd does.
+ * grid[b] (and, backward with k == 7, grid_wgrad[b]: the CTAs of the taps-25..48 weight-gradient
+ * kernel; 0 for k 3 / 5) must be what yamb_depthwise_fwd / _bwd launch for that branch on this
+ * device: yamb_depthwise_grouped_grids fills them.  nbranch 1..3, one stride for all branches,
+ * distinct statistics counters, every branch within the caps of yamb_depthwise_fwd / _bwd, positive
+ * grids: otherwise YAMB_EINVAL before any device work (with or without a device); YAMB_ENODEV
+ * without a device; YAMB_EINVAL also when a grid differs from the per-branch launch's. */
+#define YAMB_DW_MAX_BRANCHES 3
+typedef struct yamb_dw_fwd_grouped {
+  int32_t nbranch;
+  yamb_dw_fwd branch[YAMB_DW_MAX_BRANCHES];
+  int32_t grid[YAMB_DW_MAX_BRANCHES];
+} yamb_dw_fwd_grouped;
+
+typedef struct yamb_dw_bwd_grouped {
+  int32_t nbranch;
+  yamb_dw_bwd branch[YAMB_DW_MAX_BRANCHES];
+  int32_t grid[YAMB_DW_MAX_BRANCHES];
+  int32_t grid_wgrad[YAMB_DW_MAX_BRANCHES];
+} yamb_dw_bwd_grouped;
+
+int yamb_depthwise_fwd_grouped(const yamb_dw_fwd_grouped* args, yamb_stream_t stream);
+int yamb_depthwise_bwd_grouped(const yamb_dw_bwd_grouped* args, yamb_stream_t stream);
+/* Fill grid (and grid_wgrad) of either struct (NULL: skipped) with the grids the per-branch calls
+ * use on the current device, through the sizing those calls run; the other checks as above. */
+int yamb_depthwise_grouped_grids(yamb_dw_fwd_grouped* fwd, yamb_dw_bwd_grouped* bwd);
+
 /* ---- per-channel elementwise / reduction on [M, C] bf16 matrices ---------------------------------
  * bn_apply : y = act(scale*h + shift) * gate[n][c] + residual     (pw_bn + skip connection,
  *            reference models/mobilenet_base.py:448-450, :340-341; SE gating :113)
@@ -837,7 +872,8 @@ int yamb_max_ctas(void);
  * 25 stem_conv_eval, 26 head_pool_eval, 27 gemm_plan_info, 28 stem_conv_u8, 29 expand_bwd_args,
  * 30 expand_bwd_plan_info, 31 head_pool_train, 32 head_pool_train_grad, 33 stem_conv_train,
  * 34 stem_conv_train_grad, 35 block_eval_mb_pack_args, 36 block_eval_mb, 37 se_bwd_stats,
- * 38 se_bn_bwd_finalize_args, 39 dw_bwd_se, 40 expand_dw_train) so bindings can self-check */
+ * 38 se_bn_bwd_finalize_args, 39 dw_bwd_se, 40 expand_dw_train, 41 dw_fwd_grouped,
+ * 42 dw_bwd_grouped) so bindings can self-check */
 int yamb_struct_size(int which);
 
 const char* yamb_last_error(void);

@@ -152,6 +152,8 @@ int yamb_struct_size(int which) {
     case 38: return (int)sizeof(yamb_se_bn_bwd_finalize_args);
     case 39: return (int)sizeof(yamb_dw_bwd_se);
     case 40: return (int)sizeof(yamb_expand_dw_train);
+    case 41: return (int)sizeof(yamb_dw_fwd_grouped);
+    case 42: return (int)sizeof(yamb_dw_bwd_grouped);
     default: return -1;
   }
 }
@@ -173,6 +175,15 @@ int yamb_expand_bwd_plan(const yamb_expand_bwd_args* args, int32_t num_sms, yamb
 #define YAMB_ST(s) reinterpret_cast<cudaStream_t>(s)
 int yamb_depthwise_fwd(const yamb_dw_fwd* a, yamb_stream_t s) { return yamb::dw_fwd_launch(a, YAMB_ST(s)); }
 int yamb_depthwise_bwd(const yamb_dw_bwd* a, yamb_stream_t s) { return yamb::dw_bwd_launch(a, YAMB_ST(s)); }
+int yamb_depthwise_fwd_grouped(const yamb_dw_fwd_grouped* a, yamb_stream_t s) {
+  return yamb::dw_fwd_grouped_launch(a, YAMB_ST(s));
+}
+int yamb_depthwise_bwd_grouped(const yamb_dw_bwd_grouped* a, yamb_stream_t s) {
+  return yamb::dw_bwd_grouped_launch(a, YAMB_ST(s));
+}
+int yamb_depthwise_grouped_grids(yamb_dw_fwd_grouped* f, yamb_dw_bwd_grouped* b) {
+  return yamb::dw_grouped_grids(f, b);
+}
 int yamb_bn_apply_fwd(const yamb_bn_apply* a, yamb_stream_t s) { return yamb::bn_apply_launch(a, YAMB_ST(s)); }
 int yamb_bn_reduce_bwd(const yamb_bn_reduce* a, yamb_stream_t s) { return yamb::bn_reduce_launch(a, YAMB_ST(s)); }
 int yamb_bn_stats_fwd(const yamb_bn_stats* a, yamb_stream_t s) { return yamb::bn_stats_launch(a, YAMB_ST(s)); }

@@ -41,6 +41,20 @@ __device__ __forceinline__ bool arrive_last(uint32_t* counter) {
   return s_is_last != 0;
 }
 
+// arrive_last for a CTA that is one of `nblk` CTAs counted on `counter` (a range of a grouped grid)
+__device__ __forceinline__ bool arrive_last_of(uint32_t* counter, unsigned nblk) {
+  __shared__ uint32_t s_is_last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t prev = atomicAdd(counter, 1u);
+    s_is_last = (prev == nblk - 1) ? 1u : 0u;
+  }
+  __syncthreads();
+  if (s_is_last) __threadfence();
+  return s_is_last != 0;
+}
+
 // Add this CTA's partials (s_part: [2][C] in shared memory) to the global accumulator and return
 // true in the last CTA.  Must be called by ALL threads of the CTA.
 __device__ __forceinline__ bool publish_partials(const stat_t* s_part, int C, stat_t* partials,

@@ -29,17 +29,18 @@ static int pick_ct(int C, int H) {
   return pad32 < pad64 ? 32 : 64;
 }
 
-int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
+int dw_fwd_setup(const yamb_dw_fwd* a, DwFwdDev* out, int* ct_out, int* tw_out, size_t* smem_out,
+                 bool check_device) {
   if (!a) return set_error(YAMB_EINVAL, "null args");
   int rc = check_common(a->N, a->H, a->W, a->C, a->ldc, a->k, a->stride);
   if (rc) return rc;
   if (!a->x || !a->y || !a->w) return set_error(YAMB_EINVAL, "depthwise fwd: null pointer");
   if ((((uintptr_t)a->x) | ((uintptr_t)a->y)) & 15)
     return set_error(YAMB_EINVAL, "depthwise: activations must be 16-byte aligned");
-  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  if (check_device && max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   const int k = a->k, s = a->stride, pad = (k - 1) / 2;
   const int ct = pick_ct(a->C, (a->H + 2 * pad - k) / s + 1);
-  DwFwdDev p;
+  DwFwdDev& p = *out;
   p.N = a->N; p.H = a->H; p.W = a->W; p.C = a->C; p.ldc = a->ldc;
   p.Ho = (a->H + 2 * pad - k) / s + 1;
   p.Wo = (a->W + 2 * pad - k) / s + 1;
@@ -61,9 +62,17 @@ int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
   const int ih = (toh - 1) * s + k, iw = (tow - 1) * s + k;
   const size_t smem = (size_t)ih * iw * ct * sizeof(float) + 2 * (size_t)ct * sizeof(stat_t);
   if (smem > 220 * 1024) return set_error(YAMB_EINVAL, "depthwise fwd: tile too large");
-  if (ct <= 16) return dw_fwd_dispatch_narrow(p, k, s, ct, tw, smem, st);
+  *ct_out = ct;
+  *tw_out = tw;
+  *smem_out = smem;
+  return 0;
+}
+
+int dw_fwd_dispatch(const DwFwdDev& p, int k, int s, int ct, int tw, size_t smem, cudaStream_t st,
+                    int* grid) {
+  if (ct <= 16) return dw_fwd_dispatch_narrow(p, k, s, ct, tw, smem, st, grid);
 #define YAMB_FWD_CASE(KK, SS, CC, TT) \
-  if (k == KK && s == SS && ct == CC && tw == TT) return launch_k(dw_fwd_kernel<KK, SS, CC, TT>, p, smem, p.num_tiles, st)
+  if (k == KK && s == SS && ct == CC && tw == TT) return grid ? grid_k("dw fwd launch", dw_fwd_kernel<KK, SS, CC, TT>, p, smem, p.num_tiles, grid) : launch_k(dw_fwd_kernel<KK, SS, CC, TT>, p, smem, p.num_tiles, st)
   YAMB_FWD_CASE(3, 1, 64, 1); YAMB_FWD_CASE(3, 1, 64, 2); YAMB_FWD_CASE(3, 2, 64, 1); YAMB_FWD_CASE(3, 2, 64, 2);
   YAMB_FWD_CASE(3, 1, 32, 1); YAMB_FWD_CASE(3, 1, 32, 2); YAMB_FWD_CASE(3, 2, 32, 1); YAMB_FWD_CASE(3, 2, 32, 2);
   YAMB_FWD_CASE(5, 1, 64, 1); YAMB_FWD_CASE(5, 1, 64, 2); YAMB_FWD_CASE(5, 2, 64, 1); YAMB_FWD_CASE(5, 2, 64, 2);
@@ -73,7 +82,17 @@ int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
   return set_error(YAMB_ECUDA, "dw fwd launch: no kernel for k=%d stride=%d ct=%d tw=%d", k, s, ct, tw);
 }
 
-int dw_bwd_setup(const yamb_dw_bwd* a, DwBwdDev* out, int* ct_out, size_t* smem_out) {
+int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t st) {
+  DwFwdDev p;
+  int ct, tw;
+  size_t smem;
+  int rc = dw_fwd_setup(a, &p, &ct, &tw, &smem);
+  if (rc) return rc;
+  return dw_fwd_dispatch(p, a->k, a->stride, ct, tw, smem, st);
+}
+
+int dw_bwd_setup(const yamb_dw_bwd* a, DwBwdDev* out, int* ct_out, size_t* smem_out,
+                 bool check_device) {
   if (!a) return set_error(YAMB_EINVAL, "null args");
   int rc = check_common(a->N, a->H, a->W, a->C, a->ldc, a->k, a->stride);
   if (rc) return rc;
@@ -85,7 +104,7 @@ int dw_bwd_setup(const yamb_dw_bwd* a, DwBwdDev* out, int* ct_out, size_t* smem_
     return set_error(YAMB_EINVAL, "depthwise bwd: dz, h and x must be 16-byte aligned");
   if ((((uintptr_t)a->dx) | ((uintptr_t)a->residual)) & 7)
     return set_error(YAMB_EINVAL, "depthwise bwd: dx and residual must be 8-byte aligned");
-  if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
+  if (check_device && max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
   const int k = a->k, s = a->stride, pad = (k - 1) / 2;
   const int ct = pick_ct(a->C, a->H);
   DwBwdDev& p = *out;
@@ -122,27 +141,32 @@ int dw_bwd_setup(const yamb_dw_bwd* a, DwBwdDev* out, int* ct_out, size_t* smem_
   return 0;
 }
 
+int dw_bwd_dispatch(const DwBwdDev& p, int k, int s, int ct, size_t smem, cudaStream_t st,
+                    int* grid) {
+  int rc;
+  if (ct <= 16) rc = dw_bwd_dispatch_narrow(p, k, s, ct, smem, st, grid);
+  else if (k == 3 && s == 1 && ct == 64) YAMB_DW_BWD(3, 1, 64, p, smem, p.num_tiles, st, grid);
+  else if (k == 3 && s == 2 && ct == 64) YAMB_DW_BWD(3, 2, 64, p, smem, p.num_tiles, st, grid);
+  else if (k == 3 && s == 1) YAMB_DW_BWD(3, 1, 32, p, smem, p.num_tiles, st, grid);
+  else if (k == 3 && s == 2) YAMB_DW_BWD(3, 2, 32, p, smem, p.num_tiles, st, grid);
+  else if (k == 5 && s == 1 && ct == 64) YAMB_DW_BWD(5, 1, 64, p, smem, p.num_tiles, st, grid);
+  else if (k == 5 && s == 2 && ct == 64) YAMB_DW_BWD(5, 2, 64, p, smem, p.num_tiles, st, grid);
+  else if (k == 5 && s == 1) YAMB_DW_BWD(5, 1, 32, p, smem, p.num_tiles, st, grid);
+  else if (k == 5 && s == 2) YAMB_DW_BWD(5, 2, 32, p, smem, p.num_tiles, st, grid);
+  else if (k == 7 && s == 1 && ct == 64) YAMB_DW_BWD(7, 1, 64, p, smem, p.num_tiles, st, grid);
+  else if (k == 7 && s == 2 && ct == 64) YAMB_DW_BWD(7, 2, 64, p, smem, p.num_tiles, st, grid);
+  else if (k == 7 && s == 1) YAMB_DW_BWD(7, 1, 32, p, smem, p.num_tiles, st, grid);
+  else YAMB_DW_BWD(7, 2, 32, p, smem, p.num_tiles, st, grid);
+  return rc;
+}
+
 int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t st) {
   DwBwdDev p;
   int ct;
   size_t smem;
   int rc = dw_bwd_setup(a, &p, &ct, &smem);
   if (rc) return rc;
-  const int k = a->k, s = a->stride;
-  if (ct <= 16) rc = dw_bwd_dispatch_narrow(p, k, s, ct, smem, st);
-  else if (k == 3 && s == 1 && ct == 64) YAMB_DW_BWD(3, 1, 64, p, smem, p.num_tiles, st);
-  else if (k == 3 && s == 2 && ct == 64) YAMB_DW_BWD(3, 2, 64, p, smem, p.num_tiles, st);
-  else if (k == 3 && s == 1) YAMB_DW_BWD(3, 1, 32, p, smem, p.num_tiles, st);
-  else if (k == 3 && s == 2) YAMB_DW_BWD(3, 2, 32, p, smem, p.num_tiles, st);
-  else if (k == 5 && s == 1 && ct == 64) YAMB_DW_BWD(5, 1, 64, p, smem, p.num_tiles, st);
-  else if (k == 5 && s == 2 && ct == 64) YAMB_DW_BWD(5, 2, 64, p, smem, p.num_tiles, st);
-  else if (k == 5 && s == 1) YAMB_DW_BWD(5, 1, 32, p, smem, p.num_tiles, st);
-  else if (k == 5 && s == 2) YAMB_DW_BWD(5, 2, 32, p, smem, p.num_tiles, st);
-  else if (k == 7 && s == 1 && ct == 64) YAMB_DW_BWD(7, 1, 64, p, smem, p.num_tiles, st);
-  else if (k == 7 && s == 2 && ct == 64) YAMB_DW_BWD(7, 2, 64, p, smem, p.num_tiles, st);
-  else if (k == 7 && s == 1) YAMB_DW_BWD(7, 1, 32, p, smem, p.num_tiles, st);
-  else YAMB_DW_BWD(7, 2, 32, p, smem, p.num_tiles, st);
-  return rc;
+  return dw_bwd_dispatch(p, a->k, a->stride, ct, smem, st);
 }
 
 }  // namespace yamb

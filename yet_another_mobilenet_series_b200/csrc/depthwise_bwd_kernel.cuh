@@ -5,9 +5,15 @@
 // before dh is formed from it.  Both come from one text so that they cannot drift apart, and as
 // preprocessor text rather than a shared device function so that dw_bwd_kernel keeps exactly the
 // code it compiled to before the SE variant existed (a function boundary changes its register
-// allocation).  No include guard: meant to be included more than once.
+// allocation).  depthwise_grouped.cu includes it a third time, with YAMB_DW_GROUPED 1, as the
+// device function dw_bwd_body(p, vbid, vnblk) that one CTA of a grouped launch runs as CTA vbid of
+// a grid of vnblk (YAMB_DW_BID / YAMB_DW_NBLK / YAMB_DW_ARRIVE_LAST, see depthwise.cuh).  No
+// include guard: meant to be included more than once.
 template <int K, int S, int CT, int TAP0, int TAP1, bool DGRAD>
-#if YAMB_DW_BWD_SE
+#if YAMB_DW_GROUPED
+__device__ __forceinline__ void dw_bwd_body(const DwBwdDev& p, const unsigned vbid,
+                                            const unsigned vnblk) {
+#elif YAMB_DW_BWD_SE
 __global__ void __launch_bounds__(256, (K == 3 ? kDw3MinBlocks : 1)) dw_bwd_se_kernel(
     const __grid_constant__ DwBwdSeDev pse) {
   const DwBwdDev& p = pse.dw;
@@ -83,7 +89,7 @@ __global__ void __launch_bounds__(256, (K == 3 ? kDw3MinBlocks : 1)) dw_bwd_kern
     for (int i = tid; i < KK * CT; i += 256) {
       const int tp = i / CT, c = cbase + i % CT;
       const float g = s_gw[i];
-      if (c < p.C && g != 0.f) p.part[((size_t)blockIdx.x * p.C + c) * KK + tp] = g;   // once per CTA
+      if (c < p.C && g != 0.f) p.part[((size_t)YAMB_DW_BID * p.C + c) * KK + tp] = g;   // once per CTA
       s_gw[i] = 0.f;
     }
     if (DGRAD && p.has_bn && tid < 2 * CT) {
@@ -184,8 +190,8 @@ __global__ void __launch_bounds__(256, (K == 3 ? kDw3MinBlocks : 1)) dw_bwd_kern
   };
 
   // contiguous tile range per CTA (halo reuse in L2, see the forward kernel)
-  const unsigned t_end = (unsigned)(((unsigned long long)(blockIdx.x + 1) * p.num_tiles) / gridDim.x);
-  unsigned t = (unsigned)(((unsigned long long)blockIdx.x * p.num_tiles) / gridDim.x);
+  const unsigned t_end = (unsigned)(((unsigned long long)(YAMB_DW_BID + 1) * p.num_tiles) / YAMB_DW_NBLK);
+  unsigned t = (unsigned)(((unsigned long long)YAMB_DW_BID * p.num_tiles) / YAMB_DW_NBLK);
   Coord cur = decode(t);
   uint32_t mask_next = 0;
   __syncthreads();
@@ -348,7 +354,7 @@ __global__ void __launch_bounds__(256, (K == 3 ? kDw3MinBlocks : 1)) dw_bwd_kern
   cp_async_wait<0>();
   if (cur_chunk >= 0) flush(cur_chunk);
   if (p.has_bn && DGRAD) {
-    if (arrive_last(p.bn.counter)) {
+    if (YAMB_DW_ARRIVE_LAST(p.bn.counter)) {
       bn_bwd_finalize(p.bn, p.C);
       __syncthreads();
       if (threadIdx.x == 0) *p.bn.counter = 0;

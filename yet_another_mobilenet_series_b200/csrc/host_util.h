@@ -32,6 +32,9 @@ int expand_bwd_launch(const yamb_expand_bwd_args* a, cudaStream_t stream);
 int expand_bwd_plan_query(const yamb_expand_bwd_args* a, int num_sms, yamb_expand_bwd_plan_info* out);
 int dw_fwd_launch(const yamb_dw_fwd* a, cudaStream_t stream);
 int dw_bwd_launch(const yamb_dw_bwd* a, cudaStream_t stream);
+int dw_fwd_grouped_launch(const yamb_dw_fwd_grouped* a, cudaStream_t stream);
+int dw_bwd_grouped_launch(const yamb_dw_bwd_grouped* a, cudaStream_t stream);
+int dw_grouped_grids(yamb_dw_fwd_grouped* fwd, yamb_dw_bwd_grouped* bwd);
 int bn_apply_launch(const yamb_bn_apply* a, cudaStream_t stream);
 int bn_reduce_launch(const yamb_bn_reduce* a, cudaStream_t stream);
 int bn_stats_launch(const yamb_bn_stats* a, cudaStream_t stream);

@@ -127,6 +127,10 @@ class Workspace:
         # 2 * max_c doubles, kept in a float32 tensor
         self.partials = torch.zeros(4 * self.max_c, device=device, dtype=torch.float32)
         self.counter = torch.zeros(4, device=device, dtype=torch.int32)
+        # slots 1 .. nat.DW_MAX_BRANCHES - 1: the branches of a grouped depthwise launch run at the
+        # same time, each with its own accumulator (and counter[slot])
+        self.branch_partials = torch.zeros((nat.DW_MAX_BRANCHES - 1) * 4 * self.max_c,
+                                           device=device, dtype=torch.float32)
         self._se_sums = None
         self._se_sums_old = []
 
@@ -141,12 +145,16 @@ class Workspace:
             self._se_sums = torch.empty(n, device=self.partials.device, dtype=torch.float64)
         return self._se_sums
 
-    def stats(self, C):
-        """(partials, counter) device pointers for a statistics kernel over C channels."""
+    def stats(self, C, slot=0):
+        """(partials, counter) device pointers for a statistics kernel over C channels; `slot` > 0:
+        those of branch `slot` of a grouped depthwise launch."""
         if C > self.max_c:
             raise nat.NativeError("BatchNorm of %d channels: the statistics accumulator holds %d"
                                   % (C, self.max_c))
-        return self.partials.data_ptr(), self.counter.data_ptr()
+        if slot == 0:
+            return self.partials.data_ptr(), self.counter.data_ptr()
+        return (self.branch_partials.data_ptr() + (slot - 1) * 4 * self.max_c * 4,
+                self.counter.data_ptr() + 4 * slot)
 
     @classmethod
     def get(cls, device):
@@ -333,14 +341,15 @@ class _Bn:
                 return i, 0
         raise nat.NativeError("BatchNorm slice does not match a reference module")
 
-    def fwd_struct(self, count, c0=0, C=None):
+    def fwd_struct(self, count, c0=0, C=None, slot=0):
         """yamb_bn_fwd of channels [c0, c0+C) (all by default) over `count` rows, with the
-        statistics workspace of the current stream: build it right before its launch."""
+        statistics workspace of the current stream (its `slot`, see Workspace.stats): build it
+        right before its launch."""
         C = self.C if C is None else C
         i, off = self._module(c0, C)
         m = self.mods[i]
         s = nat.BnFwd()
-        s.partials, s.counter = Workspace.get(self.dev).stats(C)
+        s.partials, s.counter = Workspace.get(self.dev).stats(C, slot)
         s.gamma, s.beta = _at(m.weight, off), _at(m.bias, off)
         s.eps, s.momentum = self.eps, self.momentum_value()
         if m.track_running_stats and m.running_mean is not None:
@@ -351,13 +360,13 @@ class _Bn:
         s.count = count
         return s
 
-    def bwd_struct(self, count, grads, c0=0, C=None):
+    def bwd_struct(self, count, grads, c0=0, C=None, slot=0):
         """yamb_bn_bwd of channels [c0, c0+C) (all by default) over `count` rows; grads: the
         (dgamma, dbeta) accumulation targets of every module.  Built like `fwd_struct`."""
         C = self.C if C is None else C
         i, off = self._module(c0, C)
         s = nat.BnBwd()
-        s.partials, s.counter = Workspace.get(self.dev).stats(C)
+        s.partials, s.counter = Workspace.get(self.dev).stats(C, slot)
         s.gamma = _at(self.mods[i].weight, off)
         s.mean, s.invstd = _at(self.mean, c0), _at(self.invstd, c0)
         dg, db = grads[i]
@@ -454,6 +463,12 @@ def _bn_bwd_apply(bn, dy, h, dh, tag, z=None):
 def _dw_fwd(conv, nhw, x, y, tag, pre=None, stats=None):
     """y = depthwise `conv` of x over N x H x W pixels (x read with y's pitch); pre = (scale,
     shift, act) is applied to x on load; `stats` takes y's BatchNorm statistics."""
+    d, nbytes, flops = _dw_fwd_args(conv, nhw, x, y, pre, stats)
+    launch(nat.lib().yamb_depthwise_fwd, d, tag, nbytes, flops)
+
+
+def _dw_fwd_args(conv, nhw, x, y, pre=None, stats=None):
+    """(yamb_dw_fwd, bytes, flops) of `_dw_fwd`."""
     k, s = conv.kernel_size[0], conv.stride[0]
     Cc = y.shape[1]
     d = nat.DwFwd()
@@ -465,7 +480,7 @@ def _dw_fwd(conv, nhw, x, y, tag, pre=None, stats=None):
     if stats is not None:
         d.bn = C.pointer(stats)
     m_in, m_out = N * H * W, N * ((H - 1) // s + 1) * ((W - 1) // s + 1)
-    launch(nat.lib().yamb_depthwise_fwd, d, tag, 2 * Cc * (m_in + m_out), 2 * m_out * Cc * k * k)
+    return d, 2 * Cc * (m_in + m_out), 2 * m_out * Cc * k * k
 
 
 def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, stats=None, se=None):
@@ -475,6 +490,19 @@ def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, sta
     pitch.  se = (gate, dpool, scale, shift, act) of a Squeeze-and-Excitation block: dz is then
     dY = d(a2*gate) and the kernel forms dz2 = (dY*gate + dpool)*act'(scale*h + shift) on load
     (yamb_depthwise_bwd_se)."""
+    d, nbytes, flops = _dw_bwd_args(conv, nhw, dz, h, coef, dw, x, dx, pre, residual, stats)
+    if se is None:
+        launch(nat.lib().yamb_depthwise_bwd, d, tag, nbytes, flops)
+        return
+    a = nat.DwBwdSe()
+    a.dw = d
+    a.gate, a.dpool, a.ldg = se[0].data_ptr(), se[1].data_ptr(), se[0].stride(0)
+    a.scale, a.shift, a.act = se[2].data_ptr(), se[3].data_ptr(), se[4]
+    launch(nat.lib().yamb_depthwise_bwd_se, a, tag + "_se", nbytes, flops)
+
+
+def _dw_bwd_args(conv, nhw, dz, h, coef, dw, x, dx, pre=None, residual=None, stats=None):
+    """(yamb_dw_bwd, bytes, flops) of `_dw_bwd` without `se`."""
     k, s = conv.kernel_size[0], conv.stride[0]
     Cc = dz.shape[1]
     d = nat.DwBwd()
@@ -489,16 +517,7 @@ def _dw_bwd(conv, nhw, dz, h, coef, dw, x, dx, tag, pre=None, residual=None, sta
     if stats is not None:
         d.bn = C.pointer(stats)
     m_in, m_out = N * H * W, N * ((H - 1) // s + 1) * ((W - 1) // s + 1)
-    if se is None:
-        launch(nat.lib().yamb_depthwise_bwd, d, tag, 4 * Cc * (m_in + m_out),
-               4 * m_out * Cc * k * k)
-        return
-    a = nat.DwBwdSe()
-    a.dw = d
-    a.gate, a.dpool, a.ldg = se[0].data_ptr(), se[1].data_ptr(), se[0].stride(0)
-    a.scale, a.shift, a.act = se[2].data_ptr(), se[3].data_ptr(), se[4]
-    launch(nat.lib().yamb_depthwise_bwd_se, a, tag + "_se", 4 * Cc * (m_in + m_out),
-           4 * m_out * Cc * k * k)
+    return d, 4 * Cc * (m_in + m_out), 4 * m_out * Cc * k * k
 
 
 def _se_fc(se, pooled, u, v, gate, packed=None):
@@ -732,6 +751,7 @@ class BlockPlan:
             self.dpool = _f32(N * Chid, dev).view(N, Chid)
         self.conv_dw = [conv for conv, _ in parts.dws]
         self.expand_dw_kind = expand_dw_kind(block, H, W)
+        self.mb_dw_kind = mb_dw_kind(block, H, W)
         self.bn1 = _Bn(parts.bn1s, dev) if self.expand else None
         self.bn2 = _Bn([bn for _, bn in parts.dws], dev)
         self.bn3 = _Bn([parts.bn3], dev)
@@ -820,7 +840,8 @@ class BlockPlan:
         #    expanded tile recomputed from x instead of reading h1 back, where the kernel covers it
         if not self.bn2.batch_stats:
             self.bn2.eval_coeffs()
-        if not (expand_dw_fused(self) and self._expand_dw_train(xm)):
+        if not (expand_dw_fused(self) and self._expand_dw_train(xm)) and \
+                not (mb_dw_grouped(self) and self._dw_fwd_grouped()):
             for (c0, cb), conv in zip(self.bn2.slices, self.conv_dw):
                 s = slice(c0, c0 + cb)
                 _dw_fwd(conv, (self.N, self.H, self.W), self.h1[:, s] if self.expand else xm,
@@ -887,6 +908,61 @@ class BlockPlan:
                           2 * self.Chid * (self.M_in * self.Cin + self.M_out * k * k)):
             return False
         TRAIN_EXPAND_DW_CALLS += 1
+        return True
+
+    def _dw_fwd_grouped(self):
+        """Step 2 of TRAIN_MB_DW_GROUPED: every branch's depthwise in one
+        yamb_depthwise_fwd_grouped launch, branch b with statistics slot b; False, with nothing
+        enqueued, when the launcher declines (the caller then runs one dw_fwd per branch)."""
+        global TRAIN_MB_DW_GROUPED_CALLS
+        a = nat.DwFwdGrouped()
+        a.nbranch = len(self.conv_dw)
+        keep, nbytes, flops = [], 0, 0
+        for b, ((c0, cb), conv) in enumerate(zip(self.bn2.slices, self.conv_dw)):
+            s = slice(c0, c0 + cb)
+            stats = self.bn2.fwd_struct(self.M_out, c0, cb, slot=b) if self.bn2.batch_stats \
+                else None
+            keep.append(stats)
+            d, nb, fl = _dw_fwd_args(conv, (self.N, self.H, self.W), self.h1[:, s], self.h2[:, s],
+                                     (self.bn1.scale[s], self.bn1.shift[s], self.act), stats)
+            a.branch[b] = d
+            nbytes, flops = nbytes + nb, flops + fl
+        lib = nat.lib()
+        rc = lib.yamb_depthwise_grouped_grids(C.byref(a), None)
+        if rc == nat.EINVAL:
+            return False
+        nat.check(rc)
+        if not try_launch(lib.yamb_depthwise_fwd_grouped, a, "dw_fwd_grouped", nbytes, flops):
+            return False
+        TRAIN_MB_DW_GROUPED_CALLS += 1
+        return True
+
+    def _dw_bwd_grouped(self, grads):
+        """Step 4 of TRAIN_MB_DW_GROUPED: every branch's depthwise backward in one
+        yamb_depthwise_bwd_grouped launch, branch b with statistics slot b; False, with nothing
+        enqueued, when the launcher declines (the caller then runs one dw_bwd per branch)."""
+        global TRAIN_MB_DW_GROUPED_CALLS
+        a = nat.DwBwdGrouped()
+        a.nbranch = len(self.conv_dw)
+        keep, nbytes, flops = [], 0, 0
+        for b, ((c0, cb), conv, dw) in enumerate(zip(self.bn2.slices, self.conv_dw, grads["dw"])):
+            s = slice(c0, c0 + cb)
+            stats = self.bn1.bwd_struct(self.M_in, grads["bn1"], c0, cb, slot=b)
+            keep.append(stats)
+            d, nb, fl = _dw_bwd_args(conv, (self.N, self.H, self.W), self.dz2[:, s], self.h2[:, s],
+                                     (self.bn2.ca[s], self.bn2.cb[s], self.bn2.cc[s]), dw,
+                                     self.h1[:, s], self.dz1[:, s],
+                                     (self.bn1.scale[s], self.bn1.shift[s], self.act), None, stats)
+            a.branch[b] = d
+            nbytes, flops = nbytes + nb, flops + fl
+        lib = nat.lib()
+        rc = lib.yamb_depthwise_grouped_grids(None, C.byref(a))
+        if rc == nat.EINVAL:
+            return False
+        nat.check(rc)
+        if not try_launch(lib.yamb_depthwise_bwd_grouped, a, "dw_bwd_grouped", nbytes, flops):
+            return False
+        TRAIN_MB_DW_GROUPED_CALLS += 1
         return True
 
     def _se_backward(self, grads):
@@ -1028,8 +1104,10 @@ class BlockPlan:
         self._call_side(lib.yamb_pointwise_gemm, g, "pw_project_wgrad",
                         2 * self.M_out * (self.Cout + self.Chid),
                         2 * self.M_out * self.Chid * self.Cout, fork_ev, (self.dh3,))
-        # 4. depthwise backward per branch
-        for (c0, cb), conv, dw in zip(self.bn2.slices, self.conv_dw, grads["dw"]):
+        # 4. depthwise backward per branch, or of all branches in one launch (TRAIN_MB_DW_GROUPED)
+        grouped = mb_dw_grouped(self) and not se_fused and self._dw_bwd_grouped(grads)
+        for (c0, cb), conv, dw in [] if grouped else zip(self.bn2.slices, self.conv_dw,
+                                                           grads["dw"]):
             s = slice(c0, c0 + cb)
             coef = (self.bn2.ca[s], self.bn2.cb[s], self.bn2.cc[s])
             se_args = (self.gate[:, s], self.dpool[:, s], self.bn2.scale[s], self.bn2.shift[s],
@@ -1582,6 +1660,62 @@ def expand_dw_fused(plan):
     return (TRAIN_EXPAND_DW_FUSED and plan.expand and len(plan.conv_dw) == 1
             and plan.bn1.batch_stats and plan.bn2.batch_stats
             and _expand_dw_rule(plan.expand_dw_kind))
+
+
+# ---- training mode: the depthwise of every branch in one launch each way ---------------------------
+# Off by default.  When True (trainer.TrainStep(grouped_branches=True) turns it on for its own
+# forwards and backwards) step 2 of BlockPlan.forward and step 4 of BlockPlan.backward of a
+# training block with expansion and two or more branches launch yamb_depthwise_fwd_grouped /
+# _bwd_grouped once instead of dw_fwd / dw_bwd once per branch.  Each CTA of the grouped grid runs
+# what one CTA of a per-branch launch runs, so every output keeps its bits.  Only kinds
+# MB_DW_SHAPE_RULE accepts take the path (none by default, see there).  Single-branch blocks,
+# blocks without expansion, the backward with TRAIN_SE_FUSED (depthwise_bwd_se is not grouped) and
+# arguments the launcher declines run the per-branch launches.
+TRAIN_MB_DW_GROUPED = False
+TRAIN_MB_DW_GROUPED_CALLS = 0    # grouped depthwise launches, forward and backward (tests)
+# MB_DW_SHAPE_RULE groups a block only when its kind (mb_dw_kind) is in MB_DW_FASTER: the kinds
+# whose grouped launches measured faster than the per-branch ones.  Empty: on an H100 most kinds
+# of AtomNAS-C / C+ measured slower grouped and none faster in a way that survives run-to-run noise,
+# and whole steps were 4-6 % slower (tests/gpu_mb_dw_grouped_bench.py; BASELINE.md §5).  False:
+# every multi-branch block.
+MB_DW_SHAPE_RULE = True
+MB_DW_FASTER = frozenset()
+
+
+def mb_dw_kind(block, H, W):
+    """(kernel sizes, stride, H, W, Cin, hidden widths as run, padded to multiples of 8) of a
+    block with an expansion and two or more branches, the key of MB_DW_SHAPE_RULE; None for a
+    block that keeps its per-branch launches."""
+    parts = block_parts(block)
+    if not parts.expand_convs or len(parts.dws) < 2:
+        return None
+    return (tuple(conv.kernel_size[0] for conv, _ in parts.dws), parts.dws[0][0].stride[0], H, W,
+            parts.expand_convs[0].in_channels, tuple(_ceil8(conv.out_channels)
+                                                     for conv, _ in parts.dws))
+
+
+def mb_dw_grouped(plan):
+    """Whether step 2 / step 4 of `plan` (a BlockPlan) tries the grouped depthwise launch."""
+    return (TRAIN_MB_DW_GROUPED and plan.expand and len(plan.conv_dw) >= 2
+            and (not MB_DW_SHAPE_RULE or plan.mb_dw_kind in MB_DW_FASTER))
+
+
+def mb_dw_group_plan(block, N, H, W):
+    """The grouping of a training `block` on N x H x W inputs, as BlockPlan launches it: None when
+    the block keeps its per-branch launches (one branch, no expansion), else a list with one dict
+    per branch in launch order (the hidden tensor's channel order): its channel slice `c0`, `C`
+    (BatchNorm-2 forward and BatchNorm-1 backward statistics of that slice, in statistics slot
+    `slot`), `k` and `stride`."""
+    parts = block_parts(block)
+    if not parts.expand_convs or len(parts.dws) < 2:
+        return None
+    out, c0 = [], 0
+    for b, (conv, _) in enumerate(parts.dws):
+        cb = _ceil8(conv.out_channels)    # odd widths run as the padded shadow (_PadShadow)
+        out.append({"slot": b, "c0": c0, "C": cb, "k": conv.kernel_size[0],
+                    "stride": conv.stride[0]})
+        c0 += cb
+    return out
 
 
 def _se_fused(se):

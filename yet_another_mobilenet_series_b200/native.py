@@ -96,6 +96,23 @@ class DwBwd(C.Structure):
     ]
 
 
+DW_MAX_BRANCHES = 3
+
+
+class DwFwdGrouped(C.Structure):
+    _fields_ = [
+        ("nbranch", C.c_int32), ("branch", DwFwd * DW_MAX_BRANCHES),
+        ("grid", C.c_int32 * DW_MAX_BRANCHES),
+    ]
+
+
+class DwBwdGrouped(C.Structure):
+    _fields_ = [
+        ("nbranch", C.c_int32), ("branch", DwBwd * DW_MAX_BRANCHES),
+        ("grid", C.c_int32 * DW_MAX_BRANCHES), ("grid_wgrad", C.c_int32 * DW_MAX_BRANCHES),
+    ]
+
+
 class BnApply(C.Structure):
     _fields_ = [
         ("M", C.c_int64), ("C", C.c_int32), ("ldh", C.c_int32), ("ldr", C.c_int32),
@@ -462,10 +479,11 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
             25: StemConvEval, 26: HeadPoolEval, 27: GemmPlanInfo, 28: StemConvU8,
             29: ExpandBwd, 30: ExpandBwdPlanInfo, 31: HeadPoolTrain, 32: HeadPoolTrainGrad,
             33: StemConvTrain, 34: StemConvTrainGrad, 35: BlockEvalMbPack, 36: BlockEvalMb,
-            37: SeBwdStats, 38: SeBnBwdFinalize, 39: DwBwdSe, 40: ExpandDwTrain}
+            37: SeBwdStats, 38: SeBnBwdFinalize, 39: DwBwdSe, 40: ExpandDwTrain,
+            41: DwFwdGrouped, 42: DwBwdGrouped}
 
 # every symbol include/yamb200.h declares
-SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_bn_apply_fwd",
+SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_depthwise_fwd_grouped", "yamb_depthwise_bwd_grouped", "yamb_depthwise_grouped_grids", "yamb_bn_apply_fwd",
            "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_se_bwd_stats_bwd", "yamb_se_bn_bwd_finalize", "yamb_depthwise_bwd_se", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_expand_dw_train_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
@@ -501,6 +519,9 @@ def lib():
                                            C.POINTER(ExpandBwdPlanInfo)]
         l.yamb_depthwise_fwd.argtypes = [C.POINTER(DwFwd), C.c_void_p]
         l.yamb_depthwise_bwd.argtypes = [C.POINTER(DwBwd), C.c_void_p]
+        l.yamb_depthwise_fwd_grouped.argtypes = [C.POINTER(DwFwdGrouped), C.c_void_p]
+        l.yamb_depthwise_bwd_grouped.argtypes = [C.POINTER(DwBwdGrouped), C.c_void_p]
+        l.yamb_depthwise_grouped_grids.argtypes = [C.POINTER(DwFwdGrouped), C.POINTER(DwBwdGrouped)]
         l.yamb_bn_apply_fwd.argtypes = [C.POINTER(BnApply), C.c_void_p]
         l.yamb_bn_reduce_bwd.argtypes = [C.POINTER(BnReduce), C.c_void_p]
         l.yamb_bn_stats_fwd.argtypes = [C.POINTER(BnStats), C.c_void_p]

@@ -86,7 +86,8 @@ class TrainStep:
                  ema_decay=0.9999, ema_base_batch=4096, use_graph=True, input_dtype=torch.bfloat16,
                  optimizer="rmsprop", nesterov=False, dampening=0.0, weight_decay_method="mnas",
                  input_norm=None, micro_batch=None, fused_tail=False, fused_stem=False,
-                 fused_multi_branch=False, fused_se=False, fused_expand_dw=False):
+                 fused_multi_branch=False, fused_se=False, fused_expand_dw=False,
+                 grouped_branches=False):
         """`alpha` and `eps` apply to RMSprop only; `nesterov` and `dampening` to SGD only;
         `momentum`, `weight_decay` (folded in by `weight_decay_method`) and the EMA to both.
         `input_norm` = (mean, std) of the uint8 batches of `input_dtype=torch.uint8` (required
@@ -134,6 +135,17 @@ class TrainStep:
         differ from the default in the last bits.  It combines with `fused_stem`, `fused_tail`,
         `fused_se` and `micro_batch`; a plain `model(x)` is not affected.
 
+        `grouped_branches=True` runs the depthwise of every branch of this step's multi-branch
+        blocks with an expansion (AtomNAS, the single-path supernet) as one launch each way
+        (engine.TRAIN_MB_DW_GROUPED) instead of one launch per branch: the grouped grid is the
+        concatenation of the per-branch grids and each CTA runs what its per-branch CTA runs, so a
+        step with it has the default's bits.  Only block kinds engine.MB_DW_SHAPE_RULE accepts are
+        grouped; none by default, because grouping measured slower on an H100 (BASELINE.md §5).
+        The backward of a block with Squeeze-and-Excitation
+        keeps its per-branch launches under `fused_se`.  It is not recorded in checkpoints, and it
+        combines with `micro_batch`, partial batches, `fused_stem`, `fused_tail`, `fused_se` and
+        `fused_expand_dw`; a plain `model(x)` is not affected.
+
         `fused_multi_branch=True` is handed to the EvalStep that `validate` builds (see there)."""
         self.world = udist.get_world_size_fallback()
         self.micro_batch, self.accum, self.lr, self.ema_decay, self.grad_scale = step_hyper(
@@ -150,6 +162,7 @@ class TrainStep:
         self.fused_stem = bool(fused_stem)
         self.fused_se = bool(fused_se)
         self.fused_expand_dw = bool(fused_expand_dw)
+        self.grouped_branches = bool(grouped_branches)
         self.fused_multi_branch = bool(fused_multi_branch)
         if optimizer == "rmsprop":
             self.opt = RMSprop(model.parameters(), lr=self.lr, alpha=alpha, momentum=momentum,
@@ -222,6 +235,7 @@ class TrainStep:
         engine.TRAIN_STEM_FUSED = self.fused_stem
         engine.TRAIN_SE_FUSED = self.fused_se
         engine.TRAIN_EXPAND_DW_FUSED = self.fused_expand_dw
+        engine.TRAIN_MB_DW_GROUPED = self.grouped_branches
         try:
             self._passes(self.x if x is None else x, self.t if t is None else t)
         finally:
@@ -229,6 +243,7 @@ class TrainStep:
             engine.TRAIN_STEM_FUSED = False
             engine.TRAIN_SE_FUSED = False
             engine.TRAIN_EXPAND_DW_FUSED = False
+            engine.TRAIN_MB_DW_GROUPED = False
 
     def _passes(self, x, t):
         n, b = x.shape[0], self.micro_batch
