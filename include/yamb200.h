@@ -774,8 +774,9 @@ typedef struct yamb_block_eval_mb_pack_args {
  * packed width, w_expand / w_dw / w_project / bn1 / bn2 the packed tensors, gate / pooled over Chid).
  * Hidden channels [group_c0[i], group_c0[i+1]) (the last group up to Chid) have kernel group_k[i];
  * group_k strictly decreasing from group_k[0] = kmax, group_c0 increasing multiples of 8 from 0.
- * No cluster split.  YAMB_EINVAL for what yamb_block_eval_fwd does not cover or bad groups
- * (nothing enqueued), YAMB_ENODEV without a device. */
+ * No cluster split (see yamb_block_eval_mb_cluster_fwd below).  YAMB_EINVAL for what
+ * yamb_block_eval_fwd does not cover or bad groups (nothing enqueued), YAMB_ENODEV without a
+ * device. */
 typedef struct yamb_block_eval_mb {
   yamb_block_eval base;
   int32_t ngroups;            /* 1..3 */
@@ -786,6 +787,19 @@ typedef struct yamb_block_eval_mb {
 int yamb_block_eval_mb_pack(const yamb_block_eval_mb_pack_args* args, yamb_stream_t stream);
 int yamb_block_eval_mb_fwd(const yamb_block_eval_mb* args, yamb_stream_t stream);
 int yamb_block_eval_mb_pool_fwd(const yamb_block_eval_mb* args, yamb_stream_t stream);
+
+/* The same two calls with the 64-channel slices of the packed hidden dimension of every output tile
+ * split over the `cluster` CTAs (2, 4 or 8) of a thread-block cluster, as yamb_block_eval_cluster_fwd
+ * splits a single-branch block: every slice runs the stencil of its own group whatever rank holds
+ * it, and the ranks add their fp32 project partials in rank order before BN3 (+x).  For small
+ * batches (AtomNAS at batch 1).  The same function as yamb_block_eval_mb_fwd with the sum over the
+ * slices associated differently (the same bits on every run); the pool pass writes the same values
+ * as yamb_block_eval_mb_pool_fwd.  YAMB_EINVAL for another cluster size, bad groups, a shape
+ * yamb_block_eval_mb_fwd does not cover, and a tile plan whose partials do not fit a CTA's shared
+ * memory (nothing enqueued: the caller runs the unsplit call); YAMB_ENODEV without a device. */
+int yamb_block_eval_mb_cluster_fwd(const yamb_block_eval_mb* args, int32_t cluster, yamb_stream_t stream);
+int yamb_block_eval_mb_cluster_pool_fwd(const yamb_block_eval_mb* args, int32_t cluster,
+                                        yamb_stream_t stream);
 
 /* ---- training-mode expand + depthwise forward, the expanded tile recomputed from x ---------------
  * Step 2 of a single-branch training block with expansion (reference models/mobilenet_base.py:

@@ -231,6 +231,12 @@ int yamb_block_eval_mb_fwd(const yamb_block_eval_mb* a, yamb_stream_t s) {
 int yamb_block_eval_mb_pool_fwd(const yamb_block_eval_mb* a, yamb_stream_t s) {
   return yamb::block_eval_mb_launch(a, true, YAMB_ST(s));
 }
+int yamb_block_eval_mb_cluster_fwd(const yamb_block_eval_mb* a, int32_t cluster, yamb_stream_t s) {
+  return yamb::block_eval_mb_cluster_launch(a, false, cluster, YAMB_ST(s));
+}
+int yamb_block_eval_mb_cluster_pool_fwd(const yamb_block_eval_mb* a, int32_t cluster, yamb_stream_t s) {
+  return yamb::block_eval_mb_cluster_launch(a, true, cluster, YAMB_ST(s));
+}
 int yamb_expand_dw_train_fwd(const yamb_expand_dw_train* a, yamb_stream_t s) {
   return yamb::expand_dw_train_launch(a, YAMB_ST(s));
 }

@@ -9,14 +9,9 @@
 // products with zero taps, and the centred window of a smaller-k slice is the same convolution as
 // the branch's own (padding (k - 1) / 2 for every k).  Padded channels have zero W1 rows and W3
 // columns and BatchNorms that map 0 to 0: they contribute nothing.
-#include "block_eval.cuh"
+#include "block_eval_mb.cuh"
 
 namespace yamb {
-
-template <int K_, int S_, int TOH_, int TOW_, int TI_, int CPT_>
-struct EvGeomMB : EvGeom<K_, S_, TOH_, TOW_, TI_, CPT_> {
-  static constexpr bool MB = true;
-};
 
 // ---- packing: one CTA per packed hidden channel ---------------------------------------------------
 struct MbPackDev {
@@ -101,23 +96,11 @@ int block_eval_mb_launch(const yamb_block_eval_mb* m, bool pool, cudaStream_t st
   if (!m) return set_error(YAMB_EINVAL, "null args");
   const yamb_block_eval* a = &m->base;
   if (max_ctas() <= 0) return set_error(YAMB_ENODEV, "no CUDA device");
-  if (a->kernel != 5 && a->kernel != 7)
-    return set_error(YAMB_EINVAL, "block_eval_mb: kmax in {5,7} (got %d)", a->kernel);
-  if (!a->w_expand) return set_error(YAMB_EINVAL, "block_eval_mb: built with expansion only");
-  if (m->ngroups < 1 || m->ngroups > 3 || m->group_k[0] != a->kernel || m->group_c0[0] != 0)
-    return set_error(YAMB_EINVAL, "block_eval_mb: 1 to 3 groups, the first of k = kmax from channel 0");
-  for (int i = 1; i < m->ngroups; ++i)
-    if ((m->group_k[i] != 3 && m->group_k[i] != 5) || m->group_k[i] >= m->group_k[i - 1] ||
-        m->group_c0[i] <= m->group_c0[i - 1] || m->group_c0[i] % 8 || m->group_c0[i] >= a->Chid)
-      return set_error(YAMB_EINVAL, "block_eval_mb: group %d: k decreasing, c0 increasing multiples of 8 < Chid", i);
-  BlockEvalDev p;
-  int rc = block_eval_setup(a, pool, 1, p);
+  int rc = block_eval_mb_check(m);
   if (rc) return rc;
-  p.ngroups = m->ngroups;
-  for (int i = 0; i < 3; ++i) {
-    p.gk[i] = i < m->ngroups ? m->group_k[i] : 0;
-    p.gc0[i] = i < m->ngroups ? m->group_c0[i] : 0;
-  }
+  BlockEvalDev p;
+  if ((rc = block_eval_setup(a, pool, 1, p))) return rc;
+  block_eval_mb_groups(m, p);
   // the tile plan of block_eval_launch_impl for (kmax, stride)
   const bool wide = p.Npad > 16 * kMaxProjChunks;
   auto tiles_of = [&](int toh, int tow, int ti) {

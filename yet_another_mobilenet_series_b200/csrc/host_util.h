@@ -70,6 +70,7 @@ int block_eval_cluster_launch(const yamb_block_eval* a, int cluster, cudaStream_
 int block_eval_cluster_pool_launch(const yamb_block_eval* a, int cluster, cudaStream_t stream);
 int block_eval_mb_pack_launch(const yamb_block_eval_mb_pack_args* a, cudaStream_t stream);
 int block_eval_mb_launch(const yamb_block_eval_mb* a, bool pool, cudaStream_t stream);
+int block_eval_mb_cluster_launch(const yamb_block_eval_mb* a, bool pool, int cluster, cudaStream_t stream);
 int expand_dw_train_launch(const yamb_expand_dw_train* a, cudaStream_t stream);
 int in_fwd_launch(const yamb_in_fwd* a, cudaStream_t stream);
 int in_bwd_launch(const yamb_in_bwd* a, cudaStream_t stream);

@@ -1886,8 +1886,9 @@ def eval_supported(block, x):
         return False
     if not parts.fused:
         return k == 3 or act in (0, 1, 2)     # k = 5 / 7: built with relu / relu6 only
-    if FUSED_CLASS_SHAPE_RULE and (k != 3 or not block.expand):
-        return False        # measured slower than the four-launch sequence (see above)
+    if FUSED_CLASS_SHAPE_RULE and (k != 3 or not block.expand) and \
+            not small_batch_listed(block, x.shape[0]):
+        return False        # measured slower than the four-launch sequence at N = 256 (see above)
     nl = parts.nl
     if nl is not None:
         c = int(nl.nl_c * cout)
@@ -1898,13 +1899,14 @@ def eval_supported(block, x):
 
 def _block_eval_launch(fn, fn_cluster, a, cluster, tag, nbytes, flops):
     """One block kernel launch, split over clusters of `cluster` CTAs when cluster > 1 and the
-    tile plan with the exchanged partials fits shared memory, else unsplit."""
+    tile plan with the exchanged partials fits shared memory, else unsplit.  True when split."""
     global EVAL_CLUSTER_CALLS
     if cluster > 1 and try_launch(lambda st, s: fn_cluster(st, cluster, s), a, tag + "_cluster",
                                   nbytes, flops):
         EVAL_CLUSTER_CALLS += 1
-        return
+        return True
     launch(fn, a, tag, nbytes, flops)
+    return False
 
 
 def eval_forward(block, x):
@@ -1982,6 +1984,54 @@ EVAL_MB_CALLS = 0        # blocks that went through yamb_block_eval_mb_fwd (test
 MB_SHAPE_RULE = True
 MB_FASTER = frozenset()
 
+# ---- small batches (trainer.EvalStep(small_batch=True) sets EVAL_SMALL_BATCH around its evaluation
+# forwards).  Both shape rules above were measured at N = 256, where the work is bandwidth-bound;
+# at N = 1 a block is one or a few tiles and the count of serial launches decides.  While the
+# switch is on:
+#   - eval_forward_mb splits the packed hidden slices of every tile over a thread-block cluster
+#     (yamb_block_eval_mb_cluster_fwd, the size from eval_cluster_size as in eval_forward);
+#   - a multi-branch block whose kind is listed in SMALL_BATCH_FASTER takes the multi-branch path
+#     at N <= the listed bound, whatever EVAL_MULTI_BRANCH / MB_SHAPE_RULE say;
+#   - a fused-class block FUSED_CLASS_SHAPE_RULE keeps on the four-launch sequence takes the
+#     one-launch path at N <= the bound of its kind.
+# Kinds (small_batch_kind): ("mb", K_MAX, stride, fused class) and ("fused", k, stride, expansion).
+# SMALL_BATCH_RULE = False: every kind at every N (tests, tests/gpu_eval_latency_bench_searched.py).
+# SMALL_BATCH_FASTER: tests/gpu_eval_latency_bench_searched.py --rule off on one H100 80GB HBM3
+# (700 W power limit), every block of the kind alone in a CUDA graph, summed per kind, at
+# N = 1, 2, 4, 8, 16, 64; a kind is listed up to the largest measured N at which it and every smaller
+# N were faster than the default in every config that has it (BASELINE.md §5, "Small-batch eval of
+# the searched networks").  At N = 1: AtomNAS-C (7, 1) 1.64 -> 0.64 ms over 16 blocks, AtomNAS-C+
+# (7, 1, SE) 2.06 -> 1.54 ms, AutoNL-L 5x5 stride 1 0.83 -> 0.63 ms.  The SE kinds lose from
+# N = 16 / 64 on, where their pool pass's recompute costs more than the launches it saves.
+EVAL_SMALL_BATCH = False
+EVAL_MB_CLUSTER_CALLS = 0   # multi-branch block kernel launches split over a cluster (tests)
+SMALL_BATCH_RULE = True
+SMALL_BATCH_FASTER = (      # ((kind, max N), ...)
+    (("mb", 5, 1, False), 64), (("mb", 7, 1, False), 64), (("mb", 7, 2, False), 64),
+    (("mb", 5, 1, True), 16), (("mb", 7, 1, True), 16), (("mb", 7, 2, True), 8),
+    (("fused", 3, 1, False), 4), (("fused", 5, 1, True), 64), (("fused", 5, 2, True), 64),
+)
+
+
+def small_batch_kind(block):
+    """What SMALL_BATCH_FASTER decides on: ("mb",) + mb_kind for a multi-branch block, else
+    ("fused", k, stride, expansion)."""
+    if len(block.channels) > 1:
+        return ("mb",) + mb_kind(block)
+    return ("fused", list(block.kernel_sizes)[0], block.stride, bool(block.expand))
+
+
+def small_batch_listed(block, N):
+    """True while EVAL_SMALL_BATCH is on for a block whose kind SMALL_BATCH_FASTER lists with a
+    bound >= N (any block when SMALL_BATCH_RULE is off)."""
+    if not EVAL_SMALL_BATCH:
+        return False
+    if not SMALL_BATCH_RULE:
+        return True
+    kind = small_batch_kind(block)
+    return any(k == kind and N <= n for k, n in SMALL_BATCH_FASTER)
+
+
 MbLayout = collections.namedtuple("MbLayout", "map Chid kmax groups")
 
 
@@ -2008,8 +2058,9 @@ def eval_mb_supported(block, x):
     no gradient wanted, 2 or 3 branches with the expansion and 3x3 / 5x5 / 7x7 depthwise kernels
     (K_MAX 5 or 7), stride 1 or 2, Cin <= 256 and Cout <= 320 multiples of 8, every BatchNorm
     normalising with running statistics and one eps, an activation the kernel has, no non-local
-    block, and a kind MB_SHAPE_RULE lets through."""
-    if not (EVAL_MULTI_BRANCH and EVAL_FUSED) or torch.is_grad_enabled():
+    block, and a kind MB_SHAPE_RULE lets through, or one small_batch_listed lets through while
+    EVAL_SMALL_BATCH is on."""
+    if not ((EVAL_MULTI_BRANCH or EVAL_SMALL_BATCH) and EVAL_FUSED) or torch.is_grad_enabled():
         return False
     ks, chans = list(block.kernel_sizes), list(block.channels)
     if not 2 <= len(ks) <= 3 or not block.expand or block.stride not in (1, 2):
@@ -2033,7 +2084,9 @@ def eval_mb_supported(block, x):
             act_code_of(parts.se.active_fn)
     except ValueError:
         return False
-    return not MB_SHAPE_RULE or mb_kind(block) in MB_FASTER
+    if small_batch_listed(block, x.shape[0]):
+        return True
+    return EVAL_MULTI_BRANCH and (not MB_SHAPE_RULE or mb_kind(block) in MB_FASTER)
 
 
 def _mb_state(block, dev, R):
@@ -2106,8 +2159,9 @@ def _mb_pack_args(block, parts, ms):
 def eval_forward_mb(block, x):
     """y = block(x) in eval mode for a multi-branch block; x channels_last bf16 on CUDA.  C-ABI
     calls: the packing kernel and the block kernel (2); with SE the pool pass and the gate FCs
-    between them (+2)."""
-    global EVAL_MB_CALLS
+    between them (+2).  While EVAL_SMALL_BATCH is on, the block kernel and the pool pass split
+    over a cluster as eval_forward's do."""
+    global EVAL_MB_CALLS, EVAL_MB_CLUSTER_CALLS
     dev = x.device
     N, Cin, H, W = x.shape
     parts = block_parts(block)
@@ -2146,17 +2200,24 @@ def eval_forward_mb(block, x):
     flops = 2 * Chid * N * (H * W * Cin + Ho * Wo * Cout) + \
         2 * N * Ho * Wo * sum(k * k * c for k, c in zip(block.kernel_sizes, block.channels))
     act_bytes = 2 * N * H * W * Cin * (2 if a.residual else 1)
+    cluster = 1
+    if EVAL_SMALL_BATCH:
+        cluster = EVAL_CLUSTER if EVAL_CLUSTER is not None else eval_cluster_size(
+            lay.kmax, stride, N, Ho, Wo, Chid, Cout, _sm_count(dev))
     if se is not None:
         pooled = torch.empty(N, Chid, device=dev, dtype=torch.float32)
         gate = torch.empty(N, Chid, device=dev, dtype=torch.float32)
         uv = torch.empty(2, N, R, device=dev, dtype=torch.float32)
         a.pooled = pooled.data_ptr()
-        launch(lib.yamb_block_eval_mb_pool_fwd, m, "block_eval_mb_pool", act_bytes + 4 * N * Chid,
-               flops)
+        if _block_eval_launch(lib.yamb_block_eval_mb_pool_fwd, lib.yamb_block_eval_mb_cluster_pool_fwd,
+                              m, cluster, "block_eval_mb_pool", act_bytes + 4 * N * Chid, flops):
+            EVAL_MB_CLUSTER_CALLS += 1
         _se_fc(se, pooled, uv[0], uv[1], gate, packed=ms["se"])
         a.pooled = None
         a.gate = gate.data_ptr()
-    launch(lib.yamb_block_eval_mb_fwd, m, "block_eval_mb", act_bytes + 2 * N * Ho * Wo * Cout, flops)
+    if _block_eval_launch(lib.yamb_block_eval_mb_fwd, lib.yamb_block_eval_mb_cluster_fwd, m, cluster,
+                          "block_eval_mb", act_bytes + 2 * N * Ho * Wo * Cout, flops):
+        EVAL_MB_CLUSTER_CALLS += 1
     EVAL_MB_CALLS += 1
     return y
 

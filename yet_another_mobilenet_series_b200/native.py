@@ -484,7 +484,7 @@ _STRUCTS = {0: BnFwd, 1: BnBwd, 2: Gemm, 3: DwFwd, 4: DwBwd, 5: BnApply, 6: BnRe
 
 # every symbol include/yamb200.h declares
 SYMBOLS = ["yamb_pointwise_gemm", "yamb_gemm_plan", "yamb_expand_bwd", "yamb_expand_bwd_plan", "yamb_depthwise_fwd", "yamb_depthwise_bwd", "yamb_depthwise_fwd_grouped", "yamb_depthwise_bwd_grouped", "yamb_depthwise_grouped_grids", "yamb_bn_apply_fwd",
-           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_se_bwd_stats_bwd", "yamb_se_bn_bwd_finalize", "yamb_depthwise_bwd_se", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_expand_dw_train_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
+           "yamb_bn_reduce_bwd", "yamb_bn_stats_fwd", "yamb_bn_bwd_apply_bwd", "yamb_se_pool_fwd", "yamb_se_bwd_reduce_bwd", "yamb_se_bwd_apply_bwd", "yamb_se_bwd_stats_bwd", "yamb_se_bn_bwd_finalize", "yamb_depthwise_bwd_se", "yamb_nl_gram_fwd", "yamb_nl_rowmat_fwd", "yamb_se_fc_fwd", "yamb_se_fc_bwd", "yamb_softmax_ce_fwd", "yamb_softmax_ce_bwd", "yamb_colsum_bf16", "yamb_stem_conv_fwd", "yamb_stem_conv_wgrad", "yamb_stem_conv_eval_fwd", "yamb_stem_conv_u8_fwd", "yamb_stem_conv_u8_wgrad", "yamb_stem_conv_u8_eval_fwd", "yamb_stem_conv_train_fwd", "yamb_stem_conv_train_wgrad", "yamb_head_pool_eval_fwd", "yamb_head_pool_train_fwd", "yamb_head_pool_train_bwd", "yamb_block_eval_fwd", "yamb_block_eval_pool_fwd", "yamb_block_eval_cluster_fwd", "yamb_block_eval_cluster_pool_fwd", "yamb_block_eval_mb_pack", "yamb_block_eval_mb_fwd", "yamb_block_eval_mb_pool_fwd", "yamb_block_eval_mb_cluster_fwd", "yamb_block_eval_mb_cluster_pool_fwd", "yamb_expand_dw_train_fwd", "yamb_instance_norm_fwd", "yamb_instance_norm_bwd", "yamb_rmsprop_step", "yamb_sgd_step", "yamb_ema_update",
            "yamb_cast_bf16", "yamb_max_ctas", "yamb_struct_size", "yamb_last_error",
            "yamb_version"]
 _lib = None
@@ -557,6 +557,8 @@ def lib():
         l.yamb_block_eval_mb_pack.argtypes = [C.POINTER(BlockEvalMbPack), C.c_void_p]
         for fn in (l.yamb_block_eval_mb_fwd, l.yamb_block_eval_mb_pool_fwd):
             fn.argtypes = [C.POINTER(BlockEvalMb), C.c_void_p]
+        for fn in (l.yamb_block_eval_mb_cluster_fwd, l.yamb_block_eval_mb_cluster_pool_fwd):
+            fn.argtypes = [C.POINTER(BlockEvalMb), C.c_int32, C.c_void_p]
         l.yamb_expand_dw_train_fwd.argtypes = [C.POINTER(ExpandDwTrain), C.c_void_p]
         l.yamb_instance_norm_fwd.argtypes = [C.POINTER(InFwd), C.c_void_p]
         l.yamb_instance_norm_bwd.argtypes = [C.POINTER(InBwd), C.c_void_p]

@@ -527,13 +527,19 @@ class EvalStep:
 
     def __init__(self, model, per_gpu_batch, image_size=224, calib_batch=None, use_graph=True,
                  input_dtype=torch.bfloat16, optimizer=None, input_norm=None,
-                 fused_multi_branch=False):
+                 fused_multi_branch=False, small_batch=False):
         """`fused_multi_branch=True` runs the multi-branch blocks (several depthwise kernel sizes:
         AtomNAS) of the evaluation forwards as one packing launch and one block kernel each
         (engine.EVAL_MULTI_BRANCH) where engine.eval_mb_supported covers them.  Off by default: the
         hidden channels are regrouped by kernel size, so the project sums in another order and
         the logits differ from the default in the last bits (the same bits on every run).  A plain
-        `model(x)` outside the step is not affected."""
+        `model(x)` outside the step is not affected.
+
+        `small_batch=True` (engine.EVAL_SMALL_BATCH) is for evaluation at a few images per batch
+        (the searched networks at batch 1): multi-branch blocks split their hidden channels over a
+        thread-block cluster, and the block kinds engine.SMALL_BATCH_FASTER lists run as one
+        launch at batch sizes up to their measured bound.  Off by default, for the same reason;
+        calibration and a plain `model(x)` are not affected."""
         _attach_input_norm(model, input_dtype, input_norm)
         dev = next(model.parameters()).device
         if dev.type != "cuda":
@@ -544,6 +550,7 @@ class EvalStep:
         self.optimizer = optimizer
         self.use_graph = use_graph
         self.fused_multi_branch = bool(fused_multi_branch)
+        self.small_batch = bool(small_batch)
         self.phases = {"eval": _Phase(per_gpu_batch, image_size, input_dtype, dev),
                        "calib": _Phase(calib_batch or per_gpu_batch, image_size, input_dtype, dev)}
         self.loss_sum = torch.zeros((), device=dev, dtype=torch.float64)
@@ -579,11 +586,13 @@ class EvalStep:
     def _eval_body(self, x, t):
         engine.EVAL_TAIL_FUSED = True
         engine.EVAL_MULTI_BRANCH = self.fused_multi_branch
+        engine.EVAL_SMALL_BATCH = self.small_batch
         try:
             logits = self.model(x)
         finally:
             engine.EVAL_TAIL_FUSED = False
             engine.EVAL_MULTI_BRANCH = False
+            engine.EVAL_SMALL_BATCH = False
         loss, c1, c5 = tail_ops.softmax_ce(logits, t.to(self.dev), 0.0)
         self.loss_sum.add_(loss.double().sum())
         self.counts[0].add_(c1.sum().long())
